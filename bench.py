@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- EPro-PnP hot path on B200.
+"""bench.py -- EPro-PnP hot path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config fused|lm_only|amis|dense|train]   # our arm
+                    [--dump-outputs DIR]
     python bench.py --impl reference [--gpus N] [--steps K] [--config ...]                          # CPU arm
 
 Default = the headline metric: PnP objects/sec at (B = 4096 per GPU, N = 512, M = 512), BASELINE.json configs #3 / #5's
@@ -18,10 +19,15 @@ BASELINE.json's #2 (LM only, B = 1024), #3 (B = 1024), #4 (dense 64 x 64 coordin
              launch time (CUDA events around that kernel alone, measured in this run) against MEASURED_PEAKS.json.
              The path is FP32-pipe bound, not HBM bound (DESIGN.md section 4): `issue` reports the kernel's executed
              warp-instructions (profiles/kernel_stats.json, from the committed ncu capture of the SAME SASS -- refused
-             when the kernel's SASS fingerprint has changed since) per second against 148 SM x 4 schedulers x clock.
+             when the kernel's SASS fingerprint has changed since) per second against the device's SMs x 4 schedulers
+             x clock.
   cpu_baseline   the UNMODIFIED reference layer (oracle/_ref staged by oracle/stage_ref.py + oracle/pyro_shim) -- or the
              oracle port when it has not been staged -- on all host cores (one worker process per 4 cores, the objects
              are independent), bounded sample; rank 0, N = 1 only.
+  --dump-outputs DIR   after the timed steps, what the last timed step returned (rank 0's local results) as
+             DIR/<name>.npy, float32 (float64 where the result is float64).  Inputs, seeds and the step count fix the
+             outputs, so two builds run with the same arguments can be compared array by array.  Above 64 MB in all, every
+             array with one row per object keeps the same seeded sample of objects (rows in ascending object order).
 """
 import argparse
 import json
@@ -58,15 +64,15 @@ CONFIGS = {
 }
 E2E_CHUNKS = int(os.environ.get("EPNP_E2E_CHUNKS", "8"))   # object chunks of the host-buffer pipeline (0 = whole waves)
 # host-buffer calls in flight: consecutive steps rotate over this many (stream, workspace, pinned result set) triples, so
-# step i+1's upload runs under step i's solve and step i-1's download.  3 calls x 8 chunks was the configuration with the
-# smallest box-to-box spread (2.0 M objects/s on both boxes measured; profiles/r2_e2e_sweep*.txt -- the upload bandwidth
-# of pinned memory varies between 20 and 55 GB/s from box to box and size to size, which is what e2e mostly measures)
+# step i+1's upload runs under step i's solve and step i-1's download (the upload bandwidth of pinned memory is what e2e
+# mostly measures)
 E2E_LANES = max(1, int(os.environ.get("EPNP_E2E_LANES", "3")))
 WARM_SECONDS = 0.5            # minimum duration of back-to-back warm-up launches before the timed region
 # allocate the pinned host buffers while the thread is bound to the CPUs NVML reports as local to the GPU (first touch
 # puts the pages on the GPU's NUMA node; a remote node costs upload bandwidth)
 E2E_NUMA = os.environ.get("EPNP_E2E_NUMA", "1") == "1"
-L2_BYTES = 126e6
+L2_BYTES = 50e6               # H100 L2
+DUMP_BYTES = 64 << 20         # --dump-outputs: at most this much in all
 
 
 class gpu_local_cpus:
@@ -118,8 +124,8 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)", float(d.get("sm_max_mhz", 1965.0))
-    return 6650.0, "fallback (B200_PROFILING.md)", 1965.0
+        return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)", float(d.get("sm_max_mhz", 1980.0))
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)", 1980.0
 
 
 def kernel_stats(kernel, cfg_name):
@@ -280,7 +286,24 @@ def config_block(args, cfg, world):
     return {"workload": f"{cfg['what']}, B={Bg}/GPU, N={cfg['N']}, M={M}" + (", in-kernel Philox" if M else ""),
             "name": args.config, "global_batch": Bg * world, "parallelism": f"batch-split x{world}{gather}",
             "batches_in_flight": args.streams,
-            "l2": f"rotating {n_sets} input sets ({n_sets * set_bytes / 1e6:.0f} MB > 126 MB L2)"}
+            "l2": f"rotating {n_sets} input sets ({n_sets * set_bytes / 1e6:.0f} MB > {L2_BYTES / 1e6:.0f} MB L2)"}
+
+
+def dump_outputs(path, out, n_obj):
+    """--dump-outputs: every tensor of `out` as path/<name>.npy (float64 kept, anything else as float32).  When the total
+    exceeds DUMP_BYTES, the arrays with n_obj rows keep the rows of one fixed, seeded sample of objects."""
+    import numpy as np
+    arrays = {k: v.detach() for k, v in out.items() if torch.is_tensor(v)}
+    size = lambda v: v.numel() * (8 if v.dtype == torch.float64 else 4)
+    per_obj = sum(size(v) // n_obj for v in arrays.values() if v.dim() and v.shape[0] == n_obj)
+    fixed = sum(size(v) for v in arrays.values() if not (v.dim() and v.shape[0] == n_obj))
+    if fixed + per_obj * n_obj > DUMP_BYTES:
+        keep = (DUMP_BYTES - fixed) // per_obj
+        rows = torch.randperm(n_obj, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+        arrays = {k: v[rows.to(v.device)] if v.dim() and v.shape[0] == n_obj else v for k, v in arrays.items()}
+    os.makedirs(path, exist_ok=True)
+    for k, v in arrays.items():
+        np.save(os.path.join(path, k + ".npy"), v.cpu().to(torch.float64 if v.dtype == torch.float64 else torch.float32).numpy())
 
 
 def run_reference_arm(args, cfg, rank):
@@ -322,8 +345,10 @@ def main():
     ap.add_argument("--streams", type=int, default=2,
                     help="batches in flight: consecutive (independent) batches are issued round-robin on this many CUDA streams, "
                          "so the next batch's LM kernel and first AMIS CTAs fill the SMs the previous batch's last, partial wave "
-                         "of CTAs leaves idle (measured +4.4 %% at one GPU); 1 = strictly one batch at a time")
+                         "of CTAs leaves idle; 1 = strictly one batch at a time")
     ap.add_argument("--batch", type=int, default=0, help="objects per GPU (default: the config's)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (see the module docstring)")
     args = ap.parse_args()
     cfg = dict(CONFIGS[args.config])
     if args.batch > 0:
@@ -362,7 +387,7 @@ def main():
     gathering = world > 1 and kind == "lm_amis"
 
     # ---- synthetic inputs of this rank's shard (global object index keys the RNG, rank keys the data seed); enough
-    # rotating input sets that consecutive steps cannot be served from the 126 MB L2
+    # rotating input sets that consecutive steps cannot be served from the L2
     n_sets, set_bytes = rotating_sets(cfg)
     pc = make_problem(Bg, N_PTS, seed=1000 + rank, grid2d=cfg["grid2d"])
     sets = []
@@ -526,6 +551,8 @@ def main():
     wall1 = time.time()
     timing[0] = False
     total_ms = t_begin.elapsed_time(t_end)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out, Bg)
     clocks = sampler.stop(wall0, wall1) if rank == 0 else None
     # the solve's launches inside the loop (first 64 steps): their own duration, and the gap to the next step's launches
     in_loop = None
@@ -648,7 +675,8 @@ def main():
         issue = None
         if stats is not None:
             scale = Bg / float(stats["objects_per_launch"])
-            issue_peak = 148 * 4 * clk * 1e6                      # one warp-instruction per SM sub-partition per cycle
+            sms = torch.cuda.get_device_properties(dev).multi_processor_count
+            issue_peak = sms * 4 * clk * 1e6                      # one warp-instruction per SM sub-partition per cycle
             issue_rate = stats["warp_instr_per_launch"] * scale / (dom_ms * 1e-3)
             issue = {"bound": "warp-instruction issue / FP32 pipe (the binding resource, DESIGN.md section 4)",
                      "kernel": dom, "warp_instr_per_object": stats["warp_instr_per_launch"] / stats["objects_per_launch"],

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""The reference's usage demo (demo/fit_identity.ipynb, BASELINE.json config #1) on the B200-native layer:
+"""The reference's usage demo (demo/fit_identity.ipynb, BASELINE.json config #1) on the H100-native layer:
 an MLP maps a pose to 64 2D-3D correspondences + weights, EProPnP6DoF turns them back into a pose
 distribution, trained end to end with the Monte-Carlo pose loss and the derivative regularisation loss.
 Same calls as the notebook's cells 7-12; only `import epropnp` resolves to this repository.

@@ -3,11 +3,12 @@
 //
 //   * the object's correspondences are pulled from HBM once (TMA ring -> 64-byte pair records in shared memory);
 //   * one thread owns one sample of an iteration: draws it (injected noise or Philox), sweeps all N points with the
-//     pre-multiplied projection K[R|t] (points are shared-memory broadcasts, packed fp32x2 arithmetic), evaluates the
-//     proposal densities it needs; the mixture density of a sample is kept as ONE running log-sum-exp;
+//     pre-multiplied projection K[R|t] (points are shared-memory broadcasts, two points side by side in fp32x2
+//     register pairs), evaluates the proposal densities it needs; the mixture density of a sample is kept as ONE
+//     running log-sum-exp;
 //   * a log-weight is -cost - (lse - log count): it is recomputed where needed instead of stored, and the staging ring
 //     lives inside the (not yet written) sample buffer, so a CTA needs 36.1 KB at N = M = 512; five CTAs share an SM
-//     (96 registers per thread, no spills);
+//     (96 registers per thread);
 //   * the proposal refit is four block reductions (transposed butterflies) + a short chain on one lane.
 // The LM solution (pose, covariance) comes from global memory: lm_warp_kernel wrote it just before (same stream).
 //
@@ -20,8 +21,8 @@
 namespace {
 
 // Resident CTAs per SM the 128-thread kernel is compiled for.  Shared memory (36.1 KB at N = M = 512) would allow six at 80
-// registers, but then the sweep spills; measured on B200 after the serial phases had been trimmed: five CTAs at 96
-// registers (no spill) 0.933 ms per 4096 objects, six at 80 registers 0.951 ms (profiles/r2_split_probe.jsonl).
+// registers, but then the sweep spills.  Five at 96 registers against four at 128, H100 SXM at a 400 W power limit, median
+// of 8 alternating runs per 4096 objects: 1.363 vs 1.378 ms (B = 1024: 0.351 vs 0.350 ms), so five stay.
 constexpr int AMIS_CTAS_PER_SM = 5;
 
 template <int DOF> struct ProposalOf;
@@ -408,7 +409,7 @@ struct PushArgs {
 
 // The push epilogue of one object: its M log-weights (as this CTA wrote them to global memory) and its pose go to row
 // `row` of every peer's buffers.  Not inlined: it must not take part in the main body's register allocation (inlined,
-// the kernel ran 4 % slower for every caller, pushing or not: 0.972 vs 0.934 ms per 4096 objects).
+// it would weigh on every caller, pushing or not).
 template <int T>
 __device__ __noinline__ void push_rows(const float* src, const float* pose, size_t row, int M, int PD,
                                        float* const* peer_logw, float* const* peer_pose, int n) {
@@ -465,8 +466,8 @@ __global__ void __launch_bounds__(T, T == NT ? AMIS_CTAS_PER_SM : 1) amis_kernel
     else amis_phase4<T>(a, sh, pts4, dyn + pl.smp, dyn + pl.cost, dyn + pl.logp, dyn + pl.cpart, cam, delta, obj);
     // In-kernel gather (push.n > 0, uniform for the launch).  A run-time branch of ONE kernel, not a second instantiation:
     // a sharded run must be bit-identical to the single-GPU run, and two instantiations are two compilations -- as
-    // template variants the push / plain pair agreed bit for bit at N = 64, 512, 2052 but not on two small problems
-    // (N = 51, 130: log-weights 4e-6 apart after one step, profiles/r2_sanitizer_two_instantiations.txt).
+    // template variants the push / plain pair need not agree bit for bit, since each compilation allocates registers
+    // and orders the arithmetic on its own.
     if (push.n > 0) {
         __syncthreads();                                        // the CTA's own global stores are visible to all its threads
         push_rows<T>(a.logw + (size_t)obj * M, sh.pose, (size_t)a.obj_offset + (size_t)obj, M, PD, push.logw, push.pose, push.n);

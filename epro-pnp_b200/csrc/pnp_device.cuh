@@ -1,4 +1,4 @@
-// pnp_device.cuh -- device-side plumbing shared by the sm_100a kernels of the EPro-PnP hot path: launch / shared-memory
+// pnp_device.cuh -- device-side plumbing shared by the sm_90a kernels of the EPro-PnP hot path: launch / shared-memory
 // macros (which also let the file build under the test-only CPU SIMT emulator), mbarrier + 1-D TMA bulk-copy wrappers,
 // special-function functors, the kernel argument block, warp / block reductions, the packed point store with its TMA
 // loader, and the Huber cost sweep over the resident points.  Included by pnp_kernels.cu only.
@@ -340,10 +340,10 @@ template <int T = NT> __device__ __forceinline__ float block_max(float v, float*
 
 // ------------------------------------------------------------------------------------------------
 // Huber cost of one pose over every resident point: thread-private sweep, every lane reads the same pair record
-// (shared-memory broadcast, 4 x LDS.128 per 2 points) and evaluates two points per instruction with packed fp32x2
-// arithmetic (SASS FFMA2 / FMUL2).  P2[k] = (P[k], P[k]) is the pre-multiplied projection K[R|t] duplicated into both
+// (shared-memory broadcast, 4 x LDS.128 per 2 points) and evaluates two points side by side in fp32x2 pairs
+// (two scalar FFMA / FMUL per V2 op on sm_90a).  P2[k] = (P[k], P[k]) is the pre-multiplied projection K[R|t] duplicated into both
 // halves.  Per point pair: 17 packed FP ops + 4 MUFU (rcp, sqrt); Huber as m (s - m / 2), m = min(s, delta) -- both
-// branches in one expression, no select -- accumulated by its last FFMA2.  Same arithmetic per half as pnp::point_cost.
+// branches in one expression, no select -- accumulated by its last multiply-add.  Same arithmetic per half as pnp::point_cost.
 __device__ __forceinline__ float2 splat(float x) { return make_float2(x, x); }
 
 template <bool BOUNDED>
@@ -352,31 +352,31 @@ __device__ __forceinline__ float2 pair_cost(const float2 (&P2)[12], const Cam& c
     const float2 X = make_float2(q0.x, q0.y), Y = make_float2(q0.z, q0.w), Z = make_float2(q1.x, q1.y);
     const float2 nu = make_float2(q1.z, q1.w), nv = make_float2(q2.x, q2.y);
     const float2 wu = make_float2(q2.z, q2.w), wv = make_float2(q3.x, q3.y);
-    const float2 xh = __ffma2_rn(P2[0], X, __ffma2_rn(P2[1], Y, __ffma2_rn(P2[2], Z, P2[3])));
-    const float2 yh = __ffma2_rn(P2[4], X, __ffma2_rn(P2[5], Y, __ffma2_rn(P2[6], Z, P2[7])));
-    const float2 zh = __ffma2_rn(P2[8], X, __ffma2_rn(P2[9], Y, __ffma2_rn(P2[10], Z, P2[11])));
+    const float2 xh = v2fma(P2[0], X, v2fma(P2[1], Y, v2fma(P2[2], Z, P2[3])));
+    const float2 yh = v2fma(P2[4], X, v2fma(P2[5], Y, v2fma(P2[6], Z, P2[7])));
+    const float2 zh = v2fma(P2[8], X, v2fma(P2[9], Y, v2fma(P2[10], Z, P2[11])));
     const float2 iz = make_float2(FastRcp()(fmaxf(zh.x, cam.z_min)), FastRcp()(fmaxf(zh.y, cam.z_min)));
     float2 tx, ty;
     if (BOUNDED) {
-        float2 px = __fmul2_rn(xh, iz), py = __fmul2_rn(yh, iz);
+        float2 px = v2mul(xh, iz), py = v2mul(yh, iz);
         px.x = fminf(fmaxf(px.x, cam.lbx), cam.ubx); px.y = fminf(fmaxf(px.y, cam.lbx), cam.ubx);
         py.x = fminf(fmaxf(py.x, cam.lby), cam.uby); py.y = fminf(fmaxf(py.y, cam.lby), cam.uby);
-        tx = __fadd2_rn(px, nu); ty = __fadd2_rn(py, nv);
+        tx = v2add(px, nu); ty = v2add(py, nv);
     } else {
-        tx = __ffma2_rn(xh, iz, nu); ty = __ffma2_rn(yh, iz, nv);
+        tx = v2fma(xh, iz, nu); ty = v2fma(yh, iz, nv);
     }
-    const float2 rx = __fmul2_rn(tx, wu), ry = __fmul2_rn(ty, wv);
-    const float2 s2 = __ffma2_rn(rx, rx, __fmul2_rn(ry, ry));
+    const float2 rx = v2mul(tx, wu), ry = v2mul(ty, wv);
+    const float2 s2 = v2fma(rx, rx, v2mul(ry, ry));
     const float2 s = make_float2(FastSqrt()(s2.x), FastSqrt()(s2.y));
     const float2 m = make_float2(fminf(s.x, delta), fminf(s.y, delta));
-    return __ffma2_rn(m, __ffma2_rn(m, splat(-0.5f), s), acc);
+    return v2fma(m, v2fma(m, splat(-0.5f), s), acc);
 }
 
 // pair records [j0, j1)
 template <bool BOUNDED>
 __device__ __forceinline__ float sweep_cost(const float4* pts4, int j0, int j1, const float* P, const Cam& cam, float delta) {
-    // point pairs in flight per thread.  Measured with the resident CTAs per SM (AMIS kernel, ms per 4096 objects,
-    // profiles/r2_split_probe.jsonl): U=4 / 5 CTAs 0.933, U=6 / 5 0.943, U=3 / 6 0.955, U=4 / 4 0.990, U=8 / 4 1.003, U=2 / 5 1.023
+    // point pairs in flight per thread: enough independent chains to cover the FMA and MUFU latencies at five
+    // resident CTAs per SM without raising the register count past what those five CTAs allow
     constexpr int U = 4;
     float2 P2[12];
 #pragma unroll
@@ -397,7 +397,7 @@ __device__ __forceinline__ float sweep_cost(const float4* pts4, int j0, int j1, 
     }
     float2 t = c[0];
 #pragma unroll
-    for (int u = 1; u < U; ++u) t = __fadd2_rn(t, c[u]);
+    for (int u = 1; u < U; ++u) t = v2add(t, c[u]);
     return t.x + t.y;
 }
 

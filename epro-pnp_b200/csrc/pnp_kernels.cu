@@ -1,4 +1,4 @@
-// pnp_kernels.cu -- sm_100a kernels of the EPro-PnP hot path and their C ABI (include/epropnp_b200.h).
+// pnp_kernels.cu -- sm_90a kernels of the EPro-PnP hot path and their C ABI (include/epropnp_b200.h).
 //
 //   lm_warp_kernel (pnp_lm.cuh)      Levenberg-Marquardt / Gauss-Newton pose solve, ONE WARP per object: raw correspondences
 //                                    TMA-staged into the warp's shared memory, 16 points per lane, shuffle-only reduction,
@@ -94,16 +94,24 @@ __device__ __forceinline__ bool cheaper_hypothesis(float c, int h, float wc, int
 template <int DOF, bool CLIP>
 __device__ __forceinline__ void eval_subset(const float* pts, const int* idx, int n, const float* pose, const Cam& cam,
                                             float delta, float huber_eps, float* acc) {
-    constexpr int NV = Dim<DOF>::NV;
+    // the LM kernel's per-point arithmetic (row-packed, explicitly rounded): no contraction is left to the compiler
+    constexpr int NP = Dim<DOF>::NV - 1;
     float R[9];
     pose_to_rot<DOF>(pose, R);
+    V2 acc2[NP];
 #pragma unroll
-    for (int i = 0; i < NV; ++i) acc[i] = 0.f;
+    for (int i = 0; i < NP; ++i) acc2[i] = v2splat(0.f);
+    const V2 kuv[3] = {v2(cam.k[0], cam.k[3]), v2(cam.k[1], cam.k[4]), v2(cam.k[2], cam.k[5])};
+    float cost = 0.f;
     for (int i = 0; i < n; ++i) {
         const int j = __ldg(idx + i);
         const float* q = pts + (j >> 1) * 16 + (j & 1);
-        point_normal_eq<DOF, CLIP>(R, pose, cam, delta, huber_eps, q[0], q[2], q[4], -q[6], -q[8], q[10], q[12], acc);
+        point_normal_eq_rows<DOF, CLIP>(R, pose, cam, kuv, delta, huber_eps, q[0], q[2], q[4], q[6], q[8], q[10], q[12],
+                                        acc2, cost);
     }
+#pragma unroll
+    for (int i = 0; i < NP; ++i) acc[i] = acc2[i].x + acc2[i].y;
+    acc[NP] = cost;
 }
 
 template <int DOF>
@@ -489,43 +497,43 @@ template <bool BOUNDED>
 __device__ __forceinline__ void pair_cost_backward(const float (&P)[12], const Cam& cam, float delta, float gj,
                                                    float2 X, float2 Y, float2 Z, float2 nu, float2 nv, float2 wu,
                                                    float2 wv, float2 (&g)[7], float2& gd) {
-    const float2 xh = __ffma2_rn(splat(P[0]), X, __ffma2_rn(splat(P[1]), Y, __ffma2_rn(splat(P[2]), Z, splat(P[3]))));
-    const float2 yh = __ffma2_rn(splat(P[4]), X, __ffma2_rn(splat(P[5]), Y, __ffma2_rn(splat(P[6]), Z, splat(P[7]))));
-    const float2 zh = __ffma2_rn(splat(P[8]), X, __ffma2_rn(splat(P[9]), Y, __ffma2_rn(splat(P[10]), Z, splat(P[11]))));
+    const float2 xh = v2fma(splat(P[0]), X, v2fma(splat(P[1]), Y, v2fma(splat(P[2]), Z, splat(P[3]))));
+    const float2 yh = v2fma(splat(P[4]), X, v2fma(splat(P[5]), Y, v2fma(splat(P[6]), Z, splat(P[7]))));
+    const float2 zh = v2fma(splat(P[8]), X, v2fma(splat(P[9]), Y, v2fma(splat(P[10]), Z, splat(P[11]))));
     const float2 iz = make_float2(FastRcp()(fmaxf(zh.x, cam.z_min)), FastRcp()(fmaxf(zh.y, cam.z_min)));
-    const float2 px = __fmul2_rn(xh, iz), py = __fmul2_rn(yh, iz);
+    const float2 px = v2mul(xh, iz), py = v2mul(yh, iz);
     float2 pxc = px, pyc = py;
     if (BOUNDED) {
         pxc.x = fminf(fmaxf(px.x, cam.lbx), cam.ubx); pxc.y = fminf(fmaxf(px.y, cam.lbx), cam.ubx);
         pyc.x = fminf(fmaxf(py.x, cam.lby), cam.uby); pyc.y = fminf(fmaxf(py.y, cam.lby), cam.uby);
     }
-    const float2 ex = __fadd2_rn(pxc, nu), ey = __fadd2_rn(pyc, nv);
-    const float2 rx = __fmul2_rn(ex, wu), ry = __fmul2_rn(ey, wv);
-    const float2 s2 = __ffma2_rn(rx, rx, __fmul2_rn(ry, ry));
+    const float2 ex = v2add(pxc, nu), ey = v2add(pyc, nv);
+    const float2 rx = v2mul(ex, wu), ry = v2mul(ey, wv);
+    const float2 s2 = v2fma(rx, rx, v2mul(ry, ry));
     const float2 rs = make_float2(FastRsqrt()(fmaxf(s2.x, 1e-30f)), FastRsqrt()(fmaxf(s2.y, 1e-30f)));
-    const float2 s = __fmul2_rn(s2, rs);
+    const float2 s = v2mul(s2, rs);
     const bool in0 = s.x <= delta, in1 = s.y <= delta;
-    const float2 ko = __fmul2_rn(splat(gj * delta), rs);                 // outlier: g * delta / s
+    const float2 ko = v2mul(splat(gj * delta), rs);                 // outlier: g * delta / s
     const float2 k = make_float2(in0 ? gj : ko.x, in1 ? gj : ko.y);
-    const float2 grx = __fmul2_rn(k, rx), gry = __fmul2_rn(k, ry);
-    g[5] = __ffma2_rn(grx, ex, g[5]);
-    g[6] = __ffma2_rn(gry, ey, g[6]);
-    const float2 gex = __fmul2_rn(grx, wu), gey = __fmul2_rn(gry, wv);
-    g[3] = __ffma2_rn(gex, splat(-1.0f), g[3]);
-    g[4] = __ffma2_rn(gey, splat(-1.0f), g[4]);
+    const float2 grx = v2mul(k, rx), gry = v2mul(k, ry);
+    g[5] = v2fma(grx, ex, g[5]);
+    g[6] = v2fma(gry, ey, g[6]);
+    const float2 gex = v2mul(grx, wu), gey = v2mul(gry, wv);
+    g[3] = v2fma(gex, splat(-1.0f), g[3]);
+    g[4] = v2fma(gey, splat(-1.0f), g[4]);
     float2 gpx = gex, gpy = gey;
     if (BOUNDED) {
         gpx.x = (pxc.x == px.x) ? gex.x : 0.f; gpx.y = (pxc.y == px.y) ? gex.y : 0.f;
         gpy.x = (pyc.x == py.x) ? gey.x : 0.f; gpy.y = (pyc.y == py.y) ? gey.y : 0.f;
     }
-    const float2 gxh = __fmul2_rn(gpx, iz), gyh = __fmul2_rn(gpy, iz);
-    const float2 tz = __ffma2_rn(gxh, px, __fmul2_rn(gyh, py));
+    const float2 gxh = v2mul(gpx, iz), gyh = v2mul(gpy, iz);
+    const float2 tz = v2fma(gxh, px, v2mul(gyh, py));
     const float2 gzh = make_float2(zh.x >= cam.z_min ? -tz.x : 0.f, zh.y >= cam.z_min ? -tz.y : 0.f);
-    g[0] = __ffma2_rn(splat(P[0]), gxh, __ffma2_rn(splat(P[4]), gyh, __ffma2_rn(splat(P[8]), gzh, g[0])));
-    g[1] = __ffma2_rn(splat(P[1]), gxh, __ffma2_rn(splat(P[5]), gyh, __ffma2_rn(splat(P[9]), gzh, g[1])));
-    g[2] = __ffma2_rn(splat(P[2]), gxh, __ffma2_rn(splat(P[6]), gyh, __ffma2_rn(splat(P[10]), gzh, g[2])));
-    const float2 over = __fadd2_rn(s, splat(-delta));
-    gd = __ffma2_rn(make_float2(in0 ? 0.f : over.x, in1 ? 0.f : over.y), splat(gj), gd);
+    g[0] = v2fma(splat(P[0]), gxh, v2fma(splat(P[4]), gyh, v2fma(splat(P[8]), gzh, g[0])));
+    g[1] = v2fma(splat(P[1]), gxh, v2fma(splat(P[5]), gyh, v2fma(splat(P[9]), gzh, g[1])));
+    g[2] = v2fma(splat(P[2]), gxh, v2fma(splat(P[6]), gyh, v2fma(splat(P[10]), gzh, g[2])));
+    const float2 over = v2add(s, splat(-delta));
+    gd = v2fma(make_float2(in0 ? 0.f : over.x, in1 ? 0.f : over.y), splat(gj), gd);
 }
 
 struct BwArgs {
@@ -740,7 +748,7 @@ int device_sms(int* sms) {
 bool tma_ok(const KArgs& a) { return (a.N % 4 == 0) && aligned16(a.x3d) && aligned16(a.x2d) && aligned16(a.w2d); }
 
 // One CTA of NT threads per object (grid = B): the hardware scheduler hands CTAs to SMs as slots free up, the CTAs'
-// serial and parallel phases de-synchronise and there is no lock-step tail (measured 5 % faster than a persistent grid).
+// serial and parallel phases de-synchronise and there is no lock-step tail, as a persistent grid would have.
 template <int T = NT, class Kern, class... Extra>
 int launch_cta_per_object(Kern kern, KArgs& a, int smem_bytes, cudaStream_t stream, Extra... extra) {
     if (a.B == 0) return EPNP_OK;

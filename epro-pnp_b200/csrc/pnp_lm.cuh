@@ -4,8 +4,8 @@
 // Why one warp per object.  An LM iteration is: evaluate the 28 sums (21 J^T J + 6 J^T r + cost) over the N points at
 // the candidate pose, then a short serial chain (6x6 damped Cholesky solve, SE(3) retraction, trust-region update).
 // With a 128-thread CTA per object (round 1) each thread saw only N / 128 = 4 points between two block barriers and
-// 127 threads idled through the serial chain: the phase was latency-bound (0.31 ms of a 1.40 ms fused step, measured
-// with tools/split_probe.py).  With a warp per object a lane owns N / 32 = 16 points (long independent instruction
+// 127 threads idled through the serial chain: the phase was latency-bound (tools/split_probe.py times it).  With a
+// warp per object a lane owns N / 32 = 16 points (long independent instruction
 // streams), the reduction is 31 shuffles with no block barrier, the serial chain costs the same issue slots as before
 // but 12-14 other warps of the SM -- other OBJECTS -- fill the scheduler meanwhile.  No __syncthreads anywhere.
 //
@@ -23,8 +23,8 @@
 
 namespace {
 
-constexpr int LM_STAGE_MAX_N = 640;     // 28 N bytes of shared memory per warp: 17.9 KB -> 12 resident warps per SM.  Reading
-                                        // global memory instead was measured slower at N = 512 (0.203 vs 0.168 ms, 120 registers)
+constexpr int LM_STAGE_MAX_N = 640;     // 28 N bytes of shared memory per warp: 17.9 KB -> 12 resident warps per SM.  Below
+                                        // that the K + 1 evaluations read shared memory instead of going back to L1 / L2
 
 constexpr int LM_MAX_WARPS = 8;
 template <int DOF, int WARPS> struct LmHead {
@@ -46,8 +46,8 @@ template <int DOF, int WARPS> __host__ __device__ inline int lm_smem_bytes(int N
 }
 
 // Normal equations at `pose` over the object's N points by the object's WARPS warps: result in ev[0..NV) (visible to
-// every thread of the group on return).  Jacobian rows u / v in the two lanes of fp32x2 registers (27 FFMA2 per point
-// instead of 54 FFMA).
+// every thread of the group on return).  Jacobian rows u / v in the two lanes of fp32x2 registers (27 V2 multiply-adds
+// per point, two FFMA each on sm_90a).
 template <int DOF, bool CLIP, int WARPS>
 __device__ __forceinline__ void warp_normal_eq(const float* p3, const float* p2, const float* pw, int N, const float* pose,
                                                const Cam& cam, float delta, float huber_eps, float* ev, float* part) {

@@ -1,5 +1,5 @@
 """Drop-in replacement of the reference's `epropnp` package (same module and class names) whose
-batched hot loops run in hand-written sm_100a CUDA behind libepropnp_b200.so:
+batched hot loops run in hand-written sm_90a CUDA behind libepropnp_b200.so:
 
     epropnp.epropnp               EProPnP6DoF / EProPnP4DoF / EProPnPBase / cholesky_wrapper
     epropnp.levenberg_marquardt   LMSolver / RSLMSolver

@@ -152,7 +152,7 @@ class _PosePlus(torch.autograd.Function):
 
 
 def native_gn_step_enabled():
-    """pose_opt_plus is differentiated by the native kernel (epnp_gn_plus_backward_f32; validated on B200 against the
+    """pose_opt_plus is differentiated by the native kernel (epnp_gn_plus_backward_f32; validated on the GPU against the
     float64 composite and the reference's own autograd).  EPNP_NATIVE_GN_STEP=0 selects the torch-autograd composite of
     PerspectiveCamera.project + HuberPnPCost.compute instead (exact in float64; used by the CPU tests and for A/B timing)."""
     import os

@@ -1,5 +1,5 @@
 """EProPnP6DoF / EProPnP4DoF with the reference's constructor and call signatures
-(reference epropnp/epropnp.py), executing on the native sm_100a kernels.
+(reference epropnp/epropnp.py), executing on the native sm_90a kernels.
 
 `monte_carlo_forward` = one fused launch (epnp_lm_amis_fused_f32): the LM solve, its covariance, the
 first proposal, and all AMIS iterations (draw -> cost of every sample over all points -> mixture

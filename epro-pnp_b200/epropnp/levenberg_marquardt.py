@@ -1,5 +1,5 @@
 """LMSolver / RSLMSolver with the reference's constructor and call signatures
-(reference epropnp/levenberg_marquardt.py), executing on the native sm_100a kernels.
+(reference epropnp/levenberg_marquardt.py), executing on the native sm_90a kernels.
 
 What runs where:
   * the K-iteration Levenberg-Marquardt (or Gauss-Newton `fast_mode`) loop, the pose covariance and
@@ -217,12 +217,12 @@ class RSLMSolver(LMSolver):
         """-> pose (B, 4|7), None, min_cost (B).
 
         Two launches: the set-up (epnp_rslm_draw_f32: the centre-based translation guess and, per (proposal, object), a
-        weighted subset without replacement and a random start orientation -- torch.multinomial on the (P*B, N) weight
-        rows alone took 8 ms at B = 4096, profiles/r2_side_kernels.jsonl) and the solve (epnp_rslm_f32: one
+        weighted subset without replacement and a random start orientation, in place of torch.multinomial on the (P*B, N)
+        weight rows) and the solve (epnp_rslm_f32: one
         CTA per object, thread <-> hypothesis, LM / GN on the n sampled correspondences read from the object's resident
         pair records, scored on all N points, cheapest kept).  The reference's gather of (P*B, n, .) mini-problems, its
         P-fold repeated camera / cost objects and its P*B tiny solves do not exist; run on the same kernels that
-        formulation lost in all four measured configurations (profiles/r2_rslm_ab.jsonl) and was removed.
+        formulation measured slower and was removed.
         `rslm_seed=` fixes the Philox stream of the native draws."""
         bs, pn, _ = x2d.size()
         pd = self._pose_dim()

@@ -1,6 +1,6 @@
 """Builds the in-tree native artefacts.
 
-    libepropnp_b200.so   nvcc, sm_100a only (cross-compiles without a GPU)
+    libepropnp_b200.so   nvcc, sm_90a only (cross-compiles without a GPU)
     libhost_emul.so      g++ build of csrc/pnp_math.cuh + tests/host_emul.cpp (CPU tests only)
 
 The .so files stay in the tree (epro-pnp_b200/lib/, git-ignored) so they travel to the GPU box.
@@ -17,7 +17,7 @@ INCLUDE = os.path.join(REPO_ROOT, "include")
 LIB_PATH = os.path.join(LIB_DIR, "libepropnp_b200.so")
 EMUL_PATH = os.path.join(LIB_DIR, "libhost_emul.so")
 
-NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared", "-I", INCLUDE]
 
 # kept for the test-side build helpers (tests/simt_native.py): the shipped library has no build options

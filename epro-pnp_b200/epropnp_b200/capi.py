@@ -73,7 +73,7 @@ def lib():
         if not os.path.exists(_LIB_PATH):
             raise NativeError(
                 f"{_LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). There is no CPU / PyTorch fallback for the EPro-PnP hot path.")
+                "(nvcc, sm_90a). There is no CPU / PyTorch fallback for the EPro-PnP hot path.")
         handle = ctypes.CDLL(_LIB_PATH)
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(handle, name)

@@ -15,7 +15,7 @@ from .capi import NativeError, check, default_params, lib, ptr, stream_ptr
 def _need_cuda(t, what):
     if not t.is_cuda:
         raise NativeError(f"{what}: tensor is on {t.device}; the EPro-PnP hot path runs on CUDA only "
-                          "(no CPU / PyTorch fallback). Move the inputs to a B200 device.")
+                          "(no CPU / PyTorch fallback). Move the inputs to an H100 (sm_90) device.")
 
 
 def _f32c(t):

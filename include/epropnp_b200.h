@@ -1,5 +1,5 @@
 /* epropnp_b200.h -- C ABI of libepropnp_b200.so: the EPro-PnP hot path (batched LM / GN pose solve
- * and the AMIS Monte-Carlo loop) as hand-written sm_100a CUDA.
+ * and the AMIS Monte-Carlo loop) as hand-written sm_90a CUDA.
  *
  * The reference (tjiiv-cprg/EPro-PnP) has NO native interface for this path: it is ~10^3 PyTorch
  * op launches behind Python classes.  This header is therefore the FFI a maintainer would bind
@@ -39,7 +39,7 @@ enum {
     EPNP_ERR_TOO_MANY_POINTS = -2, /* N (and M) do not fit the 227 KB shared memory of one SM       */
     EPNP_ERR_UNSUPPORTED = -3,   /* combination not supported by this build                            */
     EPNP_ERR_CUDA = -4,          /* a CUDA runtime call failed, see epnp_last_cuda_error()             */
-    EPNP_ERR_NO_DEVICE = -5      /* no sm_100 device is current                                        */
+    EPNP_ERR_NO_DEVICE = -5      /* no sm_90 device is current                                         */
 };
 
 /* Hyper-parameters of the solve.  Defaults (epnp_default_params) are the reference's constructor
@@ -234,8 +234,8 @@ int epnp_mc_lse_backward_f32(const float* logw, const float* lse, const float* g
  * `stream`, in `n_chunks` object chunks through a copy-in / solve / copy-out pipeline (helper streams owned by
  * the calling host thread, created on first use -- the only resource the library keeps).  n_chunks = 0 cuts the
  * batch at whole waves of resident CTAs (SMs x CTAs per SM objects per chunk, as few waves per chunk as the limit of
- * 64 chunks allows); n_chunks >= 1 asks for that many equal chunks (8 for B = 4096, two calls in flight, is the measured
- * configuration).
+ * 64 chunks allows); n_chunks >= 1 asks for that many equal chunks (bench.py uses 8 for B = 4096, three calls in
+ * flight).
  * workspace: device memory of at least epnp_fused_workspace_bytes(B, N, p) bytes.
  * Outputs [opt] as above (pose_samples_host may be NULL to skip the largest copy).              */
 size_t epnp_fused_workspace_bytes(int B, int N, const EpnpParams* p);

@@ -1,4 +1,4 @@
-"""Shared fixtures.  `-m "not gpu"` runs here on CPU; `-m gpu` needs a B200 and goes through the C ABI."""
+"""Shared fixtures.  `-m "not gpu"` runs here on CPU; `-m gpu` needs an H100 and goes through the C ABI."""
 import glob
 import os
 import sys
@@ -17,7 +17,7 @@ GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: the kernels are built for sm_90a only)")
 
 
 def golden_names(prefix=""):

@@ -1,5 +1,5 @@
 // host_emul.cpp -- TEST-ONLY serial driver around epro-pnp_b200/csrc/pnp_math.cuh compiled with g++.
-// It lets the CPU test-suite (-m "not gpu") exercise the exact scalar code the sm_100a kernels inline
+// It lets the CPU test-suite (-m "not gpu") exercise the exact scalar code the sm_90a kernels inline
 // (per-point math, LM state machine, small Cholesky algebra, proposal draw/density, refit formulas)
 // against the golden vectors, without a GPU.  It is NOT a product path and is not shipped in the
 // library: the library has no CPU fallback.  The loops here mirror pnp_kernels.cu's control flow with

@@ -42,11 +42,6 @@ inline float4 make_float4(float x, float y, float z, float w) { return float4{x,
 struct uint3 { unsigned x, y, z; };
 struct dim3 { unsigned x = 1, y = 1, z = 1; dim3() {} dim3(unsigned a) : x(a) {} dim3(int a) : x((unsigned)a) {} };
 
-// packed fp32x2 intrinsics: both lanes with the fused scalar op
-inline float2 __ffma2_rn(float2 a, float2 b, float2 c) { return float2{fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)}; }
-inline float2 __fmul2_rn(float2 a, float2 b) { return float2{a.x * b.x, a.y * b.y}; }
-inline float2 __fadd2_rn(float2 a, float2 b) { return float2{a.x + b.x, a.y + b.y}; }
-
 namespace simt {
 
 constexpr int kMaxThreads = 1024;
@@ -294,7 +289,7 @@ enum cudaMemcpyKind { cudaMemcpyHostToDevice = 1, cudaMemcpyDeviceToHost = 2 };
 inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
 inline cudaError_t cudaDeviceGetAttribute(int* v, int, int) {          // SM count; SIMT_EMUL_SMS shrinks the "device"
     const char* e = std::getenv("SIMT_EMUL_SMS");
-    *v = (e && std::atoi(e) > 0) ? std::atoi(e) : 148;
+    *v = (e && std::atoi(e) > 0) ? std::atoi(e) : 132;
     return cudaSuccess;
 }
 template <class F> inline cudaError_t cudaFuncSetAttribute(F, int, int) { return cudaSuccess; }

@@ -1,21 +1,22 @@
 """Drop-in check by introspection: every public function, class, method and static method of the six reference modules
 on the path (epropnp.epropnp, .levenberg_marquardt, .camera, .cost_fun, .common, .distributions) exists under the same
 name in the package, and every parameter of the reference signature is present in ours, in the same order, with the
-same default (ours may append optional keyword arguments).  Needs the reference checkout (/root/reference: present in
-the build container, absent on the GPU box) and the pyro shim; skipped where the reference is not available."""
-import importlib
-import inspect
+same default (ours may append optional keyword arguments).  The reference's surface is stored in
+tests/golden/api_surface/reference.json.gz, dumped from the unmodified reference with the pyro shim:
+
+    python tests/test_api_surface_cpu.py <reference checkout>      # rewrites the stored surface
+"""
+import gzip
+import json
 import os
 import subprocess
 import sys
-
-import pytest
 
 from conftest import ROOT
 
 MODULES = ("epropnp.epropnp", "epropnp.levenberg_marquardt", "epropnp.camera", "epropnp.cost_fun", "epropnp.common",
            "epropnp.distributions")
-REFERENCE = "/root/reference"
+GOLDEN = os.path.join(ROOT, "tests", "golden", "api_surface", "reference.json.gz")
 
 _DUMP = r'''
 import importlib, inspect, json, sys
@@ -50,13 +51,12 @@ def _surface(paths, mode):
     env = dict(os.environ, PYTHONPATH=os.pathsep.join(paths))
     r = subprocess.run([sys.executable, "-c", _DUMP, mode, *MODULES], capture_output=True, text=True, env=env, timeout=300)
     assert r.returncode == 0, r.stderr[-2000:]
-    import json
     return json.loads(r.stdout.strip().splitlines()[-1])
 
 
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REFERENCE, "epropnp")), reason="reference checkout not present")
 def test_every_public_name_and_parameter_of_the_reference_exists_here():
-    ref = _surface([os.path.join(ROOT, "oracle", "pyro_shim"), REFERENCE], "own")
+    with gzip.open(GOLDEN, "rt") as f:
+        ref = json.load(f)
     ours = _surface([os.path.join(ROOT, "epro-pnp_b200"), ROOT], "all")
     assert len(ref) > 60
     missing = sorted(k for k in ref if k not in ours)
@@ -75,3 +75,10 @@ def test_every_public_name_and_parameter_of_the_reference_exists_here():
         elif any(extra[2] is None for extra in ours_fixed[len(fixed):]):
             problems.append((name, "extra parameter without a default", ours_fixed[len(fixed):]))
     assert not problems, problems
+
+
+if __name__ == "__main__":
+    surface = _surface([os.path.join(ROOT, "oracle", "pyro_shim"), os.path.abspath(sys.argv[1])], "own")
+    os.makedirs(os.path.dirname(GOLDEN), exist_ok=True)
+    with gzip.GzipFile(GOLDEN, "wb", mtime=0) as f:
+        f.write(json.dumps(surface, sort_keys=True, separators=(",", ":")).encode())

@@ -88,6 +88,44 @@ def test_bench_loop_runs_and_prints_the_contract_line(monkeypatch, capsys, argv,
         assert set(e["step_interval_ms"]) == {"min", "median", "max"}
 
 
+@pytest.mark.parametrize("budget", [64 << 20, 700])
+def test_dump_outputs_writes_the_last_step_reproducibly(monkeypatch, capsys, tmp_path, budget):
+    """--dump-outputs: one float32 .npy per result of the last timed step, the same from run to run; over the byte budget
+    the per-object arrays keep the same sample of objects and the total stays within it."""
+    import numpy as np
+    dumps = []
+    for run in range(2):
+        d = tmp_path / str(run)
+        run_bench(monkeypatch, capsys, ["--no-e2e", "--batch", "4", "--dump-outputs", str(d)], DUMP_BYTES=budget)
+        dumps.append({p.stem: np.load(p) for p in sorted(d.iterdir())})
+    a, b = dumps
+    assert {"pose_opt", "pose_samples", "logw", "cost"} <= set(a) and set(a) == set(b)
+    assert all(v.dtype == np.float32 and np.array_equal(v, b[k], equal_nan=True) for k, v in a.items())
+    assert sum(v.nbytes for v in a.values()) <= budget
+    rows = {v.shape[0] for k, v in a.items() if k in ("pose_opt", "pose_samples", "logw", "cost")}
+    assert rows == ({4} if budget > 1 << 20 else {1})
+    if budget > 1 << 20:
+        # the LAST timed step (i = steps - 1 = 2): its rotating input set and seed, solved directly
+        import bench
+        from epropnp_b200 import native
+        from epropnp_b200.synth import make_problem
+        cfg = dict(bench.CONFIGS["fused"], B=4)
+        n_sets, _ = bench.rotating_sets(cfg)
+        params = native.default_params(6, lm_iter=cfg["lm_iter"], fast_mode=cfg["fast"], z_min=cfg["z_min"],
+                                       mc_samples=cfg["M"], mc_iter=cfg["I"])
+        pc = make_problem(4, cfg["N"], seed=1000, grid2d=cfg["grid2d"])
+
+        def step(i):
+            d = {k: torch.roll(v, shifts=((i % n_sets) * 4) // n_sets, dims=0).contiguous() for k, v in pc.items()}
+            prob = native.Problem(d["x3d"], d["x2d"], d["w2d"], d["cam_mats"], None, None,
+                                  native.adaptive_delta(d["x2d"], d["w2d"], cfg["rel_delta"]))
+            return native.lm_amis_fused(prob, d["pose_init"], params, seed=1234 + i, want_cost=True, want_cost_init=False)
+        last, first = step(2), step(0)
+        for k in ("pose_opt", "pose_samples", "logw", "cost"):
+            assert np.array_equal(a[k], last[k].numpy(), equal_nan=True), k
+        assert not np.array_equal(a["logw"], first["logw"].numpy())
+
+
 @pytest.mark.parametrize("argv", [[], ["--config", "dense"], ["--streams", "1"]])
 def test_both_arms_name_the_same_config(monkeypatch, capsys, argv):
     """`--impl reference` must report the workload of `--impl ours` word for word (the driver pairs the two lines by

@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a kernels, called through the C ABI (epropnp_b200.native -> ctypes),
+"""GPU parity tests: the sm_90a kernels, called through the C ABI (epropnp_b200.native -> ctypes),
 against (1) golden vectors produced by the unmodified reference, (2) the CPU oracle on seeded inputs at
 sizes it finishes in seconds, and (3) size-independent properties at BASELINE.json's full size.
 

@@ -107,8 +107,8 @@ def main():
     out.append(dict(config="evaluate_pnp cost, 128 poses x 4096 objects x 512 pts", B=4096, ms=ms,
                     pose_point_pairs_per_s=S * 4096 * 512 / ms * 1e3))
     # random-sample LM initialiser (RSLMSolver.solve = centre-based translation in torch + epnp_rslm_draw_f32 +
-    # epnp_rslm_f32), demo-notebook and detection configurations; draws='torch' = the reference's torch.multinomial / randn.  (An earlier run, profiles/r2_rslm_ab.jsonl, also timed the reference's own
-    # formulation -- gather + P*B tiny solves + stacked evaluate_pnp -- on the same kernels; it lost everywhere and is gone.)
+    # epnp_rslm_f32), demo-notebook and detection configurations; draws='torch' = the reference's torch.multinomial / randn.  (The reference's own formulation -- gather + P*B tiny
+    # solves + stacked evaluate_pnp -- on the same kernels measured slower and is gone.)
     if os.environ.get("EPNP_BENCH_RSLM"):
         sys.path.insert(0, os.path.join(ROOT, "epro-pnp_b200"))
         from epropnp.camera import PerspectiveCamera

@@ -2,9 +2,8 @@
 """Host <-> device copy ceiling of the box the bench runs on (pinned memory, CUDA events):
 H2D alone, D2H alone, and both directions at once, at the chunk sizes of the end-to-end path.
 
-bench.py's `e2e` number moves 59 MB in and 68 MB out per 4096-object step; whether its ~21 / 24 GB/s are the
-link's limit or the pipeline's is what this tool answers (run it once per pool:
-`gpurun -- 'python tools/pcie_probe.py > gpurun_out/pcie_probe.json'`)."""
+bench.py's `e2e` number moves 59 MB in and 68 MB out per 4096-object step; whether its rate is the link's limit or
+the pipeline's is what this tool answers (`python tools/pcie_probe.py > pcie_probe.json`)."""
 import json
 import sys
 

@@ -1,12 +1,12 @@
 #!/usr/bin/env python
 """Per-kernel SASS fingerprints of libepropnp_b200.so, and the check that the kernels which were validated on
-hardware (parity tests, sanitizer, ncu -- profiles/) are still bit-identical in the current default build.
+hardware (the GPU parity suite) are still bit-identical in the current default build.
 
     python tools/sass_identity.py                 # compare the in-tree library with profiles/validated_sass.json
     python tools/sass_identity.py --write <lib>   # record a library's fingerprints as the validated set
 
 Experiments live behind build options and new entry points get new kernels, so the validated kernels must not change
-unless a GPU run re-validates them (then the manifest is rewritten in the same commit as the new profiles)."""
+unless a GPU run re-validates them (then the manifest is rewritten in the same commit)."""
 import hashlib
 import json
 import os
@@ -40,8 +40,8 @@ def compare(lib=DEFAULT_LIB):
 
 if __name__ == "__main__":
     if len(sys.argv) >= 3 and sys.argv[1] == "--write":
-        json.dump(dict(note="SASS fingerprints of the kernels validated on a B200 (GPU parity suite green on exactly this "
-                            "build; see profiles/README.md)", kernels=fingerprints(sys.argv[2])),
+        json.dump(dict(note="SASS fingerprints of the sm_90a kernels validated on an H100 (GPU parity suite green on "
+                            "exactly this build)", kernels=fingerprints(sys.argv[2])),
                   open(MANIFEST, "w"), indent=1, sort_keys=True)
         print("wrote", MANIFEST)
     else:
