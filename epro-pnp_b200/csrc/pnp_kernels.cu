@@ -10,6 +10,7 @@
 //                                    4 points per thread between block barriers (DESIGN.md section 4).
 //   cost_kernel, evaluate_full_kernel, rslm_draw_kernel, rslm_kernel, cost_backward_kernel, gn_plus_backward_kernel, adaptive_delta_kernel,
 //   mc_epilogue_kernel, mc_lse_backward_kernel      the steps either side of the path (CTA per object).
+//   epnp_init_kernel (pnp_epnp.cuh)  EPnP initialiser with the confidence-quantile point selection, fp64, CTA per object.
 // No tensor cores: the only contraction is 6-deep, the work is FP32-pipe + MUFU bound (DESIGN.md).
 // Build options: EPNP_PHASE_TIMERS (profiling), EPNP_SIMT_EMUL (g++ build for the test-only CPU emulator).
 #include <cuda_runtime.h>
@@ -20,6 +21,7 @@
 #include "pnp_device.cuh"
 #include "pnp_lm.cuh"
 #include "pnp_amis.cuh"
+#include "pnp_epnp.cuh"
 
 namespace {
 
@@ -724,6 +726,171 @@ __global__ void __launch_bounds__(NT) mc_lse_backward_kernel(const float* logw, 
     for (int m = threadIdx.x; m < M; m += NT) o[m] = (gb == 0.f) ? 0.f : gb * expf(__ldg(l + m) - ls);
 }
 // ------------------------------------------------------------------------------------------------
+// EPnP initialiser of the 6DoF test-time solve (lib/test.py:178-194 of the reference; math in pnp_epnp.cuh), one CTA per
+// object:
+//   1. conf_i = (w2d[i,0] + w2d[i,1]) / 2 as order-preserving uint32 keys in shared memory; a NaN confidence makes the
+//      object's pose NaN with n_sel = 0 (np.quantile returns NaN, the mask is empty, cv2 refuses);
+//   2. the order statistics s[k], s[k+1] of np.quantile by a binary radix select on the keys: 32 MSB-first passes, each
+//      a block-wide count of the keys below both candidate prefixes -- no sort, no atomics;
+//   3. the kept points (conf >= threshold) compacted once into shared memory, in index order: each thread owns a
+//      contiguous run of indices, an exclusive scan of the per-thread counts places them.  Only the kept ~20 % are
+//      read from x3d / x2d, by plain loads: a TMA stage of whole rows would move five times the bytes;
+//   4. fp64 passes over the kept points with block reductions: centroid, scatter, then the 56 sums behind M^T M and
+//      the Procrustes fit; lane 0 of warp 0 solves the small problems (pnp_epnp.cuh);
+//   5. one more pass scores the three candidates by reprojection error; the cheapest is written.
+// Shared memory: keys (N) + kept points (5 N floats) = 24 N bytes, within what epnp_max_points(6, 0, 0) allows.
+struct EpnpInitArgs {
+    const float *x3d, *x2d, *w2d, *cam;
+    float* pose;                // (B, 7)
+    int* n_sel;                 // [opt] (B)
+    int N;
+    float q;
+};
+
+__host__ __device__ inline int epnp_init_smem_bytes(int N) { return N * 6 * 4; }
+
+// fp64 butterfly exchange as two 32-bit exchanges of its halves (the bits move unchanged, as a 64-bit shuffle moves them)
+__device__ __forceinline__ double shfl_xor_f64(double v, int o) {
+    uint32_t h[2];
+    memcpy(h, &v, 8);
+    h[0] = __float_as_uint(__shfl_xor_sync(0xffffffffu, __uint_as_float(h[0]), o));
+    h[1] = __float_as_uint(__shfl_xor_sync(0xffffffffu, __uint_as_float(h[1]), o));
+    memcpy(&v, h, 8);
+    return v;
+}
+
+// block-wide fp64 sums of K values per thread (NT threads); every thread gets the totals, partials added in warp order
+template <int K>
+__device__ __forceinline__ void block_sum_f64(double (&v)[K], double* red) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+#pragma unroll
+        for (int o = 16; o >= 1; o >>= 1) v[k] += shfl_xor_f64(v[k], o);
+    }
+    if (lane == 0) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) red[warp * K + k] = v[k];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < K; ++k) v[k] = (red[k] + red[K + k]) + (red[2 * K + k] + red[3 * K + k]);
+    __syncthreads();                    // red is free again
+}
+
+__global__ void __launch_bounds__(NT) epnp_init_kernel(const EpnpInitArgs a) {
+    static_assert(NW == 4, "block_sum_f64 adds four warp partials");
+    // 128: the alignment the other kernels declare for this (module-wide) symbol; a different one here moves their
+    // dynamic shared memory base
+    EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
+    __shared__ double red[NW * epnp::NSUM];
+    __shared__ float fred[2 * NW * 32];
+    __shared__ int counts[NT];
+    __shared__ epnp::Control cp;
+    __shared__ epnp::Candidate cand[3];
+    const int tid = threadIdx.x, obj = blockIdx.x, N = a.N;
+    uint32_t* keys = reinterpret_cast<uint32_t*>(smem_raw);            // [N]
+    float* P = reinterpret_cast<float*>(smem_raw) + N;                 // [5][N]: X Y Z u v of the kept points
+    const float* g3 = a.x3d + (size_t)obj * N * 3;
+    const float* g2 = a.x2d + (size_t)obj * N * 2;
+    int n = N;
+    if (a.w2d) {
+        const float* gw = a.w2d + (size_t)obj * N * 2;
+        float nan_count[1] = {0.f};
+        for (int i = tid; i < N; i += NT) {
+            const float c = (__ldg(gw + 2 * i) + __ldg(gw + 2 * i + 1)) * 0.5f;
+            keys[i] = epnp::conf_key(c);
+            nan_count[0] += (c != c) ? 1.f : 0.f;
+        }
+        block_sum<1>(nan_count, fred, 0);
+        if (nan_count[0] > 0.f) {
+            if (tid == 0) {
+#pragma unroll
+                for (int i = 0; i < 7; ++i) a.pose[(size_t)obj * 7 + i] = CUDART_NAN_F;
+                if (a.n_sel) a.n_sel[obj] = 0;
+            }
+            return;
+        }
+        const epnp::QuantileRank r = epnp::quantile_rank(N, a.q);
+        uint32_t lo = 0u, hi = 0u;          // the largest v with #{key < v} <= k (= s[k]), and the same for k1
+        for (int bit = 31; bit >= 0; --bit) {
+            const uint32_t ca = lo | (1u << bit), cb = hi | (1u << bit);
+            float c[2] = {0.f, 0.f};                // counts <= N are exact in fp32
+            for (int i = tid; i < N; i += NT) {
+                const uint32_t k = keys[i];
+                c[0] += k < ca ? 1.f : 0.f;
+                c[1] += k < cb ? 1.f : 0.f;
+            }
+            block_sum<2>(c, fred, bit & 1);
+            if (c[0] <= (float)r.k) lo = ca;
+            if (c[1] <= (float)r.k1) hi = cb;
+        }
+        const float thr = epnp::quantile_threshold(epnp::key_conf(lo), epnp::key_conf(hi), r.g);
+        const int per = (N + NT - 1) / NT, i0 = min(N, tid * per), i1 = min(N, i0 + per);
+        int mine = 0;
+        for (int i = i0; i < i1; ++i) mine += epnp::key_conf(keys[i]) >= thr ? 1 : 0;
+        counts[tid] = mine;
+        __syncthreads();
+        int off = 0;
+        n = 0;
+        for (int t = 0; t < NT; ++t) {
+            off += t < tid ? counts[t] : 0;
+            n += counts[t];
+        }
+        for (int i = i0; i < i1; ++i) {
+            if (!(epnp::key_conf(keys[i]) >= thr)) continue;
+            P[off] = __ldg(g3 + 3 * i); P[N + off] = __ldg(g3 + 3 * i + 1); P[2 * N + off] = __ldg(g3 + 3 * i + 2);
+            P[3 * N + off] = __ldg(g2 + 2 * i); P[4 * N + off] = __ldg(g2 + 2 * i + 1);
+            ++off;
+        }
+    } else {
+        for (int i = tid; i < N; i += NT) {
+            P[i] = __ldg(g3 + 3 * i); P[N + i] = __ldg(g3 + 3 * i + 1); P[2 * N + i] = __ldg(g3 + 3 * i + 2);
+            P[3 * N + i] = __ldg(g2 + 2 * i); P[4 * N + i] = __ldg(g2 + 2 * i + 1);
+        }
+    }
+    __syncthreads();
+    float Kf[9];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) Kf[i] = __ldg(a.cam + (size_t)obj * 9 + i);
+    const epnp::Intrinsics in = epnp::intrinsics(Kf);
+    double c0[3] = {0.0, 0.0, 0.0};
+    for (int j = tid; j < n; j += NT) { c0[0] += P[j]; c0[1] += P[N + j]; c0[2] += P[2 * N + j]; }
+    block_sum_f64<3>(c0, red);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) c0[c] /= n;
+    double S[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int j = tid; j < n; j += NT) {
+        const double dx = P[j] - c0[0], dy = P[N + j] - c0[1], dz = P[2 * N + j] - c0[2];
+        S[0] += dx * dx; S[1] += dx * dy; S[2] += dx * dz; S[3] += dy * dy; S[4] += dy * dz; S[5] += dz * dz;
+    }
+    block_sum_f64<6>(S, red);
+    if (tid == 0) epnp::control_points(c0, S, n, cp);
+    __syncthreads();
+    double acc[epnp::NSUM];
+#pragma unroll
+    for (int k = 0; k < epnp::NSUM; ++k) acc[k] = 0.0;
+    for (int j = tid; j < n; j += NT) epnp::accumulate_point(cp, in, P[j], P[N + j], P[2 * N + j], P[3 * N + j], P[4 * N + j], acc);
+    block_sum_f64<epnp::NSUM>(acc, red);
+    if (tid == 0) {
+        double al[4];
+        epnp::barycentric(cp, P[0], P[N], P[2 * N], al);
+        epnp::solve_candidates(acc, cp, in, al, n, cand);
+    }
+    __syncthreads();
+    double err[3] = {0.0, 0.0, 0.0};
+    for (int j = tid; j < n; j += NT) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) err[c] += epnp::reproj_error(cand[c], in, P[j], P[N + j], P[2 * N + j], P[3 * N + j], P[4 * N + j]);
+    }
+    block_sum_f64<3>(err, red);
+    if (tid == 0) {
+        epnp::write_pose(cand[epnp::pick_candidate(err)], a.pose + (size_t)obj * 7);
+        if (a.n_sel) a.n_sel[obj] = n;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Host side
 int cuda_fail(cudaError_t e) { g_last_cuda_error = (int)e; return EPNP_ERR_CUDA; }
 
@@ -1084,6 +1251,22 @@ int epnp_rslm_draw_f32(const float* x3d, const float* x2d, const float* w2d, con
         if (e != cudaSuccess) return cuda_fail(e);
         EPNP_LAUNCH(rslm_draw_kernel<4>, B, NT, smem, (cudaStream_t)stream, r);
     }
+    e = cudaGetLastError();
+    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+}
+
+int epnp_epnp_init_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats, float conf_quantile,
+                       float* pose, int* n_sel, int B, int N, void* stream) {
+    if (!x3d || !x2d || !cam_mats || !pose || B < 0 || N < 4) return EPNP_ERR_BAD_ARG;
+    if (!(conf_quantile >= 0.0f && conf_quantile <= 1.0f)) return EPNP_ERR_BAD_ARG;
+    if (N > epnp_max_points(6, 0, 0)) return EPNP_ERR_TOO_MANY_POINTS;
+    if (w2d && epnp::min_selected(N, conf_quantile) < 4) return EPNP_ERR_BAD_ARG;
+    if (B == 0) return EPNP_OK;
+    const int smem = epnp_init_smem_bytes(N);
+    cudaError_t e = cudaFuncSetAttribute(epnp_init_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return cuda_fail(e);
+    const EpnpInitArgs a{x3d, x2d, w2d, cam_mats, pose, n_sel, N, conf_quantile};
+    EPNP_LAUNCH(epnp_init_kernel, B, NT, smem, (cudaStream_t)stream, a);
     e = cudaGetLastError();
     return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
 }

@@ -3,6 +3,7 @@ batched hot loops run in hand-written sm_90a CUDA behind libepropnp_b200.so:
 
     epropnp.epropnp               EProPnP6DoF / EProPnP4DoF / EProPnPBase / cholesky_wrapper
     epropnp.levenberg_marquardt   LMSolver / RSLMSolver
+    epropnp.epnp                  EPnPSolver (EPnP initialisation of the 6DoF test-time solve)
     epropnp.camera                PerspectiveCamera
     epropnp.cost_fun              HuberPnPCost / AdaptiveHuberPnPCost
     epropnp.common                evaluate_pnp, pnp_normalize, pnp_denormalize, rotation helpers
@@ -21,7 +22,8 @@ from .camera import PerspectiveCamera                              # noqa: E402,
 from .cost_fun import HuberPnPCost, AdaptiveHuberPnPCost           # noqa: E402,F401
 from .common import evaluate_pnp                                   # noqa: E402,F401
 from .levenberg_marquardt import LMSolver, RSLMSolver              # noqa: E402,F401
+from .epnp import EPnPSolver                                       # noqa: E402,F401
 from .epropnp import EProPnP4DoF, EProPnP6DoF                      # noqa: E402,F401
 
 __all__ = ['build_pnp', 'build_camera', 'build_cost_fun', 'PerspectiveCamera', 'HuberPnPCost', 'AdaptiveHuberPnPCost',
-           'evaluate_pnp', 'LMSolver', 'RSLMSolver', 'EProPnP4DoF', 'EProPnP6DoF']
+           'evaluate_pnp', 'LMSolver', 'RSLMSolver', 'EPnPSolver', 'EProPnP4DoF', 'EProPnP6DoF']

@@ -183,6 +183,31 @@ def rslm(prob: Problem, inds, start, params, want_all=False):
     return out
 
 
+def epnp_init(x3d, x2d, w2d, cam_mats, conf_quantile=0.8, want_n_sel=False):
+    """EPnP initialisation of the 6DoF test-time solve (epnp_epnp_init_f32): per object, the points whose confidence
+    mean(w2d, -1) is >= its np.quantile(., conf_quantile) (every point when w2d is None), then EPnP as
+    cv2.solvePnP(SOLVEPNP_EPNP) computes it.  -> pose (B, 7) [x y z w i j k], w >= 0 [, n_sel (B) int32]."""
+    _need_cuda(x3d, "x3d")
+    if x3d.dim() != 3 or x3d.shape[2] != 3:
+        raise ValueError(f"x3d must be (B, N, 3), got {tuple(x3d.shape)}")
+    B, N = x3d.shape[0], x3d.shape[1]
+    dev = x3d.device
+    for t, what in ((x2d, "x2d"), (w2d, "w2d")):
+        if t is not None and (tuple(t.shape) != (B, N, 2) or t.device != dev):
+            raise ValueError(f"{what} must be ({B}, {N}, 2) on {dev}, got {tuple(t.shape)} on {t.device}")
+    x3d, x2d = _f32c(x3d), _f32c(x2d)
+    w2d = None if w2d is None else _f32c(w2d)
+    pose = torch.empty(B, 7, dtype=torch.float32, device=dev)
+    n_sel = torch.empty(B, dtype=torch.int32, device=dev) if want_n_sel else None
+    if B > 0:
+        cam = _cam(cam_mats, B, dev)
+        with torch.cuda.device(dev):
+            check(lib().epnp_epnp_init_f32(ptr(x3d), ptr(x2d), ptr(w2d), ptr(cam), ctypes.c_float(conf_quantile),
+                                           ptr(pose), None if n_sel is None else capi.iptr(n_sel), B, N,
+                                           stream_ptr(dev)), "epnp_epnp_init_f32")
+    return (pose, n_sel) if want_n_sel else pose
+
+
 def gn_plus_backward(prob: Problem, pose, grad_pose_plus, dof, z_min, eps, huber_eps, want=(True, True, True, True)):
     """dL/d(x3d, x2d, w2d, delta) of pose_opt_plus = pose (+) gn_step(pose) (epnp_gn_plus_backward_f32)."""
     B, N = prob.B, prob.N
@@ -411,4 +436,4 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
 
 
 __all__ = ["Problem", "adaptive_delta", "cost_backward", "evaluate_cost", "evaluate_full", "lm_solve", "amis", "lm_amis_fused",
-           "lm_amis_fused_host", "lm_amis_fused_push", "fused_workspace_bytes", "rslm", "gn_plus_backward", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]
+           "lm_amis_fused_host", "lm_amis_fused_push", "fused_workspace_bytes", "rslm", "epnp_init", "gn_plus_backward", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

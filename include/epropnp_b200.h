@@ -133,6 +133,21 @@ int epnp_rslm_f32(const float* x3d, const float* x2d, const float* w2d, const fl
                   float* pose_best, float* cost_best, float* pose_all, float* cost_all,
                   int P, int n, int B, int N, const EpnpParams* p, void* stream);
 
+/* EPnP initialisation of the 6DoF test-time solve (EPro-PnP-6DoF/lib/test.py:178-194): per object,
+ *   conf_i = (w2d[i,0] + w2d[i,1]) / 2, the points with conf_i >= np.quantile(conf, conf_quantile) (NumPy 2.x
+ *   'linear', evaluated in fp32 as NumPy does for a float32 row; ties kept) -> cv2.solvePnP(..., SOLVEPNP_EPNP)
+ *   (pixel coordinates, fu = K00, fv = K11, uc = K02, vc = K12; K01 is not read) -> pose (B, 7) = [x y z w i j k],
+ *   the quaternion normalised with w >= 0.  EPnP runs in fp64.  w2d [opt]: NULL keeps every point.
+ *   n_sel [opt] (B) int32: points kept per object.  The camera bounds and z_min of the other entry points do not
+ *   apply (cv2's EPnP has none).  An object with a NaN confidence gets a NaN pose and n_sel = 0; degenerate (coplanar,
+ *   collinear) kept points give a finite or NaN pose; neither affects other objects.
+ *   EPNP_ERR_BAD_ARG: N < 4, conf_quantile outside [0, 1], or fewer than 4 points kept by construction
+ *   (N - floor((N-1) q) - (fractional part > 0) < 4 with w2d given; cv2 refuses those); EPNP_ERR_TOO_MANY_POINTS:
+ *   N > epnp_max_points(6, 0, 0). */
+int epnp_epnp_init_f32(const float* x3d, const float* x2d, const float* w2d /*[opt] NULL = all points*/,
+                       const float* cam_mats, float conf_quantile, float* pose /*(B,7)*/, int* n_sel /*[opt]*/,
+                       int B, int N, void* stream);
+
 /* LMSolver.solve with a given pose_init (levenberg_marquardt.py:80-190, _lm_iter :192-241, GN
  * fast mode :136-152) plus, when pose_opt_plus != NULL, the extra Gauss-Newton step of
  * LMSolver.forward (:66-68, gn_step :243-253, pose_add :255-265).

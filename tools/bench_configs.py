@@ -184,8 +184,78 @@ def main():
                 row[key] = timed(step, iters=20)
             os.environ["EPNP_NATIVE_MC_EPILOGUE"] = "1"
             out.append(row)
+    # the 6DoF test-time path (EPro-PnP-6DoF/lib/test.py:178-211): EPnP on the 20 % most confident points, then GN(3);
+    # host_cv2_ms is the reference's own per-object loop on the same objects (device -> host copy, np.quantile mask,
+    # cv2 EPnP, scipy quaternion, host -> device copy), where OpenCV is installed
+    if os.environ.get("EPNP_BENCH_EPNP"):
+        sys.path.insert(0, os.path.join(ROOT, "epro-pnp_b200"))
+        from epropnp.camera import PerspectiveCamera
+        from epropnp.cost_fun import AdaptiveHuberPnPCost
+        from epropnp.epnp import EPnPSolver
+        from epropnp.levenberg_marquardt import LMSolver
+        card = dict(card=torch.cuda.get_device_name(dev), power_limit_w=power_limit(dev)) if dev.type == "cuda" else {}
+        N = 16 if TOY else 4096
+        for B in bs(256, 1024):
+            pc = {k: v.to(dev) for k, v in make_problem(B, N, seed=13, grid2d=True).items()}
+            camera = PerspectiveCamera(cam_mats=pc["cam_mats"], z_min=0.01)
+            cost_fun = AdaptiveHuberPnPCost(relative_delta=0.1)
+            cost_fun.set_param(pc["x2d"], pc["w2d"])
+            solver = LMSolver(dof=6, num_iter=3, init_solver=EPnPSolver(conf_quantile=0.8))
+            row = dict(config=f"6DoF test-time path: EPnP init (q=0.8) + GN(3), N={N}", B=B, **card)
+            row["ms_epnp"] = timed(lambda: native.epnp_init(pc["x3d"], pc["x2d"], pc["w2d"], pc["cam_mats"], 0.8), iters=10)
+            row["ms_epnp_gn3"] = timed(lambda: solver.solve(pc["x3d"], pc["x2d"], pc["w2d"], camera, cost_fun,
+                                                            fast_mode=True), iters=10)
+            host = host_cv2_epnp_ms(pc, 0.8)
+            if host is not None:
+                row["host_cv2_ms"] = host
+            out.append(row)
     for r in out:
         print(json.dumps(r))
+
+
+def power_limit(dev):
+    """The card's power limit in W (read-only nvidia-smi query), None when it cannot be read."""
+    import subprocess
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=power.limit",
+                            "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30)
+        return float(r.stdout.strip())
+    except (OSError, ValueError, subprocess.SubprocessError):
+        return None
+
+
+def host_cv2_epnp_ms(pc, q, reps=3):
+    """Wall time of the reference's per-object EPnP loop (lib/test.py:178-194) on the objects of `pc`, None without
+    OpenCV."""
+    try:
+        import cv2
+        import numpy as np
+        from scipy.spatial.transform import Rotation
+    except ImportError:
+        return None
+    import time
+    dev = pc["x3d"].device
+
+    def loop():
+        x3d, x2d, w2d, K = (pc[k].cpu().numpy() for k in ("x3d", "x2d", "w2d", "cam_mats"))
+        pose = np.empty((x3d.shape[0], 7), np.float32)
+        for b in range(x3d.shape[0]):
+            conf = w2d[b].mean(-1)
+            m = conf >= np.quantile(conf, q)
+            _, rvec, tvec = cv2.solvePnP(x3d[b][m], x2d[b][m], K[b], None, flags=cv2.SOLVEPNP_EPNP)
+            pose[b, :3] = tvec[:, 0]
+            pose[b, 3:] = Rotation.from_rotvec(rvec[:, 0]).as_quat()[[3, 0, 1, 2]]
+        return torch.from_numpy(pose).to(dev)
+    ts = []
+    for _ in range(reps):
+        if dev.type == "cuda":
+            torch.cuda.synchronize(dev)
+        t0 = time.perf_counter()
+        loop()
+        if dev.type == "cuda":
+            torch.cuda.synchronize(dev)
+        ts.append((time.perf_counter() - t0) * 1e3)
+    return statistics.median(ts)
 
 
 if __name__ == "__main__":
