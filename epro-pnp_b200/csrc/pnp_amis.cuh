@@ -20,9 +20,11 @@
 
 namespace {
 
-// Resident CTAs per SM the 128-thread kernel is compiled for.  Shared memory (36.1 KB at N = M = 512) would allow six at 80
-// registers, but then the sweep spills.  Five at 96 registers against four at 128, H100 SXM at a 400 W power limit, median
-// of 8 alternating runs per 4096 objects: 1.363 vs 1.378 ms (B = 1024: 0.351 vs 0.350 ms), so five stay.
+// Resident CTAs per SM the 128-thread kernel is compiled for.  Six fit in shared memory (36.1 KB at N = M = 512) at 80
+// registers; ptxas then spills 76 bytes, none of it inside the sweep loops.  H100 SXM at a 400 W power limit (power-capped,
+// SM clock 1575-1690 MHz), 4096 objects, 3 alternating runs each: amis_kernel 1.222 ms at five against 1.245 ms at six,
+// 2.483 M against 2.420 M objects/s on the bench step, so five stay.  (Eight point pairs per sweep trip instead of four, same
+// chains: 1.256 ms at five.)
 constexpr int AMIS_CTAS_PER_SM = 5;
 
 template <int DOF> struct ProposalOf;
@@ -38,6 +40,7 @@ template <int DOF, int T> struct AmisHead {
     float red[2 * (T / 32) * 32];           // two halves: consecutive reductions alternate, one barrier each
     float pose[8];                          // the LM solution ...
     float cov[DOF * DOF];                   // ... and its covariance
+    float box[6];                           // bounding box of the object's points (point_box)
     typename ProposalOf<DOF>::type prop[MAX_ITER];
 };
 
@@ -113,10 +116,7 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
             proposal_draw6(sh.prop[i], n3, chi2, n4, q);
 #pragma unroll
             for (int k = 0; k < 7; ++k) smp[m * 7 + k] = q[k];
-            float* out = a.pose_samples + ((size_t)obj * M + m) * 7;
-#pragma unroll
-            for (int k = 0; k < 7; ++k) out[k] = q[k];
-            if constexpr (PARTS == 1) cst[m] = pose_cost<6>(pts4, a.N, q, cam, delta);
+            if constexpr (PARTS == 1) cst[m] = pose_cost_pairs<6>(pts4, 0, (a.N + 1) >> 1, q, cam, delta, sh.box);
             RunningLse l;
             l.start(proposal_logpdf6(sh.prop[0], q));
             for (int j = 1; j <= i; ++j) l.add(proposal_logpdf6(sh.prop[j], q));
@@ -131,7 +131,7 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
                 float q[7];
 #pragma unroll
                 for (int k = 0; k < 7; ++k) q[k] = smp[m * 7 + k];
-                cpart[part * M + m] = pose_cost_pairs<6>(pts4, j0, j1, q, cam, delta);
+                cpart[part * M + m] = pose_cost_pairs<6>(pts4, j0, j1, q, cam, delta, sh.box);
             }
             __syncthreads();
             for (int s = tid; s < S; s += T) {
@@ -311,10 +311,9 @@ __device__ void amis_phase4(const KArgs& a, AmisHead<4, T>& sh, const float* pts
                 q[3] = draw_yaw(a.seed, a.obj_offset + (uint32_t)obj, (uint32_t)m, s, S, sh.prop[i].mode, sh.prop[i].kappa);
             }
             draw_translation(sh.prop[i].mu, sh.prop[i].lt, n3, chi2, q);
-            float* out = a.pose_samples + ((size_t)obj * M + m) * 4;
 #pragma unroll
-            for (int k = 0; k < 4; ++k) { smp[m * 4 + k] = q[k]; out[k] = q[k]; }
-            if constexpr (PARTS == 1) cst[m] = pose_cost<4>(pts4, a.N, q, cam, delta);
+            for (int k = 0; k < 4; ++k) smp[m * 4 + k] = q[k];
+            if constexpr (PARTS == 1) cst[m] = pose_cost_pairs<4>(pts4, 0, (a.N + 1) >> 1, q, cam, delta, sh.box);
             RunningLse l;
             l.start(proposal_logpdf4(sh.prop[0], q));
             for (int j = 1; j <= i; ++j) l.add(proposal_logpdf4(sh.prop[j], q));
@@ -326,7 +325,7 @@ __device__ void amis_phase4(const KArgs& a, AmisHead<4, T>& sh, const float* pts
             const int j0 = (int)((long long)npair * part / PARTS) & ~3, j1 = part + 1 == PARTS ? npair : ((int)((long long)npair * (part + 1) / PARTS) & ~3);
             for (int s = tid % NT; s < S; s += NT) {
                 const int m = i * S + s;
-                cpart[part * M + m] = pose_cost_pairs<4>(pts4, j0, j1, smp + m * 4, cam, delta);
+                cpart[part * M + m] = pose_cost_pairs<4>(pts4, j0, j1, smp + m * 4, cam, delta, sh.box);
             }
             __syncthreads();
             for (int s = tid; s < S; s += T) {
@@ -407,6 +406,17 @@ struct PushArgs {
     int n;
 };
 
+// dst[0, n) = src[0, n) by the T threads of the CTA: float4 runs where n and both addresses allow, single floats otherwise.
+template <int T>
+__device__ __forceinline__ void block_copy(float* dst, const float* src, int n) {
+    const int tid = threadIdx.x;
+    if ((n & 3) == 0 && ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15u) == 0) {
+        for (int q = tid; q < n / 4; q += T) reinterpret_cast<float4*>(dst)[q] = reinterpret_cast<const float4*>(src)[q];
+    } else {
+        for (int m = tid; m < n; m += T) dst[m] = src[m];
+    }
+}
+
 // The push epilogue of one object: its M log-weights (as this CTA wrote them to global memory) and its pose go to row
 // `row` of every peer's buffers.  Not inlined: it must not take part in the main body's register allocation (inlined,
 // it would weigh on every caller, pushing or not).
@@ -415,12 +425,7 @@ __device__ __noinline__ void push_rows(const float* src, const float* pose, size
                                        float* const* peer_logw, float* const* peer_pose, int n) {
     const int tid = threadIdx.x;
     for (int r = 0; r < n; ++r) {
-        float* dst = peer_logw[r] + row * M;
-        if ((M & 3) == 0 && ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15u) == 0) {
-            for (int q = tid; q < M / 4; q += T) reinterpret_cast<float4*>(dst)[q] = reinterpret_cast<const float4*>(src)[q];
-        } else {
-            for (int m = tid; m < M; m += T) dst[m] = src[m];
-        }
+        block_copy<T>(peer_logw[r] + row * M, src, M);
         if (tid < PD) peer_pose[r][row * PD + tid] = pose[tid];
     }
 }
@@ -459,11 +464,15 @@ __global__ void __launch_bounds__(T, T == NT ? AMIS_CTAS_PER_SM : 1) amis_kernel
         ld.template load_object<T>(obj, pts4, serial_warp);
     }
     __syncthreads();
+    point_box<T>(pts4, a.N, sh.red + (T / 32) * 32, sh.box);     // the second half of `red`: the AMIS loop starts on the first
     const Cam cam = load_cam(a, obj);
     const float delta = __ldg(a.delta + obj);
     PH_MARK(a, PH_LOAD);
     if constexpr (DOF == 6) amis_phase6<T>(a, sh, pts4, dyn + pl.smp, dyn + pl.cost, dyn + pl.logp, dyn + pl.cpart, cam, delta, obj);
     else amis_phase4<T>(a, sh, pts4, dyn + pl.smp, dyn + pl.cost, dyn + pl.logp, dyn + pl.cpart, cam, delta, obj);
+    // The samples leave as one contiguous run per object: `smp` holds them in the output's (M, PD) layout, complete since
+    // the AMIS loop's last barrier.  (The covariance the fused call may have parked in these rows was read at set-up.)
+    block_copy<T>(a.pose_samples + (size_t)obj * M * PD, dyn + pl.smp, M * PD);
     // In-kernel gather (push.n > 0, uniform for the launch).  A run-time branch of ONE kernel, not a second instantiation:
     // a sharded run must be bit-identical to the single-GPU run, and two instantiations are two compilations -- as
     // template variants the push / plain pair need not agree bit for bit, since each compilation allocates registers

@@ -346,7 +346,9 @@ template <int T = NT> __device__ __forceinline__ float block_max(float v, float*
 // branches in one expression, no select -- accumulated by its last multiply-add.  Same arithmetic per half as pnp::point_cost.
 __device__ __forceinline__ float2 splat(float x) { return make_float2(x, x); }
 
-template <bool BOUNDED>
+// ZCLAMP = false drops the depth clamp: only for a pose whose every point is known to lie beyond z_min (depth_clears),
+// where fmaxf(zh, z_min) == zh and the result is the same.
+template <bool BOUNDED, bool ZCLAMP = true>
 __device__ __forceinline__ float2 pair_cost(const float2 (&P2)[12], const Cam& cam, float delta, float2 acc,
                                             const float4 q0, const float4 q1, const float4 q2, const float4 q3) {
     const float2 X = make_float2(q0.x, q0.y), Y = make_float2(q0.z, q0.w), Z = make_float2(q1.x, q1.y);
@@ -355,7 +357,8 @@ __device__ __forceinline__ float2 pair_cost(const float2 (&P2)[12], const Cam& c
     const float2 xh = v2fma(P2[0], X, v2fma(P2[1], Y, v2fma(P2[2], Z, P2[3])));
     const float2 yh = v2fma(P2[4], X, v2fma(P2[5], Y, v2fma(P2[6], Z, P2[7])));
     const float2 zh = v2fma(P2[8], X, v2fma(P2[9], Y, v2fma(P2[10], Z, P2[11])));
-    const float2 iz = make_float2(FastRcp()(fmaxf(zh.x, cam.z_min)), FastRcp()(fmaxf(zh.y, cam.z_min)));
+    const float2 iz = ZCLAMP ? make_float2(FastRcp()(fmaxf(zh.x, cam.z_min)), FastRcp()(fmaxf(zh.y, cam.z_min)))
+                             : make_float2(FastRcp()(zh.x), FastRcp()(zh.y));
     float2 tx, ty;
     if (BOUNDED) {
         float2 px = v2mul(xh, iz), py = v2mul(yh, iz);
@@ -373,7 +376,7 @@ __device__ __forceinline__ float2 pair_cost(const float2 (&P2)[12], const Cam& c
 }
 
 // pair records [j0, j1)
-template <bool BOUNDED>
+template <bool BOUNDED, bool ZCLAMP = true>
 __device__ __forceinline__ float sweep_cost(const float4* pts4, int j0, int j1, const float* P, const Cam& cam, float delta) {
     // point pairs in flight per thread: enough independent chains to cover the FMA and MUFU latencies at five
     // resident CTAs per SM without raising the register count past what those five CTAs allow
@@ -389,11 +392,11 @@ __device__ __forceinline__ float sweep_cost(const float4* pts4, int j0, int j1, 
     for (; j + U <= npair; j += U) {
         const float4* q = pts4 + 4 * j;
 #pragma unroll
-        for (int u = 0; u < U; ++u) c[u] = pair_cost<BOUNDED>(P2, cam, delta, c[u], q[4 * u], q[4 * u + 1], q[4 * u + 2], q[4 * u + 3]);
+        for (int u = 0; u < U; ++u) c[u] = pair_cost<BOUNDED, ZCLAMP>(P2, cam, delta, c[u], q[4 * u], q[4 * u + 1], q[4 * u + 2], q[4 * u + 3]);
     }
     for (; j < npair; ++j) {
         const float4* q = pts4 + 4 * j;
-        c[0] = pair_cost<BOUNDED>(P2, cam, delta, c[0], q[0], q[1], q[2], q[3]);
+        c[0] = pair_cost<BOUNDED, ZCLAMP>(P2, cam, delta, c[0], q[0], q[1], q[2], q[3]);
     }
     float2 t = c[0];
 #pragma unroll
@@ -413,6 +416,72 @@ __device__ __forceinline__ float pose_cost_pairs(const float* pts, int j0, int j
 template <int DOF>
 __device__ __forceinline__ float pose_cost(const float* pts, int N, const float* pose, const Cam& cam, float delta) {
     return pose_cost_pairs<DOF>(pts, 0, (N + 1) >> 1, pose, cam, delta);
+}
+
+// Axis-aligned bounding box of an object's resident points: box[0..2] = min X, Y, Z, box[3..5] = max X, Y, Z.  An axis
+// with a non-finite coordinate gets (-inf, +inf), so depth_clears fails for every pose.  Block-wide (T threads), the
+// per-warp partials pass through `red`; `box` is shared memory and complete when the function returns.
+template <int T>
+__device__ __forceinline__ void point_box(const float* pts, int N, float* red, float* box) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float v[6];                             // min X, min Y, min Z, -max X, -max Y, -max Z
+#pragma unroll
+    for (int k = 0; k < 6; ++k) v[k] = CUDART_INF_F;
+    const float4* pts4 = reinterpret_cast<const float4*>(pts);
+    for (int j = threadIdx.x; j < (N + 1) >> 1; j += T) {
+        const float4 a = pts4[4 * j], b = pts4[4 * j + 1];      // X0 X1 Y0 Y1, Z0 Z1 ..
+        const float c[6] = {a.x, a.y, a.z, a.w, b.x, b.y};
+#pragma unroll
+        for (int k = 0; k < 6; ++k) {
+            const int ax = k >> 1;
+            if (isfinite(c[k])) { v[ax] = fminf(v[ax], c[k]); v[3 + ax] = fminf(v[3 + ax], -c[k]); }
+            else v[ax] = v[3 + ax] = -CUDART_INF_F;
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < 6; ++k)
+#pragma unroll
+        for (int o = 16; o >= 1; o >>= 1) v[k] = fminf(v[k], __shfl_xor_sync(0xffffffffu, v[k], o));
+    if (lane == 0) {
+#pragma unroll
+        for (int k = 0; k < 6; ++k) red[warp * 32 + k] = v[k];
+    }
+    __syncthreads();
+    if (threadIdx.x < 6) {
+        const int k = threadIdx.x;
+        float m = red[k];
+#pragma unroll
+        for (int w = 1; w < T / 32; ++w) m = fminf(m, red[w * 32 + k]);
+        box[k] = k < 3 ? m : -m;
+    }
+    __syncthreads();
+}
+
+// Whether zh = P[8] X + P[9] Y + P[10] Z + P[11] exceeds z_min for every point of `box`, however the sweep rounds it: the
+// box's lowest zh, less a margin far above the rounding error of both that bound and the sweep's three-FFMA chain (each a
+// few units in the last place of |P[8]| |X| + |P[9]| |Y| + |P[10]| |Z| + |P[11]|).  NaN anywhere makes it false.
+__device__ __forceinline__ bool depth_clears(const float* P, const float* box, float z_min) {
+    float lo = P[11], mag = fabsf(P[11]);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        lo += fminf(P[8 + k] * box[k], P[8 + k] * box[3 + k]);
+        mag += fabsf(P[8 + k]) * fmaxf(fabsf(box[k]), fabsf(box[3 + k]));
+    }
+    return lo - (1e-5f * mag + 1e-30f) > z_min;
+}
+
+// pose_cost_pairs for an object whose points lie in `box`.  Where no point of the pose can reach the depth clamp and the
+// camera has no bounds, the sweep runs without the clamp; the lanes sweeping together vote, so a warp runs one loop.
+template <int DOF>
+__device__ __forceinline__ float pose_cost_pairs(const float* pts, int j0, int j1, const float* pose, const Cam& cam, float delta,
+                                                 const float* box) {
+    float R[9], P[12];
+    pose_to_rot<DOF>(pose, R);
+    make_proj(cam.k, R, pose, P);
+    const float4* pts4 = reinterpret_cast<const float4*>(pts);
+    if (__all_sync(__activemask(), !cam.bounded && depth_clears(P, box, cam.z_min)))
+        return sweep_cost<false, false>(pts4, j0, j1, P, cam, delta);
+    return cam.bounded ? sweep_cost<true>(pts4, j0, j1, P, cam, delta) : sweep_cost<false>(pts4, j0, j1, P, cam, delta);
 }
 
 }  // namespace
