@@ -82,11 +82,21 @@ __device__ __forceinline__ float log_add_exp(float a, float b) {
     return (lo == -CUDART_INF_F) ? hi : hi + fast_log1p(fast_exp(lo - hi));
 }
 
+// One object's AMIS loop split over a thread-block cluster (amis_split_kernel): this CTA is rank `rank` of `ctas` and
+// holds `npair` pair records of the object.  xbuf: 2 S floats of this CTA's shared memory, the per-sample partial costs
+// of its point range in the half of the current iteration's parity.
+struct SplitCtx {
+    float* xbuf;
+    int rank, ctas, npair;
+};
+
 // ------------------------------------------------------------------------------------------------
 // AMIS loop for the resident object, 6DoF.  sh.prop[0] holds the first proposal (the kernel fitted it to the LM solution).
-template <int T>
+// SPLIT: the cluster form (sc describes the CTA's share); every rank draws the same samples and, after the exchange of
+// the partial costs, holds the same costs, so each runs the same refits; rank 0 alone writes the outputs.
+template <int T, bool SPLIT = false>
 __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts4, float* smp, float* cst, float* logp,
-                            float* cpart, const Cam& cam, float delta, int obj) {
+                            float* cpart, const Cam& cam, float delta, int obj, const SplitCtx sc = SplitCtx{}) {
     constexpr int PARTS = T / NT;           // threads sweeping one sample (1: the thread that drew it)
     const Params& p = a.p;
     const int tid = threadIdx.x;
@@ -124,7 +134,7 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
         }
         if constexpr (PARTS > 1) {
             __syncthreads();
-            const int part = tid / NT, npair = (a.N + 1) >> 1;
+            const int part = tid / NT, npair = SPLIT ? sc.npair : (a.N + 1) >> 1;
             const int j0 = (int)((long long)npair * part / PARTS) & ~3, j1 = part + 1 == PARTS ? npair : ((int)((long long)npair * (part + 1) / PARTS) & ~3);
             for (int s = tid % NT; s < S; s += NT) {
                 const int m = i * S + s;
@@ -139,7 +149,19 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
                 float c = cpart[m];
 #pragma unroll
                 for (int r = 1; r < PARTS; ++r) c += cpart[r * M + m];
-                cst[m] = c;
+                if constexpr (SPLIT) sc.xbuf[(i & 1) * S + s] = c;
+                else cst[m] = c;
+            }
+            if constexpr (SPLIT) {
+                // One cluster barrier per iteration: the half (i & 1) of xbuf is written again at iteration i + 2, after
+                // the barrier of iteration i + 1, which every rank reaches only once its reads below are done.
+                cluster_sync();
+                for (int s = tid; s < S; s += T) {
+                    const float* x = sc.xbuf + (i & 1) * S + s;
+                    float c = dsmem_ld(x, 0);
+                    for (int r = 1; r < sc.ctas; ++r) c += dsmem_ld(x, r);
+                    cst[i * S + s] = c;
+                }
             }
         }
         PH_MARK(a, PH_DRAW_SWEEP);
@@ -157,7 +179,8 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
         const float log_cnt = logf((float)(i + 1));
         auto logweight = [&](int m) { return -cst[m] - (logp[m] - log_cnt); };
         if (i == I - 1) {
-            for (int m = tid; m < M; m += T) logw_out[m] = logweight(m);
+            if (!SPLIT || sc.rank == 0)
+                for (int m = tid; m < M; m += T) { logw_out[m] = logweight(m); SPLIT_AUDIT_STORES(1); }
             PH_MARK(a, PH_OUTPUT);
             break;
         }
@@ -268,8 +291,9 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
         PH_MARK(a, PH_REFIT_FINISH);
         __syncthreads();
     }
-    if (a.proposals && tid < I) {
+    if (a.proposals && tid < I && (!SPLIT || sc.rank == 0)) {
         float* o = a.proposals + ((size_t)obj * I + tid) * PROP_FLOATS;
+        SPLIT_AUDIT_STORES(PROP_FLOATS);
         const Proposal6& pr = sh.prop[tid];
         o[0] = pr.mu[0]; o[1] = pr.mu[1]; o[2] = pr.mu[2];
 #pragma unroll
@@ -284,9 +308,11 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
 // with the yaw proposal 0.75 von Mises + 0.25 uniform.  Injected noise: noise_rot (B, M) holds the yaw
 // draws themselves (the reference samples them with numpy on the host, distributions.py:61-72, so there
 // is no base noise to replay).
-template <int T>
+// SPLIT: the cluster form (sc describes the CTA's share); every rank draws the same samples and, after the exchange of
+// the partial costs, holds the same costs, so each runs the same refits; rank 0 alone writes the outputs.
+template <int T, bool SPLIT = false>
 __device__ void amis_phase4(const KArgs& a, AmisHead<4, T>& sh, const float* pts4, float* smp, float* cst, float* logp,
-                            float* cpart, const Cam& cam, float delta, int obj) {
+                            float* cpart, const Cam& cam, float delta, int obj, const SplitCtx sc = SplitCtx{}) {
     constexpr int PARTS = T / NT;
     const Params& p = a.p;
     const int tid = threadIdx.x;
@@ -321,7 +347,7 @@ __device__ void amis_phase4(const KArgs& a, AmisHead<4, T>& sh, const float* pts
         }
         if constexpr (PARTS > 1) {
             __syncthreads();
-            const int part = tid / NT, npair = (a.N + 1) >> 1;
+            const int part = tid / NT, npair = SPLIT ? sc.npair : (a.N + 1) >> 1;
             const int j0 = (int)((long long)npair * part / PARTS) & ~3, j1 = part + 1 == PARTS ? npair : ((int)((long long)npair * (part + 1) / PARTS) & ~3);
             for (int s = tid % NT; s < S; s += NT) {
                 const int m = i * S + s;
@@ -333,7 +359,19 @@ __device__ void amis_phase4(const KArgs& a, AmisHead<4, T>& sh, const float* pts
                 float c = cpart[m];
 #pragma unroll
                 for (int r = 1; r < PARTS; ++r) c += cpart[r * M + m];
-                cst[m] = c;
+                if constexpr (SPLIT) sc.xbuf[(i & 1) * S + s] = c;
+                else cst[m] = c;
+            }
+            if constexpr (SPLIT) {
+                // One cluster barrier per iteration: the half (i & 1) of xbuf is written again at iteration i + 2, after
+                // the barrier of iteration i + 1, which every rank reaches only once its reads below are done.
+                cluster_sync();
+                for (int s = tid; s < S; s += T) {
+                    const float* x = sc.xbuf + (i & 1) * S + s;
+                    float c = dsmem_ld(x, 0);
+                    for (int r = 1; r < sc.ctas; ++r) c += dsmem_ld(x, r);
+                    cst[i * S + s] = c;
+                }
             }
         }
         PH_MARK(a, PH_DRAW_SWEEP);
@@ -344,7 +382,8 @@ __device__ void amis_phase4(const KArgs& a, AmisHead<4, T>& sh, const float* pts
         const float log_cnt = logf((float)(i + 1));
         auto logweight = [&](int m) { return -cst[m] - (logp[m] - log_cnt); };
         if (i == I - 1) {
-            for (int m = tid; m < M; m += T) logw_out[m] = logweight(m);
+            if (!SPLIT || sc.rank == 0)
+                for (int m = tid; m < M; m += T) { logw_out[m] = logweight(m); SPLIT_AUDIT_STORES(1); }
             PH_MARK(a, PH_OUTPUT);
             break;
         }
@@ -380,8 +419,9 @@ __device__ void amis_phase4(const KArgs& a, AmisHead<4, T>& sh, const float* pts
         PH_MARK(a, PH_REFIT_FINISH);
         __syncthreads();
     }
-    if (a.proposals && tid < I) {       // (B, I, 19): mu3, Lt6, mode, kappa, 0...
+    if (a.proposals && tid < I && (!SPLIT || sc.rank == 0)) {       // (B, I, 19): mu3, Lt6, mode, kappa, 0...
         float* o = a.proposals + ((size_t)obj * I + tid) * PROP_FLOATS;
+        SPLIT_AUDIT_STORES(PROP_FLOATS);
         const Proposal4& pr = sh.prop[tid];
         o[0] = pr.mu[0]; o[1] = pr.mu[1]; o[2] = pr.mu[2];
 #pragma unroll
@@ -481,6 +521,109 @@ __global__ void __launch_bounds__(T, T == NT ? AMIS_CTAS_PER_SM : 1) amis_kernel
         __syncthreads();                                        // the CTA's own global stores are visible to all its threads
         push_rows<T>(a.logw + (size_t)obj * M, sh.pose, (size_t)a.obj_offset + (size_t)obj, M, PD, push.logw, push.pose, push.n);
     }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Objects whose points do not fit one SM: one object per thread-block CLUSTER of `ctas` CTAs (grid = B * ctas), rank r
+// holding the contiguous point range [r share, (r + 1) share) (split_share).  Every rank runs the whole AMIS control
+// flow of amis_kernel<DOF, 512> on the same samples -- Philox keyed by (seed, obj_offset + object, m), or the same
+// injected noise -- and sweeps only its own range, in the dense kernel's four point ranges.  Per iteration the ranks
+// exchange their per-sample partial costs through distributed shared memory and add them in rank order 0 .. ctas - 1, so
+// all ranks hold bit-identical costs and log-densities and compute the refits redundantly (no proposal broadcast).  The
+// result depends on ctas (the order of that sum), never on B, the shard or obj_offset.
+constexpr int SPLIT_MAX_CTAS = 8;                   // the portable cluster size
+
+// Points per rank: ceil(N / C) rounded up to a multiple of 8, so every range starts where a bulk copy may start; the
+// last rank's range is the remainder (shorter, or empty when C is larger than N needs).
+__host__ __device__ inline int split_share(int N, int C) { return ((N + C - 1) / C + 7) / 8 * 8; }
+
+struct AmisSplitPlan {
+    AmisPlan a;
+    int xbuf;                                       // 2 S floats: the partial costs exchanged per iteration
+};
+// plan_amis<DOF, 512> for a rank holding `share` points, with the 128-point staging ring (inside the sample buffer
+// whenever it fits) instead of the 512-point one: the points are what has to fit.
+template <int DOF>
+__host__ __device__ inline AmisSplitPlan plan_amis_split(int share, int M, int I) {
+    constexpr int T = AMIS_T_DENSE;
+    AmisSplitPlan s;
+    int off = (int)((sizeof(AmisHead<DOF, T>) + 127) / 128 * 128 / 4);
+    constexpr int ring = 2 * STAGE_FLOATS;
+    const bool alias = Dim<DOF>::POSE * M >= ring;
+    s.a.stage = off; if (!alias) off += ring;
+    s.a.pts = off; off += 16 * ((share + 1) / 2);
+    s.a.smp = off; off += Dim<DOF>::POSE * M;
+    if (alias) s.a.stage = s.a.smp;
+    s.a.cost = off; off += M;
+    s.a.logp = off; off += M;
+    s.a.cpart = off; off += (T / NT) * M;
+    s.xbuf = off; off += 2 * (M / I);
+    s.a.total_bytes = off * 4;
+    return s;
+}
+
+template <int DOF>
+__global__ void __launch_bounds__(AMIS_T_DENSE, 1) amis_split_kernel(const KArgs a, const int ctas) {
+    constexpr int T = AMIS_T_DENSE;
+    EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
+    AmisHead<DOF, T>& sh = *reinterpret_cast<AmisHead<DOF, T>*>(smem_raw);
+    float* dyn = reinterpret_cast<float*>(smem_raw);
+    constexpr int PD = Dim<DOF>::POSE;
+    const int M = a.p.mc_samples;
+    const int share = split_share(a.N, ctas);
+    const AmisSplitPlan pl = plan_amis_split<DOF>(share, M, a.p.mc_iter);
+    const int rank = cluster_rank(), obj = blockIdx.x / ctas, tid = threadIdx.x;
+    const int p0 = min(a.N, rank * share), p1 = min(a.N, p0 + share);
+    const int st = serial_thread<T>(a);
+    float* pts4 = dyn + pl.a.pts;
+    PH_DECL;
+    // Set-up as in amis_kernel, the loader taking this rank's range only.
+    // Ordering rule 1: the fused entry point may have parked the covariance in this object's sample rows
+    // (cov_stride = M * D).  Every rank reads it here, before its first cluster barrier (AMIS iteration 0), and rank 0
+    // writes the sample rows only after the AMIS loop: no rank can read a row that rank 0 has overwritten.
+    const int serial_warp = st >> 5;
+    if ((tid >> 5) == serial_warp) {
+        if (tid == st) {
+#pragma unroll
+            for (int i = 0; i < PD; ++i) sh.pose[i] = a.pose_opt_in[(size_t)obj * PD + i];
+#pragma unroll
+            for (int i = 0; i < DOF * DOF; ++i) sh.cov[i] = a.pose_cov_in[(size_t)obj * a.cov_stride + i];
+            if constexpr (DOF == 6) initial_fit6(sh.pose, sh.cov, a.p.acg_dispersion, sh.prop[0]);
+            else initial_fit4(sh.pose, sh.cov, a.p.amis_eps, sh.prop[0]);
+        }
+    } else {
+        LoaderT<CH> ld(a, sh.bar, dyn + pl.a.stage);
+        ld.template load_range<T>(obj, pts4, p0, p1, serial_warp);
+    }
+    __syncthreads();
+    // the rank's own bounding box: the sweep without the depth clamp gives the same bits as the clamped one, so which of
+    // the two a rank runs cannot change a result
+    point_box<T>(pts4, p1 - p0, sh.red + (T / 32) * 32, sh.box);
+    const Cam cam = load_cam(a, obj);
+    const float delta = __ldg(a.delta + obj);
+    PH_MARK(a, PH_LOAD);
+    const SplitCtx sc{dyn + pl.xbuf, rank, ctas, (p1 - p0 + 1) >> 1};
+    if constexpr (DOF == 6)
+        amis_phase6<T, true>(a, sh, pts4, dyn + pl.a.smp, dyn + pl.a.cost, dyn + pl.a.logp, dyn + pl.a.cpart, cam, delta, obj, sc);
+    else
+        amis_phase4<T, true>(a, sh, pts4, dyn + pl.a.smp, dyn + pl.a.cost, dyn + pl.a.logp, dyn + pl.a.cpart, cam, delta, obj, sc);
+#ifdef EPNP_SPLIT_AUDIT
+    cluster_sync();                         // every rank's state is final
+    for (int m = tid; m < M; m += T) {
+        const float* own[3] = {dyn + pl.a.cost + m, dyn + pl.a.logp + m, dyn + pl.a.smp + m * PD};
+        for (int k = 0; k < 2 + PD; ++k) {
+            const float* x = k < 2 ? own[k] : own[2] + (k - 2);
+            if (__float_as_uint(dsmem_ld(x, 0)) != __float_as_uint(*x)) SPLIT_AUDIT_MISMATCH();
+        }
+    }
+#endif
+    if (rank == 0) {
+        block_copy<T>(a.pose_samples + (size_t)obj * M * PD, dyn + pl.a.smp, M * PD);
+        SPLIT_AUDIT_STORES(tid == 0 ? M * PD : 0);
+    }
+    // Ordering rule 2: a CTA's shared memory disappears when it exits; this barrier keeps every CTA of the cluster alive
+    // until no rank can still read its partial costs of the last iteration.
+    cluster_sync();
 }
 
 }  // namespace

@@ -48,6 +48,17 @@ enum Phase { PH_LOAD = 0, PH_DRAW_SWEEP, PH_LOGP_OLD, PH_WEIGHTS, PH_REFIT_SUMS,
 #define PH_MARK(a_, which)
 #endif
 
+// Cluster audit, a build option of the test-only emulator (-DEPNP_SPLIT_AUDIT): the split kernels count, per cluster
+// rank, the output elements each rank stores and the elements of its AMIS state (costs, log-densities, samples) that
+// differ from rank 0's.  The shipped build compiles the macros away.
+#if defined(EPNP_SIMT_EMUL) && defined(SIMT_EMUL_HAS_CLUSTERS) && defined(EPNP_SPLIT_AUDIT)
+#define SPLIT_AUDIT_STORES(n) (simt::audit().stores[simt::cluster_rank()] += (n))
+#define SPLIT_AUDIT_MISMATCH() (++simt::audit().mismatches[simt::cluster_rank()])
+#else
+#define SPLIT_AUDIT_STORES(n)
+#define SPLIT_AUDIT_MISMATCH()
+#endif
+
 // ------------------------------------------------------------------------------------------------
 // PTX wrappers: mbarrier + 1-D TMA bulk copy; special-function units
 #if defined(EPNP_SIMT_EMUL)
@@ -65,6 +76,18 @@ inline void tma_load_1d(void* dst_smem, const void* src, uint32_t bytes, uint64_
     if ((*bar >> 32) == 0) *bar = (uint32_t)*bar + 1u;
 }
 inline void named_barrier(int id, int count) { simt::named_barrier(id, count); }
+#if defined(SIMT_EMUL_HAS_CLUSTERS)
+// thread-block clusters: the cluster emulator (tests/simt_cluster) runs a cluster's CTAs as one set of fibers
+inline int cluster_rank() { return simt::cluster_rank(); }
+inline void cluster_sync() { simt::cluster_sync(); }
+inline float dsmem_ld(const float* p, int rank) { return *simt::map_shared_rank(p, rank); }
+#else
+// the single-CTA emulator (tests/simt_emul) has no clusters: the split kernels compile, their launches are refused
+// (launch_cluster_per_object), so these never run
+inline int cluster_rank() { return 0; }
+inline void cluster_sync() { std::abort(); }
+inline float dsmem_ld(const float*, int) { std::abort(); }
+#endif
 struct FastRcp { float operator()(float x) const { return 1.0f / x; } };
 struct FastSqrt { float operator()(float x) const { return sqrtf(x); } };
 struct FastRsqrt { float operator()(float x) const { return 1.0f / sqrtf(x); } };
@@ -100,6 +123,25 @@ __device__ __forceinline__ void tma_load_1d(void* dst_smem, const void* src, uin
 // barrier `id` (1..15; 0 is __syncthreads) among `count` threads (a multiple of 32) of the CTA
 __device__ __forceinline__ void named_barrier(int id, int count) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
+// Thread-block clusters (sm_90): the CTA's rank in its cluster; a barrier of every thread of every CTA in the cluster
+// whose release / acquire orders shared-memory writes before it against distributed-shared-memory reads after it; a
+// read of the float at the same shared-memory offset as `p` in the CTA of rank `rank` (mapa + ld.shared::cluster).
+__device__ __forceinline__ int cluster_rank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return (int)r;
+}
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+__device__ __forceinline__ float dsmem_ld(const float* p, int rank) {
+    uint32_t remote;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(p)), "r"(rank));
+    float v;
+    asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(remote) : "memory");
+    return v;
 }
 
 struct FastRcp {
@@ -210,6 +252,58 @@ struct LoaderT {
             const float* gw = a.w2d + (size_t)obj * a.N * 2;
             for (int n = rank; n < a.N; n += nthr)
                 store_point_padded(pts, n, a.N, __ldg(g3 + 3 * n), __ldg(g3 + 3 * n + 1), __ldg(g3 + 3 * n + 2),
+                                   __ldg(g2 + 2 * n), __ldg(g2 + 2 * n + 1), __ldg(gw + 2 * n), __ldg(gw + 2 * n + 1));
+            sync();
+        }
+    }
+
+    // load_object for the points [p0, p1) of object `obj` only (a CTA of a cluster-split kernel): they become pair records
+    // 0, 1, ... of `pts`, an odd count padded like an odd N.  p0 is a multiple of 8 points, so with N % 4 == 0 every bulk
+    // copy starts on 16 bytes and moves a multiple of 16 bytes, as load_object's do.  Same participants and barriers.
+    __device__ void issue_range(int obj, int k, int p0, int p1) {
+        const int npts = min(CHUNK, p1 - p0 - k * CHUNK);
+        const size_t first = (size_t)obj * a.N + (size_t)p0 + (size_t)k * CHUNK;
+        float* dst = stage + (k & 1) * SLOT_FLOATS;
+        uint64_t* b = bar + (k & 1);
+        mbar_expect_tx(b, (uint32_t)npts * 28u);
+        tma_load_1d(dst, a.x3d + first * 3, (uint32_t)npts * 12u, b);
+        tma_load_1d(dst + CHUNK * 3, a.x2d + first * 2, (uint32_t)npts * 8u, b);
+        tma_load_1d(dst + CHUNK * 5, a.w2d + first * 2, (uint32_t)npts * 8u, b);
+    }
+    template <int T> __device__ void load_range(int obj, float* pts, int p0, int p1, int skip_warp = -1) {
+        const int tid = threadIdx.x;
+        const bool partial = skip_warp >= 0;
+        const int nthr = partial ? T - 32 : T;
+        const int rank = (partial && tid >= 32 * (skip_warp + 1)) ? tid - 32 : tid;
+        auto sync = [&]() { if (partial) named_barrier(1, T - 32); else __syncthreads(); };
+        const int cnt = p1 - p0, nchr = (cnt + CHUNK - 1) / CHUNK;
+        if (a.use_tma) {
+            if (rank == 0) {
+                mbar_init(bar + 0, 1);
+                mbar_init(bar + 1, 1);
+                fence_barrier_init();
+                if (nchr > 0) issue_range(obj, 0, p0, p1);
+                if (nchr > 1) issue_range(obj, 1, p0, p1);
+            }
+            sync();
+            for (int k = 0; k < nchr; ++k) {
+                const float* st = stage + (k & 1) * SLOT_FLOATS;
+                mbar_wait(bar + (k & 1), (uint32_t)((k >> 1) & 1));
+                const int npts = min(CHUNK, cnt - k * CHUNK);
+                for (int n = rank; n < npts; n += nthr) {
+                    const float2 uv = reinterpret_cast<const float2*>(st + CHUNK * 3)[n];
+                    const float2 w = reinterpret_cast<const float2*>(st + CHUNK * 5)[n];
+                    store_point_padded(pts, k * CHUNK + n, cnt, st[3 * n], st[3 * n + 1], st[3 * n + 2], uv.x, uv.y, w.x, w.y);
+                }
+                sync();
+                if (rank == 0 && k + 2 < nchr) { fence_proxy_async(); issue_range(obj, k + 2, p0, p1); }
+            }
+        } else {
+            const float* g3 = a.x3d + ((size_t)obj * a.N + p0) * 3;
+            const float* g2 = a.x2d + ((size_t)obj * a.N + p0) * 2;
+            const float* gw = a.w2d + ((size_t)obj * a.N + p0) * 2;
+            for (int n = rank; n < cnt; n += nthr)
+                store_point_padded(pts, n, cnt, __ldg(g3 + 3 * n), __ldg(g3 + 3 * n + 1), __ldg(g3 + 3 * n + 2),
                                    __ldg(g2 + 2 * n), __ldg(g2 + 2 * n + 1), __ldg(gw + 2 * n), __ldg(gw + 2 * n + 1));
             sync();
         }

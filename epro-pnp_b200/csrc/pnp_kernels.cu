@@ -11,6 +11,9 @@
 //   cost_kernel, evaluate_full_kernel, rslm_draw_kernel, rslm_kernel, cost_backward_kernel, gn_plus_backward_kernel, adaptive_delta_kernel,
 //   mc_epilogue_kernel, mc_lse_backward_kernel      the steps either side of the path (CTA per object).
 //   epnp_init_kernel (pnp_epnp.cuh)  EPnP initialiser with the confidence-quantile point selection, fp64, CTA per object.
+//   amis_split_kernel (pnp_amis.cuh), cost_split_kernel   the AMIS loop and the stacked-pose cost for objects whose points
+//                                    do not fit one SM: one thread-block CLUSTER of 2..8 CTAs per object, each holding a
+//                                    point range, partial costs summed over distributed shared memory.
 // No tensor cores: the only contraction is 6-deep, the work is FP32-pipe + MUFU bound (DESIGN.md).
 // Build options: EPNP_PHASE_TIMERS (profiling), EPNP_SIMT_EMUL (g++ build for the test-only CPU emulator).
 #include <cuda_runtime.h>
@@ -65,6 +68,61 @@ __global__ void __launch_bounds__(NT, 4) cost_kernel(const KArgs a) {
         for (int k = 0; k < PD; ++k) pose[k] = __ldg(a.poses + ((size_t)s * a.B + obj) * PD + k);
         a.cost_out[(size_t)s * a.B + obj] = pose_cost<DOF>(pts4, a.N, pose, cam, delta);
     }
+}
+
+// cost_kernel for objects too large for one SM: one cluster of `ctas` CTAs per object (grid = B * ctas), rank r holding
+// the points [r share, (r + 1) share) (split_share).  Every rank evaluates every pose on its own range, COST_SPLIT_TILE
+// poses at a time (one per thread); rank 0 adds the ranks' partial costs in rank order through distributed shared memory
+// and writes the result.  The result depends on ctas (the order of that sum), never on B.
+constexpr int COST_SPLIT_TILE = 512;
+struct CostSplitPlan { int stage, pts, xbuf, total_bytes; };
+__host__ __device__ inline CostSplitPlan plan_cost_split(int share) {
+    CostSplitPlan s;
+    int off = 128 / 4;                      // the two mbarriers of the staging ring, 128-byte aligned
+    s.stage = off; off += 2 * STAGE_FLOATS;
+    s.pts = off; off += 16 * ((share + 1) / 2);
+    s.xbuf = off; off += 2 * COST_SPLIT_TILE;
+    s.total_bytes = off * 4;
+    return s;
+}
+
+template <int DOF>
+__global__ void __launch_bounds__(COST_SPLIT_TILE, 1) cost_split_kernel(const KArgs a, const int ctas) {
+    EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
+    float* dyn = reinterpret_cast<float*>(smem_raw);
+    constexpr int PD = Dim<DOF>::POSE, TILE = COST_SPLIT_TILE;
+    const int share = split_share(a.N, ctas);
+    const CostSplitPlan pl = plan_cost_split(share);
+    const int rank = cluster_rank(), obj = blockIdx.x / ctas, tid = threadIdx.x;
+    const int p0 = min(a.N, rank * share), p1 = min(a.N, p0 + share);
+    float* pts4 = dyn + pl.pts;
+    Loader ld(a, reinterpret_cast<uint64_t*>(smem_raw), dyn + pl.stage);
+    ld.load_range<TILE>(obj, pts4, p0, p1);
+    const Cam cam = load_cam(a, obj);
+    const float delta = __ldg(a.delta + obj);
+    const int npair = (p1 - p0 + 1) >> 1;
+    for (int t = 0; t * TILE < a.S_eval; ++t) {
+        const int s = t * TILE + tid;
+        float part = 0.f;
+        if (s < a.S_eval) {
+            float pose[PD];
+#pragma unroll
+            for (int k = 0; k < PD; ++k) pose[k] = __ldg(a.poses + ((size_t)s * a.B + obj) * PD + k);
+            part = pose_cost_pairs<DOF>(pts4, 0, npair, pose, cam, delta);
+        }
+        // tiles alternate between the two halves of xbuf: one cluster barrier per tile (a half is written again two tiles
+        // later, after the next barrier, which rank 0 reaches only once its reads of this tile are done)
+        float* x = dyn + pl.xbuf + (t & 1) * TILE + tid;
+        *x = part;
+        cluster_sync();
+        if (rank == 0 && s < a.S_eval) {
+            float c = dsmem_ld(x, 0);
+            for (int r = 1; r < ctas; ++r) c += dsmem_ld(x, r);
+            a.cost_out[(size_t)s * a.B + obj] = c;
+            SPLIT_AUDIT_STORES(1);
+        }
+    }
+    cluster_sync();                         // no CTA leaves while rank 0 may still read its shared memory
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -989,6 +1047,77 @@ int launch_amis(KArgs& a, const PushArgs* push, cudaStream_t stream) {
     return launch_cta_per_object<NT>(amis_kernel<DOF, NT>, a, smem_bytes, stream, push ? *push : none);
 }
 
+// Cluster-split launches (amis_split_kernel, cost_split_kernel): `ctas` CTAs of T threads per object.  A device that
+// cannot co-schedule one such cluster (a MIG slice, or SMs taken by other work) gets EPNP_ERR_UNSUPPORTED; nothing is
+// launched then.  launch = false: only that check (run_lm_amis_split makes it before its LM launch).
+#if defined(EPNP_SIMT_EMUL) && !defined(SIMT_EMUL_HAS_CLUSTERS)
+// The single-CTA emulator build (tests/simt_emul) cannot run a cluster: every launch is refused.
+template <int T, class Kern>
+int launch_cluster_per_object(Kern, KArgs& a, int smem_bytes, int, cudaStream_t, bool = true) {
+    if (a.B == 0) return EPNP_OK;
+    if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
+    return EPNP_ERR_UNSUPPORTED;
+}
+#else
+template <int T, class Kern>
+int launch_cluster_per_object(Kern kern, KArgs& a, int smem_bytes, int ctas, cudaStream_t stream, bool launch = true) {
+    if (a.B == 0) return EPNP_OK;
+    if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+    if (e != cudaSuccess) return cuda_fail(e);
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (e != cudaSuccess) return cuda_fail(e);
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)ctas;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)a.B * (unsigned)ctas);
+    cfg.blockDim = dim3(T);
+    cfg.dynamicSmemBytes = (size_t)smem_bytes;
+    cfg.stream = stream;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int clusters = 0;
+    e = cudaOccupancyMaxActiveClusters(&clusters, kern, &cfg);
+    if (e != cudaSuccess) return cuda_fail(e);
+    if (clusters == 0) return EPNP_ERR_UNSUPPORTED;
+    if (!launch) return EPNP_OK;
+    a.use_tma = tma_ok(a);
+    const int rc = device_sms(&a.num_sms);
+    if (rc != EPNP_OK) return rc;
+    e = cudaLaunchKernelEx(&cfg, kern, a, ctas);
+    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+}
+#endif
+
+// Shared memory per CTA of a split launch; mc_samples = 0: the cost kernel.
+int split_smem_bytes(int dof, int N, int ctas, int mc_samples, int mc_iter) {
+    const int share = split_share(N, ctas);
+    if (mc_samples == 0) return plan_cost_split(share).total_bytes;
+    return dof == 6 ? plan_amis_split<6>(share, mc_samples, mc_iter).a.total_bytes
+                    : plan_amis_split<4>(share, mc_samples, mc_iter).a.total_bytes;
+}
+
+// The automatic cluster size: the smallest C >= 2 whose largest rank share fits, 0 when even 8 do not.  A function of
+// (N, M, I) only, so that an object's result does not depend on the batch it is solved in.
+int split_min_ctas(int dof, int N, int mc_samples, int mc_iter) {
+    for (int c = 2; c <= SPLIT_MAX_CTAS; ++c)
+        if ((size_t)split_smem_bytes(dof, N, c, mc_samples, mc_iter) <= SMEM_LIMIT) return c;
+    return 0;
+}
+
+// Cluster size of a split call: `requested` = 0 picks split_min_ctas; otherwise it must lie in [that minimum, 8].
+// Returns C > 0, or a (negative) error code.
+int split_ctas_for(int dof, int N, int mc_samples, int mc_iter, int requested) {
+    const int c_min = split_min_ctas(dof, N, mc_samples, mc_iter);
+    if (c_min == 0) return EPNP_ERR_TOO_MANY_POINTS;
+    if (requested == 0) return c_min;
+    if (requested < c_min || requested > SPLIT_MAX_CTAS) return EPNP_ERR_BAD_ARG;
+    return requested;
+}
+
 unsigned long long* g_prof_buffer = nullptr;     // set by epnp_debug_set_phase_buffer (profiling build)
 
 // Objects the device works on at once in the AMIS kernel: SMs x resident CTAs per SM.  Used by the host-buffer entry
@@ -1027,6 +1156,30 @@ int run_lm_amis(KArgs& a, const PushArgs* push, cudaStream_t stream) {
     a.pose_opt_in = a.pose_opt;
     a.pose_cov_in = a.pose_cov;
     return dof == 6 ? launch_amis<6>(a, push, stream) : launch_amis<4>(a, push, stream);
+}
+
+// run_lm_amis with the cluster-split AMIS kernel.  The LM half is the unstaged 8-warp LM kernel, which streams any N.
+int run_lm_amis_split(KArgs& a, int cluster_ctas, cudaStream_t stream) {
+    const int dof = a.p.dof, D = dof == 6 ? 7 : 4;
+    const int ctas = split_ctas_for(dof, a.N, a.p.mc_samples, a.p.mc_iter, cluster_ctas);
+    if (ctas < 0) return ctas;                  // before anything is launched
+    if (a.pose_cov) a.cov_stride = dof * dof;
+    else {
+        if (a.p.mc_samples * D < dof * dof) return EPNP_ERR_BAD_ARG;
+        a.pose_cov = a.pose_samples;
+        a.cov_stride = a.p.mc_samples * D;
+    }
+    const int smem_bytes = split_smem_bytes(dof, a.N, ctas, a.p.mc_samples, a.p.mc_iter);
+    // a device that cannot run the cluster gets no LM launch either
+    int rc = dof == 6 ? launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<6>, a, smem_bytes, ctas, stream, false)
+                      : launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<4>, a, smem_bytes, ctas, stream, false);
+    if (rc != EPNP_OK) return rc;
+    rc = dof == 6 ? launch_lm<6>(a, stream) : launch_lm<4>(a, stream);
+    if (rc != EPNP_OK) return rc;
+    a.pose_opt_in = a.pose_opt;
+    a.pose_cov_in = a.pose_cov;
+    return dof == 6 ? launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<6>, a, smem_bytes, ctas, stream)
+                    : launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<4>, a, smem_bytes, ctas, stream);
 }
 
 }  // namespace
@@ -1077,6 +1230,23 @@ int epnp_max_points(int dof, int mc_samples, int mc_iter) {
     return lo;
 }
 
+int epnp_split_ctas(int dof, int N, int mc_samples, int mc_iter) {
+    if ((dof != 4 && dof != 6) || N <= 0 || mc_samples < 0) return 0;
+    if (mc_samples > 0 && (mc_iter <= 0 || mc_iter > MAX_ITER || mc_samples % mc_iter != 0)) return 0;
+    return split_min_ctas(dof, N, mc_samples, mc_iter);
+}
+
+int epnp_max_points_split(int dof, int mc_samples, int mc_iter) {
+    if (epnp_split_ctas(dof, 8, mc_samples, mc_iter) == 0) return 0;
+    int lo = 8, hi = 1 << 16;               // rank shares (multiples of 8) that fit / do not fit
+    while (hi - lo > 8) {
+        const int mid = (lo + hi) / 2 / 8 * 8;
+        if ((size_t)split_smem_bytes(dof, SPLIT_MAX_CTAS * mid, SPLIT_MAX_CTAS, mc_samples, mc_iter) <= SMEM_LIMIT) lo = mid;
+        else hi = mid;
+    }
+    return SPLIT_MAX_CTAS * lo;
+}
+
 int epnp_adaptive_delta_f32(const float* x2d, const float* w2d, float relative_delta, float* delta, int B, int N,
                             void* stream) {
     if (!x2d || !w2d || !delta || B < 0 || N <= 0) return EPNP_ERR_BAD_ARG;
@@ -1125,6 +1295,25 @@ int epnp_evaluate_cost_f32(const float* x3d, const float* x2d, const float* w2d,
     if (S == 0) return EPNP_OK;
     if (dof == 6) return launch_cta_per_object(cost_kernel<6>, a, plan_obj<6>(N).total_bytes, (cudaStream_t)stream);
     return launch_cta_per_object(cost_kernel<4>, a, plan_obj<4>(N).total_bytes, (cudaStream_t)stream);
+}
+
+int epnp_evaluate_cost_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                 const float* lb, const float* ub, const float* delta, const float* poses, float* cost,
+                                 int S, int B, int N, int dof, float z_min, int cluster_ctas, void* stream) {
+    KArgs a{};
+    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
+    a.poses = poses; a.cost_out = cost; a.S_eval = S; a.B = B; a.N = N;
+    epnp_default_params(&a.p, dof);
+    a.p.z_min = z_min;
+    int rc = check_common(a);
+    if (rc != EPNP_OK) return rc;
+    if (!poses || !cost || S < 0) return EPNP_ERR_BAD_ARG;
+    const int ctas = split_ctas_for(dof, N, 0, 0, cluster_ctas);
+    if (ctas < 0) return ctas;
+    if (S == 0) return EPNP_OK;
+    const int smem_bytes = split_smem_bytes(dof, N, ctas, 0, 0);
+    if (dof == 6) return launch_cluster_per_object<COST_SPLIT_TILE>(cost_split_kernel<6>, a, smem_bytes, ctas, (cudaStream_t)stream);
+    return launch_cluster_per_object<COST_SPLIT_TILE>(cost_split_kernel<4>, a, smem_bytes, ctas, (cudaStream_t)stream);
 }
 
 int epnp_evaluate_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
@@ -1319,6 +1508,32 @@ int epnp_lm_amis_fused_f32(const float* x3d, const float* x2d, const float* w2d,
     const bool any = noise_normal || noise_chi2 || noise_rot, all = noise_normal && noise_chi2 && noise_rot;
     if (any && !all) return EPNP_ERR_BAD_ARG;
     return run_lm_amis(a, nullptr, (cudaStream_t)stream);
+}
+
+int epnp_lm_amis_fused_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                 const float* lb, const float* ub, const float* delta, const float* pose_init,
+                                 const float* noise_normal, const float* noise_chi2, const float* noise_rot,
+                                 uint64_t seed, uint32_t obj_offset,
+                                 float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus, float* cost_init,
+                                 float* pose_samples, float* logw, float* proposals,
+                                 int B, int N, const EpnpParams* p, int cluster_ctas, void* stream) {
+    if (!p) return EPNP_ERR_BAD_ARG;
+    KArgs a{};
+    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
+    a.pose_init = pose_init;
+    a.noise_n3 = noise_normal; a.noise_chi2 = noise_chi2; a.noise_rot = noise_rot;
+    a.seed = seed; a.obj_offset = obj_offset;
+    a.pose_opt = pose_opt; a.pose_cov = pose_cov; a.cost = cost; a.pose_plus = pose_opt_plus; a.cost_init = cost_init;
+    a.pose_samples = pose_samples; a.logw = logw; a.proposals = proposals; a.B = B; a.N = N; a.p = *p;
+    a.prof = g_prof_buffer;
+    int rc = check_common(a);
+    if (rc != EPNP_OK) return rc;
+    rc = check_amis_params(*p);
+    if (rc != EPNP_OK) return rc;
+    if (!pose_init || !pose_opt || !pose_samples || !logw || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
+    const bool any = noise_normal || noise_chi2 || noise_rot, all = noise_normal && noise_chi2 && noise_rot;
+    if (any && !all) return EPNP_ERR_BAD_ARG;
+    return run_lm_amis_split(a, cluster_ctas, (cudaStream_t)stream);
 }
 
 int epnp_lm_amis_fused_push_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,

@@ -10,12 +10,35 @@
                                     (a single evaluation, levenberg_marquardt.py:243-253 -- not the iterated path),
                                     or, with EPNP_NATIVE_GN_STEP=1, by the native kernel epnp_gn_plus_backward_f32
 
+Objects with more points than one SM holds (N above epnp_max_points: about 5,400 for the AMIS loop at M = 512, 7,000
+for the cost) take the cluster-split kernels (fused_forward, stacked_cost); at or below those limits nothing changes.
+The backward kernel streams the points, so it serves both.
+
 Gradients w.r.t. poses (pose_init / stacked hypotheses) are not provided: the reference's losses never use
 them (pose_init is the ground truth, lib/train.py:178-180), and asking for them raises.
 """
+import functools
+
 import torch
 
 from epropnp_b200 import native
+
+
+@functools.lru_cache(maxsize=None)
+def _resident_limit(dof, mc_samples, mc_iter):
+    return native.max_points(dof, mc_samples, mc_iter)
+
+
+def fused_forward(prob, pose_start, params, **kw):
+    """native.lm_amis_fused, or its cluster-split form when the objects' points do not fit one SM."""
+    split = prob.N > _resident_limit(params.dof, params.mc_samples, params.mc_iter)
+    return (native.lm_amis_fused_split if split else native.lm_amis_fused)(prob, pose_start, params, **kw)
+
+
+def stacked_cost(prob, poses, dof, z_min):
+    """native.evaluate_cost, or its cluster-split form when the objects' points do not fit one SM."""
+    split = prob.N > _resident_limit(dof, 0, 0)
+    return (native.evaluate_cost_split if split else native.evaluate_cost)(prob, poses, dof, z_min)
 
 
 def _delta_tensor(delta, ref):
@@ -44,12 +67,12 @@ class _MonteCarloForward(torch.autograd.Function):
     def forward(ctx, x3d, x2d, w2d, delta, cam_mats, lb, ub, pose_start, cost_init_pose, params, noise, seed,
                 want_cost, z_min):
         prob = native.Problem(x3d, x2d, w2d, cam_mats, lb, ub, delta)
-        out = native.lm_amis_fused(prob, pose_start, params, noise=noise, seed=seed, want_cost=want_cost,
-                                   want_cost_init=False, want_cov=False)
+        out = fused_forward(prob, pose_start, params, noise=noise, seed=seed, want_cost=want_cost,
+                            want_cost_init=False, want_cov=False)
         dof = params.dof
         cost_init = None
         if cost_init_pose is not None:
-            cost_init = native.evaluate_cost(prob, cost_init_pose.detach().unsqueeze(0), dof, z_min)[0]
+            cost_init = stacked_cost(prob, cost_init_pose.detach().unsqueeze(0), dof, z_min)[0]
         ctx.prob, ctx.dof, ctx.z_min = prob, dof, z_min
         ctx.samples = out["pose_samples"]
         ctx.cost_init_pose = None if cost_init_pose is None else cost_init_pose.detach()
@@ -87,7 +110,7 @@ class _CostOnly(torch.autograd.Function):
     def forward(ctx, x3d, x2d, w2d, delta, cam_mats, lb, ub, poses, dof, z_min):
         prob = native.Problem(x3d, x2d, w2d, cam_mats, lb, ub, delta)
         S = poses.shape[0]
-        cost = native.evaluate_cost(prob, poses, dof, z_min)                    # (S, B)
+        cost = stacked_cost(prob, poses, dof, z_min)                            # (S, B)
         ctx.prob, ctx.dof, ctx.z_min = prob, dof, z_min
         ctx.poses = poses.detach().transpose(0, 1).contiguous()                 # object-major (B, S, D)
         ctx.in_like = (x3d, x2d, w2d, delta if torch.is_tensor(delta) else None)

@@ -83,7 +83,8 @@ def evaluate_pnp(x3d, x2d, w2d, pose, camera, cost_fun,
     residual = cost = jac = None
     if not want_j and not want_r:
         if want_c:
-            cost = native.evaluate_cost(prob, pose.reshape(-1, B, pose.size(-1)), dof, camera.z_min).reshape(lead)
+            from .autograd import stacked_cost
+            cost = stacked_cost(prob, pose.reshape(-1, B, pose.size(-1)), dof, camera.z_min).reshape(lead)
     else:
         if pose.dim() != 2:
             # stacked hypotheses with Jacobians: treat every (hypothesis, object) as its own object

@@ -5,7 +5,10 @@
 first proposal, and all AMIS iterations (draw -> cost of every sample over all points -> mixture
 densities -> log-weights -> proposal refit) run per object inside one CTA with the correspondences
 resident in shared memory.  The reference's materialised (S, B, N, 3) intermediates, its per-iteration
-host Cholesky round trips and its ~10^3 op launches do not exist here.
+host Cholesky round trips and its ~10^3 op launches do not exist here.  Objects with more correspondences than one
+SM holds (N > epnp_max_points(dof, M, I), e.g. the 16,384 of a 128 x 128 coordinate map) run the same loop on a
+thread-block cluster of 2-8 CTAs (epnp_lm_amis_fused_split_f32); the RSLM initialiser still refuses those with its
+shared-memory error, so they need pose_init with force_init_solve=False.
 
 Layout note: the kernel writes object-major (B, M, D) / (B, M) buffers; the tuples returned below
 hold (M, B, D) / (M, B) *views* of them so reference call sites (softmax(dim=0), logsumexp(dim=0),
@@ -165,10 +168,11 @@ class EProPnPBase(torch.nn.Module, metaclass=ABCMeta):
                 params = self._amis_params(camera, cost_fun, fast_mode)
                 if not differentiable:
                     prob = native.Problem(x3d, x2d, w2d, camera.cam_mats, camera.lb, camera.ub, cost_fun.delta)
-                    out = native.lm_amis_fused(prob, start, params, noise=amis_noise, seed=seed, want_cost=with_cost,
-                                               want_plus=with_plus,
-                                               want_cost_init=(pose_init is not None and not needs_init_solver),
-                                               want_cov=False)
+                    from .autograd import fused_forward
+                    out = fused_forward(prob, start, params, noise=amis_noise, seed=seed, want_cost=with_cost,
+                                        want_plus=with_plus,
+                                        want_cost_init=(pose_init is not None and not needs_init_solver),
+                                        want_cov=False)
                     cast = lambda t: None if t is None else t.to(x3d.dtype)
                     pose_opt, cost, pose_opt_plus = cast(out["pose_opt"]), cast(out["cost"]), cast(out["pose_opt_plus"])
                     if cost_init is None:

@@ -40,6 +40,9 @@ _SIGNATURES = {
     "epnp_last_cuda_error": (ctypes.c_int, []),
     "epnp_default_params": (None, [ctypes.POINTER(EpnpParams), _I]),
     "epnp_max_points": (ctypes.c_int, [_I, _I, _I]),
+    "epnp_split_ctas": (ctypes.c_int, [_I, _I, _I, _I]),
+    "epnp_max_points_split": (ctypes.c_int, [_I, _I, _I]),
+    "epnp_evaluate_cost_split_f32": (ctypes.c_int, [_P] * 9 + [_I, _I, _I, _I, _F, _I, _P]),
     "epnp_adaptive_delta_f32": (ctypes.c_int, [_P, _P, _F, _P, _I, _I, _P]),
     "epnp_evaluate_cost_f32": (ctypes.c_int, [_P] * 9 + [_I, _I, _I, _I, _F, _P]),
     "epnp_evaluate_f32": (ctypes.c_int, [_P] * 11 + [_I, _I, _I, _I, _F, _F, _P]),
@@ -52,6 +55,8 @@ _SIGNATURES = {
                       + [_I, _I, ctypes.POINTER(EpnpParams), _P]),
     "epnp_lm_amis_fused_f32": (ctypes.c_int, [_P] * 11 + [ctypes.c_uint64, ctypes.c_uint32] + [_P] * 8
                                + [_I, _I, ctypes.POINTER(EpnpParams), _P]),
+    "epnp_lm_amis_fused_split_f32": (ctypes.c_int, [_P] * 11 + [ctypes.c_uint64, ctypes.c_uint32] + [_P] * 8
+                                     + [_I, _I, ctypes.POINTER(EpnpParams), _I, _P]),
     "epnp_lm_amis_fused_push_f32": (ctypes.c_int, [_P] * 8 + [ctypes.c_uint64, ctypes.c_uint32] + [_P] * 5
                                     + [_P, _P, _I, _I, _I, ctypes.POINTER(EpnpParams), _P]),
     "epnp_cost_backward_f32": (ctypes.c_int, [_P] * 7 + [_P, _P, _I, _P, _P, _I] + [_P] * 4 + [_I, _I, _I, _F, _P]),

@@ -98,6 +98,36 @@ def evaluate_cost(prob: Problem, poses, dof, z_min):
     return out
 
 
+def evaluate_cost_split(prob: Problem, poses, dof, z_min, cluster_ctas=0):
+    """evaluate_cost for objects larger than one SM holds (epnp_evaluate_cost_split_f32): one thread-block cluster of
+    split_ctas(dof, N) CTAs per object, or of `cluster_ctas` (that minimum .. 8).  poses (S, B, D) -> cost (S, B)."""
+    S = poses.shape[0]
+    _check_pose(poses, (S, prob.B), 7 if dof == 6 else 4, "poses")
+    poses = _f32c(poses)
+    out = prob.empty(S, prob.B)
+    with torch.cuda.device(prob.device):
+        check(lib().epnp_evaluate_cost_split_f32(*prob.common_ptrs(), ptr(poses), ptr(out), S, prob.B, prob.N, dof,
+                                                 ctypes.c_float(z_min), int(cluster_ctas), stream_ptr(prob.device)),
+              "epnp_evaluate_cost_split_f32")
+    return out
+
+
+def max_points(dof, mc_samples=0, mc_iter=0):
+    """Largest N the resident (one CTA per object) kernels take: the AMIS loop with mc_samples > 0, else the cost and
+    LM-scoring kernels."""
+    return int(lib().epnp_max_points(int(dof), int(mc_samples), int(mc_iter)))
+
+
+def max_points_split(dof, mc_samples=0, mc_iter=0):
+    """Largest N the cluster-split calls take (lm_amis_fused_split with mc_samples > 0, else evaluate_cost_split)."""
+    return int(lib().epnp_max_points_split(int(dof), int(mc_samples), int(mc_iter)))
+
+
+def split_ctas(dof, N, mc_samples=0, mc_iter=0):
+    """CTAs per object the split calls choose for N points (0: N is too large even for 8)."""
+    return int(lib().epnp_split_ctas(int(dof), int(N), int(mc_samples), int(mc_iter)))
+
+
 def evaluate_full(prob: Problem, pose, dof, z_min, huber_eps, clip_jac, want_residual, want_jac, want_cost):
     pose = _f32c(pose)
     B, N = prob.B, prob.N
@@ -250,6 +280,21 @@ def amis(prob: Problem, pose_opt, pose_cov, params, noise=None, seed=0, obj_offs
 
 def lm_amis_fused(prob: Problem, pose_init, params, noise=None, seed=0, obj_offset=0, want_cost=False,
                   want_plus=False, want_cost_init=True, want_proposals=False, want_cov=True):
+    return _fused("epnp_lm_amis_fused_f32", (), prob, pose_init, params, noise, seed, obj_offset, want_cost, want_plus,
+                  want_cost_init, want_proposals, want_cov)
+
+
+def lm_amis_fused_split(prob: Problem, pose_init, params, noise=None, seed=0, obj_offset=0, want_cost=False,
+                        want_plus=False, want_cost_init=True, want_proposals=False, want_cov=True, cluster_ctas=0):
+    """lm_amis_fused for objects larger than one SM holds (epnp_lm_amis_fused_split_f32): the AMIS loop of each object runs
+    on a thread-block cluster of split_ctas(dof, N, M, I) CTAs, or of `cluster_ctas` (that minimum .. 8).  Same outputs;
+    they depend on the cluster size, not on the batch."""
+    return _fused("epnp_lm_amis_fused_split_f32", (int(cluster_ctas),), prob, pose_init, params, noise, seed, obj_offset,
+                  want_cost, want_plus, want_cost_init, want_proposals, want_cov)
+
+
+def _fused(fn, extra, prob, pose_init, params, noise, seed, obj_offset, want_cost, want_plus, want_cost_init,
+           want_proposals, want_cov):
     D = 7 if params.dof == 6 else 4
     B, M, I = prob.B, params.mc_samples, params.mc_iter
     _check_pose(pose_init, (B,), D, "pose_init")
@@ -262,13 +307,12 @@ def lm_amis_fused(prob: Problem, pose_init, params, noise=None, seed=0, obj_offs
                proposals=prob.empty(B, I, 19) if want_proposals else None)
     p3, p2, p4, keep = _noise_ptrs(noise)
     with torch.cuda.device(prob.device):
-        check(lib().epnp_lm_amis_fused_f32(*prob.common_ptrs(), ptr(pose_init), p3, p2, p4,
-                                           ctypes.c_uint64(seed), ctypes.c_uint32(obj_offset),
-                                           ptr(out["pose_opt"]), ptr(out["pose_cov"]), ptr(out["cost"]),
-                                           ptr(out["pose_opt_plus"]), ptr(out["cost_init"]),
-                                           ptr(out["pose_samples"]), ptr(out["logw"]), ptr(out["proposals"]),
-                                           B, prob.N, ctypes.byref(params), stream_ptr(prob.device)),
-              "epnp_lm_amis_fused_f32")
+        check(getattr(lib(), fn)(*prob.common_ptrs(), ptr(pose_init), p3, p2, p4,
+                                 ctypes.c_uint64(seed), ctypes.c_uint32(obj_offset),
+                                 ptr(out["pose_opt"]), ptr(out["pose_cov"]), ptr(out["cost"]),
+                                 ptr(out["pose_opt_plus"]), ptr(out["cost_init"]),
+                                 ptr(out["pose_samples"]), ptr(out["logw"]), ptr(out["proposals"]),
+                                 B, prob.N, ctypes.byref(params), *extra, stream_ptr(prob.device)), fn)
     del keep
     return out
 
@@ -435,5 +479,5 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
     return out
 
 
-__all__ = ["Problem", "adaptive_delta", "cost_backward", "evaluate_cost", "evaluate_full", "lm_solve", "amis", "lm_amis_fused",
-           "lm_amis_fused_host", "lm_amis_fused_push", "fused_workspace_bytes", "rslm", "epnp_init", "gn_plus_backward", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]
+__all__ = ["Problem", "adaptive_delta", "cost_backward", "evaluate_cost", "evaluate_cost_split", "evaluate_full", "lm_solve",
+           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "fused_workspace_bytes", "rslm", "epnp_init", "gn_plus_backward", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

@@ -72,6 +72,17 @@ void        epnp_default_params(EpnpParams* p, int dof);
  * for the LM-only entry points. */
 int         epnp_max_points(int dof, int mc_samples, int mc_iter);
 
+/* Cluster-split entry points (epnp_lm_amis_fused_split_f32, epnp_evaluate_cost_split_f32): for N above
+ * epnp_max_points, one object is spread over a thread-block cluster of C = 2..8 CTAs on C SMs; CTA r holds the r-th
+ * range of ceil(N / C) points (rounded up to a multiple of 8) and the ranks' partial costs are added over distributed
+ * shared memory in rank order.
+ *   epnp_split_ctas: the C those calls choose automatically -- the smallest C >= 2 whose largest share fits one SM's
+ *     shared memory; 0 when even 8 CTAs are too few (or the arguments are invalid).  A function of (dof, N, M, I) only;
+ *     mc_samples = 0 gives the plan of epnp_evaluate_cost_split_f32.
+ *   epnp_max_points_split: the largest N any C can take (a multiple of 64). */
+int         epnp_split_ctas(int dof, int N, int mc_samples, int mc_iter);
+int         epnp_max_points_split(int dof, int mc_samples, int mc_iter);
+
 /* AdaptiveHuberPnPCost.set_param (cost_fun.py:123-126):
  *   delta[b] = mean(w2d[b]) * sqrt(sum_xy var_unbiased(x2d[b])) * relative_delta               */
 int epnp_adaptive_delta_f32(const float* x2d, const float* w2d, float relative_delta,
@@ -85,6 +96,15 @@ int epnp_evaluate_cost_f32(const float* x3d /*(B,N,3)*/, const float* x2d /*(B,N
                            const float* lb, const float* ub, const float* delta /*(B)*/,
                            const float* poses, float* cost,
                            int S, int B, int N, int dof, float z_min, void* stream);
+
+/* epnp_evaluate_cost_f32 for objects of up to epnp_max_points_split(dof, 0, 0) points: one cluster of C CTAs per
+ * object.  cluster_ctas = 0 takes C = epnp_split_ctas(dof, N, 0, 0); a caller may ask for any C from that minimum to
+ * 8 (EPNP_ERR_BAD_ARG outside it, EPNP_ERR_TOO_MANY_POINTS when no C fits).  The costs depend on C (it sets the order
+ * in which the ranks' partial sums are added) and never on B.  EPNP_ERR_UNSUPPORTED when the device cannot run one
+ * cluster of that size (cudaOccupancyMaxActiveClusters = 0, e.g. a MIG slice); nothing is launched then.          */
+int epnp_evaluate_cost_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                 const float* lb, const float* ub, const float* delta, const float* poses, float* cost,
+                                 int S, int B, int N, int dof, float z_min, int cluster_ctas, void* stream);
 
 /* evaluate_pnp(..., out_jacobian, out_residual, out_cost) at one pose per object (common.py:67-100,
  * camera.py:10-18,64-143, cost_fun.py:33-89): pose (B, D) ->
@@ -190,6 +210,24 @@ int epnp_lm_amis_fused_f32(const float* x3d, const float* x2d, const float* w2d,
                            float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus,
                            float* cost_init, float* pose_samples, float* logw, float* proposals,
                            int B, int N, const EpnpParams* p, void* stream);
+
+/* epnp_lm_amis_fused_f32 for objects of up to epnp_max_points_split(dof, M, I) points (the dense coordinate maps of
+ * out_res = 128 and beyond): the same arguments, outputs and noise conventions, plus cluster_ctas.  The LM half is
+ * epnp_lm_solve_f32's kernel, which takes any N; the AMIS loop runs on one cluster of C CTAs per object.  Every rank
+ * draws the same samples and, after exchanging its partial costs each iteration, holds the same costs and refits;
+ * rank 0 writes pose_samples, logw and proposals.  cluster_ctas = 0 takes C = epnp_split_ctas(dof, N, M, I); a caller
+ * may ask for any C from that minimum to 8 (EPNP_ERR_BAD_ARG outside it, EPNP_ERR_TOO_MANY_POINTS when no C fits).
+ * Results depend on C (the order in which the ranks' partial costs are added), never on B, the shard or obj_offset;
+ * they agree with epnp_lm_amis_fused_f32 to fp32 rounding, not bit for bit.  EPNP_ERR_UNSUPPORTED when the device
+ * cannot run one cluster of that size (cudaOccupancyMaxActiveClusters = 0, e.g. a MIG slice); the LM kernel is not
+ * launched either then.  There is no push or host-buffer form.                                                   */
+int epnp_lm_amis_fused_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                 const float* lb, const float* ub, const float* delta, const float* pose_init,
+                                 const float* noise_normal, const float* noise_chi2, const float* noise_rot,
+                                 uint64_t seed, uint32_t obj_offset,
+                                 float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus,
+                                 float* cost_init, float* pose_samples, float* logw, float* proposals,
+                                 int B, int N, const EpnpParams* p, int cluster_ctas, void* stream);
 
 /* Multi-GPU form of epnp_lm_amis_fused_f32 (one process per GPU, one NVLink / NVSwitch node): the solve AND the gather
  * of its small results in one kernel (the AMIS kernel).  Every CTA, when its object is finished, additionally stores the object's

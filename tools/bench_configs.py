@@ -209,6 +209,23 @@ def main():
             if host is not None:
                 row["host_cv2_ms"] = host
             out.append(row)
+    # objects larger than one SM holds: the cluster-split fused call at out_res = 128 (N = 16,384), and at N = 4,096 the
+    # split form on two CTAs next to the resident 512-thread kernel on the same inputs (the DSMEM experiment of DESIGN
+    # section 9.2: one object on two SMs against one object per SM)
+    if os.environ.get("EPNP_BENCH_SPLIT"):
+        card = dict(card=torch.cuda.get_device_name(dev), power_limit_w=power_limit(dev)) if dev.type == "cuda" else {}
+        B = b(256)
+        for N, ctas in ((16 if TOY else 16384, 0), (16 if TOY else 4096, 2)):
+            prob, p0 = setup(B, N, 0.1, grid2d=True)
+            p = native.default_params(6, lm_iter=3, fast_mode=1, z_min=0.01, mc_samples=m(512), mc_iter=2 if TOY else 4)
+            c = ctas or native.split_ctas(6, N, p.mc_samples, p.mc_iter)
+            row = dict(config=f"dense GN(3)+AMIS(4x128), N={N}, cluster-split", B=B, cluster_ctas=c, **card)
+            row["ms_split"] = timed(lambda: native.lm_amis_fused_split(prob, p0, p, seed=1, cluster_ctas=ctas), iters=10)
+            if N <= native.max_points(6, p.mc_samples, p.mc_iter):
+                row["ms_resident"] = timed(lambda: native.lm_amis_fused(prob, p0, p, seed=1), iters=10)
+            row["ms_lm_only"] = timed(lambda: native.lm_solve(prob, p0, p, want_cov=True), iters=10)
+            row["objects_per_s_split"] = B / row["ms_split"] * 1e3
+            out.append(row)
     for r in out:
         print(json.dumps(r))
 
