@@ -11,9 +11,10 @@
 //   cost_kernel, evaluate_full_kernel, rslm_draw_kernel, rslm_kernel, cost_backward_kernel, gn_plus_backward_kernel, adaptive_delta_kernel,
 //   mc_epilogue_kernel, mc_lse_backward_kernel      the steps either side of the path (CTA per object).
 //   epnp_init_kernel (pnp_epnp.cuh)  EPnP initialiser with the confidence-quantile point selection, fp64, CTA per object.
-//   amis_split_kernel (pnp_amis.cuh), cost_split_kernel   the AMIS loop and the stacked-pose cost for objects whose points
-//                                    do not fit one SM: one thread-block CLUSTER of 2..8 CTAs per object, each holding a
-//                                    point range, partial costs summed over distributed shared memory.
+//   amis_split_kernel (pnp_amis.cuh), cost_split_kernel, gn_plus_backward_split_kernel   the AMIS loop, the stacked-pose
+//                                    cost and the pose_opt_plus backward for objects whose points do not fit one SM: one
+//                                    thread-block CLUSTER of 2..8 CTAs per object, each holding a point range, partial
+//                                    sums added over distributed shared memory.
 // No tensor cores: the only contraction is 6-deep, the work is FP32-pipe + MUFU bound (DESIGN.md).
 // Build options: EPNP_PHASE_TIMERS (profiling), EPNP_SIMT_EMUL (g++ build for the test-only CPU emulator).
 #include <cuda_runtime.h>
@@ -504,6 +505,110 @@ __global__ void __launch_bounds__(NT, 2) gn_plus_backward_kernel(const GnBwArgs 
     }
     block_sum<1>(gd, sh.red, 0);
     if (tid == 0 && g.gdelta) g.gdelta[obj] = gd[0];
+}
+
+// gn_plus_backward_kernel for objects too large for one SM, on cost_split_kernel's plan: one cluster of `ctas` CTAs per
+// object (grid = B * ctas), rank r holding the points [r share, (r + 1) share) (split_share) in plan_cost_split(share),
+// with the head below in the 2 x COST_SPLIT_TILE floats the cost kernel uses for its partial costs -- so C and the point
+// limit are the cost kernel's.  Every rank evaluates the normal equations on its own range, reads every rank's partial
+// through distributed shared memory and adds them in rank order 0 .. ctas - 1: all ranks hold the same bits of H, g and
+// cost, and their serial threads form the same step and v (no broadcast).  Each rank then writes the gradient rows of
+// its own points; rank 0 adds the ranks' grad_delta partials in rank order.  The result depends on ctas, never on B.
+constexpr int GNBW_SPLIT_T = 512;
+template <int DOF> struct GnBwSplitHead {
+    float red[GNBW_SPLIT_T];            // eval_normal_eq / block_sum scratch
+    float part[32];                     // exchange slot 1: this rank's normal equations (NV floats)
+    float gdpart[4];                    // exchange slot 2: this rank's grad_delta partial
+    float ev[32];                       // the normal equations of the whole object
+    float pose[8];
+    float step[2 * DOF];                // step, v
+};
+static_assert(sizeof(GnBwSplitHead<6>) <= 2 * COST_SPLIT_TILE * sizeof(float), "the head must fit the partial-cost region");
+
+template <int DOF>
+__global__ void __launch_bounds__(GNBW_SPLIT_T, 1) gn_plus_backward_split_kernel(const GnBwArgs g, const int ctas) {
+    constexpr int T = GNBW_SPLIT_T;
+    const KArgs& a = g.k;
+    EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
+    float* dyn = reinterpret_cast<float*>(smem_raw);
+    constexpr int PD = Dim<DOF>::POSE, NA = Dim<DOF>::NA, NV = Dim<DOF>::NV;
+    const int share = split_share(a.N, ctas);
+    const CostSplitPlan pl = plan_cost_split(share);
+    GnBwSplitHead<DOF>& sh = *reinterpret_cast<GnBwSplitHead<DOF>*>(dyn + pl.xbuf);
+    const int rank = cluster_rank(), obj = blockIdx.x / ctas, tid = threadIdx.x;
+    const int p0 = min(a.N, rank * share), p1 = min(a.N, p0 + share), cnt = p1 - p0;
+    float* pts = dyn + pl.pts;
+    Loader ld(a, reinterpret_cast<uint64_t*>(smem_raw), dyn + pl.stage);
+    ld.load_range<T>(obj, pts, p0, p1);
+    const Cam cam = load_cam(a, obj);
+    const float delta = __ldg(a.delta + obj);
+    if (tid < PD) sh.pose[tid] = __ldg(a.poses + (size_t)obj * PD + tid);
+    __syncthreads();
+    // Pass 1.  Ordering rule 1: each exchange slot is written once, before the cluster barrier after which its peers
+    // read it, and never again -- the two slots are distinct, so no rank can overwrite what another is still reading.
+    eval_normal_eq<DOF, true, T>(pts, cnt, sh.pose, cam, delta, a.p.huber_eps, sh.red, sh.part);
+    cluster_sync();
+    if (tid < NV) {
+        float v = dsmem_ld(sh.part + tid, 0);
+        for (int r = 1; r < ctas; ++r) v += dsmem_ld(sh.part + tid, r);
+        sh.ev[tid] = v;
+    }
+    __syncthreads();
+    float* step = sh.step;              // [DOF]
+    float* vvec = sh.step + DOF;        // [DOF]
+    if (tid == 0) {                     // the resident kernel's serial sequence, on every rank
+        float add[DOF], st[DOF], sbar[DOF], vv[DOF], gout[PD], pose[PD];
+#pragma unroll
+        for (int i = 0; i < DOF; ++i) add[i] = a.p.eps;
+#pragma unroll
+        for (int i = 0; i < PD; ++i) { pose[i] = sh.pose[i]; gout[i] = __ldg(g.gplus + (size_t)obj * PD + i); }
+        damped_step_refined<DOF>(sh.ev, sh.ev + NA, add, st);
+        pose_add_backward<DOF>(pose, st, gout, sbar);
+        damped_step_refined<DOF>(sh.ev, sbar, add, vv);
+#pragma unroll
+        for (int i = 0; i < DOF; ++i) { step[i] = st[i]; vvec[i] = vv[i]; }
+    }
+    __syncthreads();
+    // Pass 2: thread <-> correspondence over this rank's range; every gradient row is written by the rank that owns it.
+    float R[9], t[3], sv[DOF], vv[DOF];
+    {
+        float ps[PD];
+#pragma unroll
+        for (int i = 0; i < PD; ++i) ps[i] = sh.pose[i];
+        pose_to_rot<DOF>(ps, R);
+        t[0] = ps[0]; t[1] = ps[1]; t[2] = ps[2];
+#pragma unroll
+        for (int i = 0; i < DOF; ++i) { sv[i] = step[i]; vv[i] = vvec[i]; }
+    }
+    float gd[1] = {0.f};
+    for (int n = tid; n < cnt; n += T) {
+        const float* q = pts + (n >> 1) * 16 + (n & 1);
+        float gr[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        gn_step_point_backward<DOF>(R, t, cam, delta, a.p.huber_eps, q[0], q[2], q[4], -q[6], -q[8], q[10], q[12], vv, sv, gr);
+        const size_t o = (size_t)obj * a.N + p0 + n;
+        if (g.gx3d) { g.gx3d[o * 3] = gr[0]; g.gx3d[o * 3 + 1] = gr[1]; g.gx3d[o * 3 + 2] = gr[2]; SPLIT_AUDIT_STORES(3); }
+        if (g.gx2d) { g.gx2d[o * 2] = gr[3]; g.gx2d[o * 2 + 1] = gr[4]; SPLIT_AUDIT_STORES(2); }
+        if (g.gw2d) { g.gw2d[o * 2] = gr[5]; g.gw2d[o * 2 + 1] = gr[6]; SPLIT_AUDIT_STORES(2); }
+        gd[0] += gr[7];
+    }
+    block_sum<1, T>(gd, sh.red, 0);
+    if (tid == 0) sh.gdpart[0] = gd[0];
+    cluster_sync();
+#ifdef EPNP_SPLIT_AUDIT
+    for (int k = tid; k < NV + 2 * DOF; k += T) {        // H, g, cost, step and v: rank 0's bits on every rank
+        const float* x = k < NV ? sh.ev + k : sh.step + (k - NV);
+        if (__float_as_uint(dsmem_ld(x, 0)) != __float_as_uint(*x)) SPLIT_AUDIT_MISMATCH();
+    }
+#endif
+    if (rank == 0 && tid == 0 && g.gdelta) {
+        float c = dsmem_ld(sh.gdpart, 0);
+        for (int r = 1; r < ctas; ++r) c += dsmem_ld(sh.gdpart, r);
+        g.gdelta[obj] = c;
+        SPLIT_AUDIT_STORES(1);
+    }
+    // Ordering rule 2: a CTA's shared memory disappears when it exits; this barrier keeps every CTA of the cluster alive
+    // until rank 0 has read its grad_delta partial.
+    cluster_sync();
 }
 
 // residual / Jacobian / cost written out per point (API parity with evaluate_pnp's out_* tensors)
@@ -1047,20 +1152,24 @@ int launch_amis(KArgs& a, const PushArgs* push, cudaStream_t stream) {
     return launch_cta_per_object<NT>(amis_kernel<DOF, NT>, a, smem_bytes, stream, push ? *push : none);
 }
 
-// Cluster-split launches (amis_split_kernel, cost_split_kernel): `ctas` CTAs of T threads per object.  A device that
+// Cluster-split launches (amis_split_kernel, cost_split_kernel, gn_plus_backward_split_kernel): `ctas` CTAs of T
+// threads per object; the kernel takes (Args, ctas), Args being KArgs or a struct holding one (kargs_of).  A device that
 // cannot co-schedule one such cluster (a MIG slice, or SMs taken by other work) gets EPNP_ERR_UNSUPPORTED; nothing is
 // launched then.  launch = false: only that check (run_lm_amis_split makes it before its LM launch).
+inline KArgs& kargs_of(KArgs& a) { return a; }
+inline KArgs& kargs_of(GnBwArgs& g) { return g.k; }
 #if defined(EPNP_SIMT_EMUL) && !defined(SIMT_EMUL_HAS_CLUSTERS)
 // The single-CTA emulator build (tests/simt_emul) cannot run a cluster: every launch is refused.
-template <int T, class Kern>
-int launch_cluster_per_object(Kern, KArgs& a, int smem_bytes, int, cudaStream_t, bool = true) {
-    if (a.B == 0) return EPNP_OK;
+template <int T, class Kern, class Args>
+int launch_cluster_per_object(Kern, Args& args, int smem_bytes, int, cudaStream_t, bool = true) {
+    if (kargs_of(args).B == 0) return EPNP_OK;
     if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
     return EPNP_ERR_UNSUPPORTED;
 }
 #else
-template <int T, class Kern>
-int launch_cluster_per_object(Kern kern, KArgs& a, int smem_bytes, int ctas, cudaStream_t stream, bool launch = true) {
+template <int T, class Kern, class Args>
+int launch_cluster_per_object(Kern kern, Args& args, int smem_bytes, int ctas, cudaStream_t stream, bool launch = true) {
+    KArgs& a = kargs_of(args);
     if (a.B == 0) return EPNP_OK;
     if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
@@ -1087,12 +1196,12 @@ int launch_cluster_per_object(Kern kern, KArgs& a, int smem_bytes, int ctas, cud
     a.use_tma = tma_ok(a);
     const int rc = device_sms(&a.num_sms);
     if (rc != EPNP_OK) return rc;
-    e = cudaLaunchKernelEx(&cfg, kern, a, ctas);
+    e = cudaLaunchKernelEx(&cfg, kern, args, ctas);
     return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
 }
 #endif
 
-// Shared memory per CTA of a split launch; mc_samples = 0: the cost kernel.
+// Shared memory per CTA of a split launch; mc_samples = 0: the cost and GN-plus backward kernels.
 int split_smem_bytes(int dof, int N, int ctas, int mc_samples, int mc_iter) {
     const int share = split_share(N, ctas);
     if (mc_samples == 0) return plan_cost_split(share).total_bytes;
@@ -1384,6 +1493,29 @@ int epnp_gn_plus_backward_f32(const float* x3d, const float* x2d, const float* w
     }
     e = cudaGetLastError();
     return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+}
+
+int epnp_gn_plus_backward_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                    const float* lb, const float* ub, const float* delta, const float* pose,
+                                    const float* grad_pose_plus, float* grad_x3d, float* grad_x2d, float* grad_w2d,
+                                    float* grad_delta, int B, int N, int dof, float z_min, float eps, float huber_eps,
+                                    int cluster_ctas, void* stream) {
+    GnBwArgs g{};
+    KArgs& a = g.k;
+    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
+    a.poses = pose; a.B = B; a.N = N;
+    epnp_default_params(&a.p, dof);
+    a.p.z_min = z_min; a.p.eps = eps; a.p.huber_eps = huber_eps;
+    g.gplus = grad_pose_plus; g.gx3d = grad_x3d; g.gx2d = grad_x2d; g.gw2d = grad_w2d; g.gdelta = grad_delta;
+    int rc = check_common(a);
+    if (rc != EPNP_OK) return rc;
+    if (!pose || !grad_pose_plus) return EPNP_ERR_BAD_ARG;
+    const int ctas = split_ctas_for(dof, N, 0, 0, cluster_ctas);
+    if (ctas < 0) return ctas;
+    const int smem_bytes = split_smem_bytes(dof, N, ctas, 0, 0);
+    if (dof == 6)
+        return launch_cluster_per_object<GNBW_SPLIT_T>(gn_plus_backward_split_kernel<6>, g, smem_bytes, ctas, (cudaStream_t)stream);
+    return launch_cluster_per_object<GNBW_SPLIT_T>(gn_plus_backward_split_kernel<4>, g, smem_bytes, ctas, (cudaStream_t)stream);
 }
 
 int epnp_rslm_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,

@@ -195,9 +195,10 @@ __global__ void __launch_bounds__(32 * WARPS) lm_warp_kernel(const KArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// CTA-wide evaluation over the packed pair records (gn_plus_backward_kernel): 128 threads stride over the pairs,
-// 28 partial sums per thread reduced by the transposed butterfly + one cross-warp pass; result in ev[0..NV).
-template <int DOF, bool CLIP>
+// CTA-wide evaluation over the packed pair records (gn_plus_backward_kernel and its cluster-split form): T threads stride
+// over the pairs, 28 partial sums per thread reduced by the transposed butterfly + one cross-warp pass in warp order
+// (sum_warp_partials); result in ev[0..NV).  `red` holds T floats.
+template <int DOF, bool CLIP, int T = NT>
 __device__ void eval_normal_eq(const float* pts, int N, const float* pose, const Cam& cam, float delta,
                                float huber_eps, float* red, float* ev) {
     constexpr int NV = Dim<DOF>::NV;
@@ -214,7 +215,7 @@ __device__ void eval_normal_eq(const float* pts, int N, const float* pose, const
     for (int i = 0; i < 32; ++i) acc[i] = 0.f;
     const float4* p4 = reinterpret_cast<const float4*>(pts);
     const int npair = (N + 1) >> 1;
-    for (int j = threadIdx.x; j < npair; j += NT) {
+    for (int j = threadIdx.x; j < npair; j += T) {
         const float4 q0 = p4[4 * j], q1 = p4[4 * j + 1], q2 = p4[4 * j + 2], q3 = p4[4 * j + 3];
         point_normal_eq<DOF, CLIP>(R, t, cam, delta, huber_eps, q0.x, q0.z, q1.x, -q1.z, -q2.x, q2.z, q3.x, acc);
         if (2 * j + 1 < N)
@@ -225,7 +226,7 @@ __device__ void eval_normal_eq(const float* pts, int N, const float* pose, const
     __syncthreads();
     if (threadIdx.x < NV) {
         const int j = threadIdx.x;
-        ev[j] = (red[j] + red[32 + j]) + (red[64 + j] + red[96 + j]);
+        ev[j] = sum_warp_partials<T>(red, j);
     }
     __syncthreads();
 }

@@ -11,8 +11,10 @@
                                     or, with EPNP_NATIVE_GN_STEP=1, by the native kernel epnp_gn_plus_backward_f32
 
 Objects with more points than one SM holds (N above epnp_max_points: about 5,400 for the AMIS loop at M = 512, 7,000
-for the cost) take the cluster-split kernels (fused_forward, stacked_cost); at or below those limits nothing changes.
-The backward kernel streams the points, so it serves both.
+for the cost and the pose_opt_plus backward) take the cluster-split kernels (fused_forward, stacked_cost,
+gn_plus_backward), up to epnp_max_points_split; at or below those limits nothing changes.  The Monte-Carlo cost
+backward kernel streams the points, so it serves both; the pose_opt_plus forward (the LM kernel) streams them too.
+RSLM init, EPnPSolver and the push / host-buffer entry points still refuse objects above the resident limits.
 
 Gradients w.r.t. poses (pose_init / stacked hypotheses) are not provided: the reference's losses never use
 them (pose_init is the ground truth, lib/train.py:178-180), and asking for them raises.
@@ -39,6 +41,13 @@ def stacked_cost(prob, poses, dof, z_min):
     """native.evaluate_cost, or its cluster-split form when the objects' points do not fit one SM."""
     split = prob.N > _resident_limit(dof, 0, 0)
     return (native.evaluate_cost_split if split else native.evaluate_cost)(prob, poses, dof, z_min)
+
+
+def gn_plus_backward(prob, pose, grad_pose_plus, dof, z_min, eps, huber_eps, want):
+    """native.gn_plus_backward, or its cluster-split form when the objects' points do not fit one SM."""
+    split = prob.N > _resident_limit(dof, 0, 0)
+    return (native.gn_plus_backward_split if split else native.gn_plus_backward)(
+        prob, pose, grad_pose_plus, dof, z_min, eps, huber_eps, want=want)
 
 
 def _delta_tensor(delta, ref):
@@ -153,7 +162,8 @@ def monte_carlo_autograd(x3d, x2d, w2d, camera, cost_fun, pose_start, pose_init,
 
 
 class _PosePlus(torch.autograd.Function):
-    """pose (+) gn_step(pose) with a native backward (epnp_gn_plus_backward_f32)."""
+    """pose (+) gn_step(pose) with a native backward (epnp_gn_plus_backward_f32, or its split form above the resident
+    limit)."""
 
     @staticmethod
     def forward(ctx, x3d, x2d, w2d, delta, cam_mats, lb, ub, pose, params, huber_eps):
@@ -169,7 +179,7 @@ class _PosePlus(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_plus):
         z_min, eps, huber_eps = ctx.consts
-        grads = native.gn_plus_backward(ctx.prob, ctx.pose, grad_plus, ctx.dof, z_min, eps, huber_eps, want=ctx.needs)
+        grads = gn_plus_backward(ctx.prob, ctx.pose, grad_plus, ctx.dof, z_min, eps, huber_eps, ctx.needs)
         g3, g2, gw, gd = _grads_to(ctx.in_like, grads)
         return g3, g2, gw, gd, None, None, None, None, None, None
 

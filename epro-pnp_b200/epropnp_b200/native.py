@@ -119,7 +119,8 @@ def max_points(dof, mc_samples=0, mc_iter=0):
 
 
 def max_points_split(dof, mc_samples=0, mc_iter=0):
-    """Largest N the cluster-split calls take (lm_amis_fused_split with mc_samples > 0, else evaluate_cost_split)."""
+    """Largest N the cluster-split calls take (lm_amis_fused_split with mc_samples > 0, else evaluate_cost_split and
+    gn_plus_backward_split)."""
     return int(lib().epnp_max_points_split(int(dof), int(mc_samples), int(mc_iter)))
 
 
@@ -240,6 +241,19 @@ def epnp_init(x3d, x2d, w2d, cam_mats, conf_quantile=0.8, want_n_sel=False):
 
 def gn_plus_backward(prob: Problem, pose, grad_pose_plus, dof, z_min, eps, huber_eps, want=(True, True, True, True)):
     """dL/d(x3d, x2d, w2d, delta) of pose_opt_plus = pose (+) gn_step(pose) (epnp_gn_plus_backward_f32)."""
+    return _gn_plus_backward("epnp_gn_plus_backward_f32", (), prob, pose, grad_pose_plus, dof, z_min, eps, huber_eps, want)
+
+
+def gn_plus_backward_split(prob: Problem, pose, grad_pose_plus, dof, z_min, eps, huber_eps, want=(True, True, True, True),
+                           cluster_ctas=0):
+    """gn_plus_backward for objects larger than one SM holds (epnp_gn_plus_backward_split_f32): one thread-block cluster of
+    split_ctas(dof, N) CTAs per object, or of `cluster_ctas` (that minimum .. 8).  Same outputs; they depend on the
+    cluster size, not on the batch."""
+    return _gn_plus_backward("epnp_gn_plus_backward_split_f32", (int(cluster_ctas),), prob, pose, grad_pose_plus, dof,
+                             z_min, eps, huber_eps, want)
+
+
+def _gn_plus_backward(fn, extra, prob, pose, grad_pose_plus, dof, z_min, eps, huber_eps, want):
     B, N = prob.B, prob.N
     pose, gp = _f32c(pose), _f32c(grad_pose_plus)
     g3 = prob.empty(B, N, 3) if want[0] else None
@@ -247,10 +261,9 @@ def gn_plus_backward(prob: Problem, pose, grad_pose_plus, dof, z_min, eps, huber
     gw = prob.empty(B, N, 2) if want[2] else None
     gd = prob.empty(B) if want[3] else None
     with torch.cuda.device(prob.device):
-        check(lib().epnp_gn_plus_backward_f32(*prob.common_ptrs(), ptr(pose), ptr(gp), ptr(g3), ptr(g2), ptr(gw), ptr(gd),
-                                              B, N, dof, ctypes.c_float(z_min), ctypes.c_float(eps),
-                                              ctypes.c_float(huber_eps), stream_ptr(prob.device)),
-              "epnp_gn_plus_backward_f32")
+        check(getattr(lib(), fn)(*prob.common_ptrs(), ptr(pose), ptr(gp), ptr(g3), ptr(g2), ptr(gw), ptr(gd),
+                                 B, N, dof, ctypes.c_float(z_min), ctypes.c_float(eps), ctypes.c_float(huber_eps),
+                                 *extra, stream_ptr(prob.device)), fn)
     return g3, g2, gw, gd
 
 
@@ -480,4 +493,4 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
 
 
 __all__ = ["Problem", "adaptive_delta", "cost_backward", "evaluate_cost", "evaluate_cost_split", "evaluate_full", "lm_solve",
-           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "fused_workspace_bytes", "rslm", "epnp_init", "gn_plus_backward", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]
+           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "fused_workspace_bytes", "rslm", "epnp_init", "gn_plus_backward", "gn_plus_backward_split", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

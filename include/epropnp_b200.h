@@ -78,7 +78,7 @@ int         epnp_max_points(int dof, int mc_samples, int mc_iter);
  * shared memory in rank order.
  *   epnp_split_ctas: the C those calls choose automatically -- the smallest C >= 2 whose largest share fits one SM's
  *     shared memory; 0 when even 8 CTAs are too few (or the arguments are invalid).  A function of (dof, N, M, I) only;
- *     mc_samples = 0 gives the plan of epnp_evaluate_cost_split_f32.
+ *     mc_samples = 0 gives the plan of both epnp_evaluate_cost_split_f32 and epnp_gn_plus_backward_split_f32.
  *   epnp_max_points_split: the largest N any C can take (a multiple of 64). */
 int         epnp_split_ctas(int dof, int N, int mc_samples, int mc_iter);
 int         epnp_max_points_split(int dof, int mc_samples, int mc_iter);
@@ -124,6 +124,19 @@ int epnp_gn_plus_backward_f32(const float* x3d, const float* x2d, const float* w
                               const float* grad_pose_plus, float* grad_x3d, float* grad_x2d, float* grad_w2d,
                               float* grad_delta, int B, int N, int dof, float z_min, float eps, float huber_eps,
                               void* stream);
+
+/* epnp_gn_plus_backward_f32 for objects of up to epnp_max_points_split(dof, 0, 0) points (the dense coordinate maps of
+ * training): one cluster of C CTAs per object, each rank holding one range of the points; the ranks' normal equations
+ * and grad_delta partials are added over distributed shared memory in rank order, and each rank writes the gradient rows
+ * of its own points.  cluster_ctas = 0 takes C = epnp_split_ctas(dof, N, 0, 0); a caller may ask for any C from that
+ * minimum to 8 (EPNP_ERR_BAD_ARG outside it, EPNP_ERR_TOO_MANY_POINTS when no C fits).  The gradients depend on C (the
+ * order of the sums over ranks) and never on B or the object's position in the batch.  EPNP_ERR_UNSUPPORTED when the
+ * device cannot run one cluster of that size; nothing is launched then.  Each output stays optional.               */
+int epnp_gn_plus_backward_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                    const float* lb, const float* ub, const float* delta, const float* pose,
+                                    const float* grad_pose_plus, float* grad_x3d, float* grad_x2d, float* grad_w2d,
+                                    float* grad_delta, int B, int N, int dof, float z_min, float eps, float huber_eps,
+                                    int cluster_ctas, void* stream);
 
 /* Everything RSLMSolver.solve does before its solves (levenberg_marquardt.py:283-324) in one launch:
  *   the centre-based translation guess (center_based_init, :283-298: mean ray direction times the ratio of the 3D spread

@@ -226,6 +226,44 @@ def main():
             row["ms_lm_only"] = timed(lambda: native.lm_solve(prob, p0, p, want_cov=True), iters=10)
             row["objects_per_s_split"] = B / row["ms_split"] * 1e3
             out.append(row)
+        # the derivative-regularisation term of training on the same objects: pose_opt_plus forward + backward at
+        # N = 16,384 with the native split backward next to the torch composite (EPNP_NATIVE_GN_STEP=0), the only other
+        # path that runs at that N, at the reference's training batch (32) and at 256; and at N = 4,096 the split
+        # backward on two CTAs next to the resident kernel
+        from epropnp import autograd as ag
+        from epropnp.camera import PerspectiveCamera
+        from epropnp.cost_fun import AdaptiveHuberPnPCost
+        from epropnp.levenberg_marquardt import LMSolver
+        N = 16 if TOY else 16384
+        for B in bs(32, 256):
+            pc = {k: v.to(dev) for k, v in make_problem(B, N, seed=5, grid2d=True).items()}
+            x3d, w2d = pc["x3d"].clone().requires_grad_(True), pc["w2d"].clone().requires_grad_(True)
+            camera = PerspectiveCamera(cam_mats=pc["cam_mats"], z_min=0.01)
+            cost_fun = AdaptiveHuberPnPCost(relative_delta=0.1)
+            solver = LMSolver(dof=6, num_iter=3)
+            row = dict(config=f"pose_opt_plus forward + backward, N={N}", B=B, cluster_ctas=native.split_ctas(6, N), **card)
+
+            def step():
+                x3d.grad = w2d.grad = None
+                cost_fun.set_param(pc["x2d"], w2d)
+                ag.pose_plus_autograd(solver, x3d, pc["x2d"], w2d, pc["pose_init"], camera, cost_fun).square().sum().backward()
+            for flag, key in (("0", "ms_composite"), ("1", "ms_native")):
+                os.environ["EPNP_NATIVE_GN_STEP"] = flag
+                row[key] = timed(step, iters=10)
+            os.environ["EPNP_NATIVE_GN_STEP"] = "1"
+            prob, p0 = setup(B, N, 0.1, grid2d=True)
+            gp = torch.randn(B, 7, device=dev)
+            row["ms_backward_split"] = timed(lambda: native.gn_plus_backward_split(prob, p0, gp, 6, 0.01, 1e-5, 1e-10),
+                                             iters=10)
+            out.append(row)
+        B, N = b(256), 16 if TOY else 4096
+        prob, p0 = setup(B, N, 0.1, grid2d=True)
+        gp = torch.randn(B, 7, device=dev)
+        row = dict(config=f"pose_opt_plus backward, N={N}, cluster-split", B=B, cluster_ctas=2, **card)
+        row["ms_split"] = timed(lambda: native.gn_plus_backward_split(prob, p0, gp, 6, 0.01, 1e-5, 1e-10, cluster_ctas=2),
+                                iters=10)
+        row["ms_resident"] = timed(lambda: native.gn_plus_backward(prob, p0, gp, 6, 0.01, 1e-5, 1e-10), iters=10)
+        out.append(row)
     for r in out:
         print(json.dumps(r))
 
