@@ -4,8 +4,11 @@
 // w2d.mean(-1), keep conf >= np.quantile(conf, q), cv2.solvePnP(..., flags=SOLVEPNP_EPNP), Rodrigues -> quaternion.
 //
 // Like pnp_math.cuh, everything is __host__ __device__ and allocation-free, so tests/epnp_host.cpp builds the same code
-// with g++.  The kernel (pnp_kernels.cu, epnp_init_kernel) supplies the parallel parts: the order statistics of the
-// confidences, the compaction of the selected points and the per-point sums; the serial parts are here.
+// with g++.  The kernels (pnp_kernels.cu, epnp_init_kernel and epnp_init_split_kernel) supply the parallel parts: the
+// order statistics of the confidences, the compaction of the selected points and the per-point sums; the serial parts
+// are here.  The out-of-line functions (EPNP_HD_COLD) take a SITE tag: ptxas fits an out-of-line function to all of
+// its callers, so each kernel instantiates its own copies (epnp_init_kernel SITE 0, epnp_init_split_kernel SITE 1) and
+// a new caller cannot change an existing kernel's code.
 //
 // Conventions, fixed by experiment against cv2 (OpenCV 4.13), which the reference calls:
 //   * pixel coordinates with fu = K[0][0], fv = K[1][1], uc = K[0][2], vc = K[1][2]: with fu != fv the normalised-
@@ -89,7 +92,7 @@ EPNP_HD double dot3(const double* a, const double* b) { return a[0] * b[0] + a[1
 // they are mutually orthogonal (at most max(n, 30) sweeps, so a NaN input ends too), then sorted by descending norm
 // (stable) and normalised.  On return A's rows are the left singular vectors and w the singular values.  Each rotation
 // is the one of angle at most pi/4 that orthogonalises the pair -- this choice is what fixes the vectors' signs.
-template <int n>
+template <int n, int SITE = 0>
 EPNP_HD_COLD void jacobi_svd_rows(double (&A)[n][n], double (&w)[n]) {
     const double tol = 10.0 * 2.220446049250313e-16;
     for (int i = 0; i < n; ++i) {
@@ -154,7 +157,7 @@ EPNP_HD_COLD void jacobi_svd_rows(double (&A)[n][n], double (&w)[n]) {
 
 // Least-squares solution of the M x N system A x = b (M >= N) by Householder QR.  A and b are overwritten.  A column
 // that is zero below the diagonal gives x = 0 in that component.
-template <int M, int N>
+template <int M, int N, int SITE = 0>
 EPNP_HD_COLD void lstsq(double (&A)[M][N], double (&b)[M], double (&x)[N]) {
     for (int k = 0; k < N; ++k) {
         double nrm = 0.0;
@@ -205,10 +208,11 @@ struct Control {
 };
 
 // c0: centroid of the n selected points; S: their centred scatter (xx xy xz yy yz zz)
+template <int SITE = 0>
 EPNP_HD_COLD void control_points(const double (&c0)[3], const double (&S)[6], int n, Control& cp) {
     double A[3][3] = {{S[0], S[1], S[2]}, {S[1], S[3], S[4]}, {S[2], S[4], S[5]}};
     double w[3];
-    jacobi_svd_rows<3>(A, w);
+    jacobi_svd_rows<3, SITE>(A, w);
     for (int j = 0; j < 3; ++j) cp.c[0][j] = c0[j];
     for (int i = 0; i < 3; ++i) {
         const double k = sqrt(w[i] / n);
@@ -269,6 +273,7 @@ EPNP_HD void quat_rot(const double (&q)[4], double (&R)[9]) {
 // R, t from the camera-frame control points ccs: pc_i = sum_j alpha_ij ccs_j.  Horn: q maximises q^T N(S) q with
 // S_ab = sum_i (p_i - c_0)_a pc_{i,b}; N is shifted by a Gershgorin bound so that its top eigenvector is its top
 // singular vector.  det S < 0 (the best orthogonal fit is a reflection): q of diag(-1, -1, 1) Horn(-S), see the top.
+template <int SITE = 0>
 EPNP_HD_COLD void procrustes(const double (&ccs)[4][3], const double (&acc)[NSUM], int n, const double (&c0)[3], Candidate& out) {
     double S[3][3], pc0[3];
     for (int a = 0; a < 3; ++a) {
@@ -300,7 +305,7 @@ EPNP_HD_COLD void procrustes(const double (&ccs)[4][3], const double (&acc)[NSUM
     }
     for (int i = 0; i < 4; ++i) Nm[i][i] += shift;
     double w[4];
-    jacobi_svd_rows<4>(Nm, w);
+    jacobi_svd_rows<4, SITE>(Nm, w);
     double q[4] = {Nm[0][0], Nm[0][1], Nm[0][2], Nm[0][3]};
     if (reflect) {                      // (0, 0, 0, 1) * q: a half turn about z after Horn(-S)
         const double h[4] = {-q[3], -q[2], q[1], q[0]};
@@ -314,6 +319,7 @@ EPNP_HD_COLD void procrustes(const double (&ccs)[4][3], const double (&acc)[NSUM
 }
 
 // The three candidates from the per-point sums.  al_first: barycentric coordinates of the first selected point.
+template <int SITE = 0>
 EPNP_HD_COLD void solve_candidates(const double (&acc)[NSUM], const Control& cp, const Intrinsics& in, const double (&al_first)[4],
                                    int n, Candidate (&cand)[3]) {
     // M^T M (12 x 12), block (j, k) from the factored sums
@@ -335,7 +341,7 @@ EPNP_HD_COLD void solve_candidates(const double (&acc)[NSUM], const Control& cp,
         }
     }
     double w[12];
-    jacobi_svd_rows<12>(A, w);
+    jacobi_svd_rows<12, SITE>(A, w);
     // null-space basis: v_i = the singular vector of the (i+1)-th smallest singular value
     const double* v[4] = {A[11], A[10], A[9], A[8]};
     // L (6 x 10) and rho over the control-point pairs (0,1) (0,2) (0,3) (1,2) (1,3) (2,3); betas ordered
@@ -364,7 +370,7 @@ EPNP_HD_COLD void solve_candidates(const double (&acc)[NSUM], const Control& cp,
     {   // N = 1 (paper): [b11 b12 b13 b14] from columns 0 1 3 6
         double M4[6][4], r4[6], x[4];
         for (int r = 0; r < 6; ++r) { M4[r][0] = L[r][0]; M4[r][1] = L[r][1]; M4[r][2] = L[r][3]; M4[r][3] = L[r][6]; r4[r] = rho[r]; }
-        lstsq<6, 4>(M4, r4, x);
+        lstsq<6, 4, SITE>(M4, r4, x);
         const double b0 = sqrt(fabs(x[0])), sg = x[0] < 0.0 ? -1.0 : 1.0;
         betas[0][0] = b0;
         for (int i = 1; i < 4; ++i) betas[0][i] = sg * x[i] / b0;
@@ -372,7 +378,7 @@ EPNP_HD_COLD void solve_candidates(const double (&acc)[NSUM], const Control& cp,
     {   // N = 2: [b11 b12 b22] from columns 0 1 2
         double M3[6][3], r3[6], x[3];
         for (int r = 0; r < 6; ++r) { for (int c = 0; c < 3; ++c) M3[r][c] = L[r][c]; r3[r] = rho[r]; }
-        lstsq<6, 3>(M3, r3, x);
+        lstsq<6, 3, SITE>(M3, r3, x);
         double b0, b1;
         if (x[0] < 0.0) { b0 = sqrt(-x[0]); b1 = x[2] < 0.0 ? sqrt(-x[2]) : 0.0; }
         else { b0 = sqrt(x[0]); b1 = x[2] > 0.0 ? sqrt(x[2]) : 0.0; }
@@ -382,7 +388,7 @@ EPNP_HD_COLD void solve_candidates(const double (&acc)[NSUM], const Control& cp,
     {   // N = 3: [b11 b12 b22 b13 b23] from columns 0..4
         double M5[6][5], r5[6], x[5];
         for (int r = 0; r < 6; ++r) { for (int c = 0; c < 5; ++c) M5[r][c] = L[r][c]; r5[r] = rho[r]; }
-        lstsq<6, 5>(M5, r5, x);
+        lstsq<6, 5, SITE>(M5, r5, x);
         double b0, b1;
         if (x[0] < 0.0) { b0 = sqrt(-x[0]); b1 = x[2] < 0.0 ? sqrt(-x[2]) : 0.0; }
         else { b0 = sqrt(x[0]); b1 = x[2] > 0.0 ? sqrt(x[2]) : 0.0; }
@@ -404,7 +410,7 @@ EPNP_HD_COLD void solve_candidates(const double (&acc)[NSUM], const Control& cp,
                 for (int m = 0; m < 10; ++m) s += l[m] * be[bi[m]] * be[bj[m]];
                 res[r] = rho[r] - s;
             }
-            lstsq<6, 4>(J, res, dx);
+            lstsq<6, 4, SITE>(J, res, dx);
             for (int i = 0; i < 4; ++i) be[i] += dx[i];
         }
         double ccs[4][3];
@@ -415,7 +421,7 @@ EPNP_HD_COLD void solve_candidates(const double (&acc)[NSUM], const Control& cp,
         if (z0 < 0.0)
             for (int j = 0; j < 4; ++j)
                 for (int k = 0; k < 3; ++k) ccs[j][k] = -ccs[j][k];
-        procrustes(ccs, acc, n, cp.c[0], cand[c]);
+        procrustes<SITE>(ccs, acc, n, cp.c[0], cand[c]);
     }
 }
 

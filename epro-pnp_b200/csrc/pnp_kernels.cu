@@ -11,10 +11,10 @@
 //   cost_kernel, evaluate_full_kernel, rslm_draw_kernel, rslm_kernel, cost_backward_kernel, gn_plus_backward_kernel, adaptive_delta_kernel,
 //   mc_epilogue_kernel, mc_lse_backward_kernel      the steps either side of the path (CTA per object).
 //   epnp_init_kernel (pnp_epnp.cuh)  EPnP initialiser with the confidence-quantile point selection, fp64, CTA per object.
-//   amis_split_kernel (pnp_amis.cuh), cost_split_kernel, gn_plus_backward_split_kernel   the AMIS loop, the stacked-pose
-//                                    cost and the pose_opt_plus backward for objects whose points do not fit one SM: one
-//                                    thread-block CLUSTER of 2..8 CTAs per object, each holding a point range, partial
-//                                    sums added over distributed shared memory.
+//   amis_split_kernel (pnp_amis.cuh), cost_split_kernel, gn_plus_backward_split_kernel, epnp_init_split_kernel   the AMIS
+//                                    loop, the stacked-pose cost, the pose_opt_plus backward and the EPnP initialiser for
+//                                    objects whose points do not fit one SM: one thread-block CLUSTER of 2..8 CTAs per
+//                                    object, each holding a point range, partial sums added over distributed shared memory.
 // No tensor cores: the only contraction is 6-deep, the work is FP32-pipe + MUFU bound (DESIGN.md).
 // Build options: EPNP_PHASE_TIMERS (profiling), EPNP_SIMT_EMUL (g++ build for the test-only CPU emulator).
 #include <cuda_runtime.h>
@@ -922,9 +922,11 @@ __device__ __forceinline__ double shfl_xor_f64(double v, int o) {
     return v;
 }
 
-// block-wide fp64 sums of K values per thread (NT threads); every thread gets the totals, partials added in warp order
-template <int K>
+// block-wide fp64 sums of K values per thread (T threads, whole groups of four warps); every thread gets the totals,
+// warp partials added as sum_warp_partials adds them
+template <int K, int T = NT>
 __device__ __forceinline__ void block_sum_f64(double (&v)[K], double* red) {
+    static_assert(T % 128 == 0, "block_sum_f64: whole groups of four warps");
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
     for (int k = 0; k < K; ++k) {
@@ -937,7 +939,12 @@ __device__ __forceinline__ void block_sum_f64(double (&v)[K], double* red) {
     }
     __syncthreads();
 #pragma unroll
-    for (int k = 0; k < K; ++k) v[k] = (red[k] + red[K + k]) + (red[2 * K + k] + red[3 * K + k]);
+    for (int k = 0; k < K; ++k) {
+        v[k] = (red[k] + red[K + k]) + (red[2 * K + k] + red[3 * K + k]);
+#pragma unroll
+        for (int w = 4; w < T / 32; w += 4)
+            v[k] += (red[w * K + k] + red[(w + 1) * K + k]) + (red[(w + 2) * K + k] + red[(w + 3) * K + k]);
+    }
     __syncthreads();                    // red is free again
 }
 
@@ -1053,6 +1060,220 @@ __global__ void __launch_bounds__(NT) epnp_init_kernel(const EpnpInitArgs a) {
     }
 }
 
+// epnp_init_kernel for objects too large for one SM (epnp_epnp_init_split_f32): one cluster of `ctas` CTAs per object
+// (grid = B * ctas), rank r holding the points [r share, (r + 1) share) (split_share).  Each rank runs the resident
+// kernel's steps over its own range.  What crosses ranks goes through an exchange slot in the rank's shared memory and
+// one cluster barrier, after which every rank adds the ranks' values in rank order 0 .. ctas - 1:
+//   1. the NaN counts: an object with a NaN confidence anywhere takes the NaN path on every rank;
+//   2. per radix-select pass, the two counts over the global N (integers, exact in fp32: the threshold and the kept set
+//      are np.quantile's over all N points whatever ctas is);
+//   3. the kept counts: n, and the lowest rank holding a kept point.  That rank's first kept point is the object's first
+//      in index order, which fixes the sign of the camera-frame control points; every rank reads it from there;
+//   4. the fp64 partials of the centroid, the scatter, the 56 EPnP sums and the three reprojection errors.
+// So every rank holds the same bits and runs control_points / solve_candidates itself (no broadcast); rank 0 alone
+// writes pose and n_sel.  The result depends on ctas (the order of the fp64 sums over ranks), never on B.
+// Ordering: each exchange slot is written once, before the cluster barrier after which its peers read it -- except the
+// radix counts, whose two halves alternate by pass: a half is written again two passes later, past the next barrier,
+// which no rank reaches before its reads of that half are done.  Every rank passes the same barriers whatever its range
+// holds (empty, nothing kept, the NaN path), and a last one keeps each CTA resident while its peers may read it.
+// Shared memory, all dynamic (a peer can only address the dynamic window): the head below, then the keys (share) and
+// the kept points (5 share floats), i.e. 24 share bytes + the head (about 8.5 KB).  cost_split_kernel takes
+// 32 share + 11 KB at the same share (plan_cost_split), and the static_assert below keeps the head within that margin,
+// so every C the cost kernel's plan allows (split_ctas_for(6, N, 0, 0)) fits this kernel too.
+constexpr int EPNP_SPLIT_T = 256;
+struct EpnpSplitAgreed {                // what every rank ends with, bit for bit (the audit build compares it)
+    epnp::Control cp;
+    epnp::Candidate cand[3];
+    double c0[3], S[6], acc[epnp::NSUM], err[3];    // sums over the whole object
+    float thr;
+    int n, first, best;                             // kept points, lowest rank keeping one, winning candidate
+};
+struct EpnpSplitHead {
+    double red[EPNP_SPLIT_T / 32 * epnp::NSUM];     // block_sum_f64 scratch
+    double xc0[3], xS[6], xacc[epnp::NSUM], xerr[3]; // exchange slots: this rank's fp64 partials
+    EpnpSplitAgreed g;
+    float fred[2 * EPNP_SPLIT_T];                   // block_sum scratch, two halves
+    float xsel[2][2];                               // exchange slot: radix counts, half = pass parity
+    float xnan, xkept;                              // exchange slots: NaN count, kept count
+    int counts[EPNP_SPLIT_T];                       // kept points per thread (compaction)
+};
+constexpr int EPNP_SPLIT_HEAD_BYTES = (int)((sizeof(EpnpSplitHead) + 127) / 128 * 128);
+static_assert(EPNP_SPLIT_HEAD_BYTES <= 128 + (2 * STAGE_FLOATS + 2 * COST_SPLIT_TILE) * 4,
+              "the EPnP split image must not exceed the cost split image at any share");
+__host__ __device__ inline int epnp_split_smem_bytes(int share) { return EPNP_SPLIT_HEAD_BYTES + share * 6 * 4; }
+
+__device__ __forceinline__ double dsmem_ld_f64(const double* p, int rank) {
+    const float* f = reinterpret_cast<const float*>(p);
+    uint32_t h[2] = {__float_as_uint(dsmem_ld(f, rank)), __float_as_uint(dsmem_ld(f + 1, rank))};
+    double v;
+    memcpy(&v, h, 8);
+    return v;
+}
+__device__ __forceinline__ float sum_ranks(const float* p, int ctas) {
+    float v = dsmem_ld(p, 0);
+    for (int r = 1; r < ctas; ++r) v += dsmem_ld(p, r);
+    return v;
+}
+
+// this rank's block sums of K fp64 values -> `slot`; one cluster barrier; thread k < K adds slot k of ranks 0 .. ctas - 1
+// in rank order into tot[k]; every thread gets the totals in v.  (The totals go on in a thread-local array, as in
+// epnp_init_kernel: pnp_epnp.cuh's out-of-line functions then see the address spaces they see there, and
+// epnp_init_kernel's code does not change.)
+template <int K>
+__device__ __forceinline__ void cluster_sum_f64(double (&v)[K], double* red, double* slot, double* tot, int ctas) {
+    block_sum_f64<K, EPNP_SPLIT_T>(v, red);
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) slot[k] = v[k];
+    }
+    cluster_sync();
+    if (threadIdx.x < K) {
+        double s = dsmem_ld_f64(slot + threadIdx.x, 0);
+        for (int r = 1; r < ctas; ++r) s += dsmem_ld_f64(slot + threadIdx.x, r);
+        tot[threadIdx.x] = s;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < K; ++k) v[k] = tot[k];
+}
+
+__global__ void __launch_bounds__(EPNP_SPLIT_T, 1) epnp_init_split_kernel(const EpnpInitArgs a, const int ctas) {
+    constexpr int T = EPNP_SPLIT_T;
+    EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
+    EpnpSplitHead& h = *reinterpret_cast<EpnpSplitHead*>(smem_raw);
+    const int N = a.N, share = split_share(N, ctas);
+    const int rank = cluster_rank(), obj = blockIdx.x / ctas, tid = threadIdx.x;
+    const int p0 = min(N, rank * share), cnt = min(N, p0 + share) - p0;
+    uint32_t* keys = reinterpret_cast<uint32_t*>(smem_raw + EPNP_SPLIT_HEAD_BYTES);    // [share]
+    float* P = reinterpret_cast<float*>(keys + share);                                 // [5][share]: X Y Z u v, kept
+    const float* g3 = a.x3d + ((size_t)obj * N + p0) * 3;
+    const float* g2 = a.x2d + ((size_t)obj * N + p0) * 2;
+    int nk = cnt;                           // this rank's kept points
+    float thr = 0.f;
+    if (a.w2d) {
+        const float* gw = a.w2d + ((size_t)obj * N + p0) * 2;
+        float nan_count[1] = {0.f};
+        for (int i = tid; i < cnt; i += T) {
+            const float c = (__ldg(gw + 2 * i) + __ldg(gw + 2 * i + 1)) * 0.5f;
+            keys[i] = epnp::conf_key(c);
+            nan_count[0] += (c != c) ? 1.f : 0.f;
+        }
+        block_sum<1, T>(nan_count, h.fred, 0);
+        if (tid == 0) h.xnan = nan_count[0];
+        cluster_sync();
+        if (sum_ranks(&h.xnan, ctas) > 0.f) {       // the same decision on every rank
+            if (rank == 0 && tid == 0) {
+#pragma unroll
+                for (int i = 0; i < 7; ++i) a.pose[(size_t)obj * 7 + i] = CUDART_NAN_F;
+                if (a.n_sel) a.n_sel[obj] = 0;
+                SPLIT_AUDIT_STORES(a.n_sel ? 8 : 7);
+            }
+            cluster_sync();                         // no CTA leaves while a peer may still read its NaN count
+            return;
+        }
+        const epnp::QuantileRank r = epnp::quantile_rank(N, a.q);
+        uint32_t lo = 0u, hi = 0u;
+        for (int bit = 31; bit >= 0; --bit) {
+            const uint32_t ca = lo | (1u << bit), cb = hi | (1u << bit);
+            float c[2] = {0.f, 0.f};
+            for (int i = tid; i < cnt; i += T) {
+                const uint32_t k = keys[i];
+                c[0] += k < ca ? 1.f : 0.f;
+                c[1] += k < cb ? 1.f : 0.f;
+            }
+            block_sum<2, T>(c, h.fred, bit & 1);
+            float* x = h.xsel[bit & 1];
+            if (tid == 0) { x[0] = c[0]; x[1] = c[1]; }
+            cluster_sync();
+            if (sum_ranks(x, ctas) <= (float)r.k) lo = ca;
+            if (sum_ranks(x + 1, ctas) <= (float)r.k1) hi = cb;
+        }
+        thr = epnp::quantile_threshold(epnp::key_conf(lo), epnp::key_conf(hi), r.g);
+        const int per = (cnt + T - 1) / T, i0 = min(cnt, tid * per), i1 = min(cnt, i0 + per);
+        int mine = 0;
+        for (int i = i0; i < i1; ++i) mine += epnp::key_conf(keys[i]) >= thr ? 1 : 0;
+        h.counts[tid] = mine;
+        __syncthreads();
+        int off = 0;
+        nk = 0;
+        for (int t = 0; t < T; ++t) {
+            off += t < tid ? h.counts[t] : 0;
+            nk += h.counts[t];
+        }
+        for (int i = i0; i < i1; ++i) {
+            if (!(epnp::key_conf(keys[i]) >= thr)) continue;
+            P[off] = __ldg(g3 + 3 * i); P[share + off] = __ldg(g3 + 3 * i + 1); P[2 * share + off] = __ldg(g3 + 3 * i + 2);
+            P[3 * share + off] = __ldg(g2 + 2 * i); P[4 * share + off] = __ldg(g2 + 2 * i + 1);
+            ++off;
+        }
+    } else {
+        for (int i = tid; i < cnt; i += T) {
+            P[i] = __ldg(g3 + 3 * i); P[share + i] = __ldg(g3 + 3 * i + 1); P[2 * share + i] = __ldg(g3 + 3 * i + 2);
+            P[3 * share + i] = __ldg(g2 + 2 * i); P[4 * share + i] = __ldg(g2 + 2 * i + 1);
+        }
+    }
+    if (tid == 0) h.xkept = (float)nk;
+    cluster_sync();                         // also publishes the kept points to the peers
+    int n = 0, first = -1;
+    for (int r = 0; r < ctas; ++r) {
+        const int k = (int)dsmem_ld(&h.xkept, r);
+        if (first < 0 && k > 0) first = r;
+        n += k;
+    }
+    float Kf[9];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) Kf[i] = __ldg(a.cam + (size_t)obj * 9 + i);
+    const epnp::Intrinsics in = epnp::intrinsics(Kf);
+    double c0[3] = {0.0, 0.0, 0.0};
+    for (int j = tid; j < nk; j += T) { c0[0] += P[j]; c0[1] += P[share + j]; c0[2] += P[2 * share + j]; }
+    cluster_sum_f64<3>(c0, h.red, h.xc0, h.g.c0, ctas);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) c0[c] /= n;
+    double S[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int j = tid; j < nk; j += T) {
+        const double dx = P[j] - c0[0], dy = P[share + j] - c0[1], dz = P[2 * share + j] - c0[2];
+        S[0] += dx * dx; S[1] += dx * dy; S[2] += dx * dz; S[3] += dy * dy; S[4] += dy * dz; S[5] += dz * dz;
+    }
+    cluster_sum_f64<6>(S, h.red, h.xS, h.g.S, ctas);
+    if (tid == 0) epnp::control_points<1>(c0, S, n, h.g.cp);
+    __syncthreads();
+    double acc[epnp::NSUM];
+#pragma unroll
+    for (int k = 0; k < epnp::NSUM; ++k) acc[k] = 0.0;
+    for (int j = tid; j < nk; j += T)
+        epnp::accumulate_point(h.g.cp, in, P[j], P[share + j], P[2 * share + j], P[3 * share + j], P[4 * share + j], acc);
+    cluster_sum_f64<epnp::NSUM>(acc, h.red, h.xacc, h.g.acc, ctas);
+    if (tid == 0) {
+        double al[4];               // the object's first kept point: the first one of rank `first`
+        epnp::barycentric(h.g.cp, dsmem_ld(P, first), dsmem_ld(P + share, first), dsmem_ld(P + 2 * share, first), al);
+        epnp::solve_candidates<1>(acc, h.g.cp, in, al, n, h.g.cand);
+    }
+    __syncthreads();
+    double err[3] = {0.0, 0.0, 0.0};
+    for (int j = tid; j < nk; j += T) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+            err[c] += epnp::reproj_error(h.g.cand[c], in, P[j], P[share + j], P[2 * share + j], P[3 * share + j], P[4 * share + j]);
+    }
+    cluster_sum_f64<3>(err, h.red, h.xerr, h.g.err, ctas);
+    if (tid == 0) {
+        h.g.thr = thr; h.g.n = n; h.g.first = first; h.g.best = epnp::pick_candidate(err);
+        if (rank == 0) {
+            epnp::write_pose(h.g.cand[h.g.best], a.pose + (size_t)obj * 7);
+            if (a.n_sel) a.n_sel[obj] = n;
+            SPLIT_AUDIT_STORES(a.n_sel ? 8 : 7);
+        }
+    }
+#ifdef EPNP_SPLIT_AUDIT
+    cluster_sync();                         // rank 0's agreed state is complete
+    const float* w = reinterpret_cast<const float*>(&h.g);
+    for (int k = tid; k < (int)(sizeof(EpnpSplitAgreed) / 4); k += T)
+        if (__float_as_uint(dsmem_ld(w + k, 0)) != __float_as_uint(w[k])) SPLIT_AUDIT_MISMATCH();
+#endif
+    // a CTA's shared memory disappears when it exits: no CTA leaves while a peer may still read its error partials
+    cluster_sync();
+}
+
 // ------------------------------------------------------------------------------------------------
 // Host side
 int cuda_fail(cudaError_t e) { g_last_cuda_error = (int)e; return EPNP_ERR_CUDA; }
@@ -1152,25 +1373,28 @@ int launch_amis(KArgs& a, const PushArgs* push, cudaStream_t stream) {
     return launch_cta_per_object<NT>(amis_kernel<DOF, NT>, a, smem_bytes, stream, push ? *push : none);
 }
 
-// Cluster-split launches (amis_split_kernel, cost_split_kernel, gn_plus_backward_split_kernel): `ctas` CTAs of T
-// threads per object; the kernel takes (Args, ctas), Args being KArgs or a struct holding one (kargs_of).  A device that
-// cannot co-schedule one such cluster (a MIG slice, or SMs taken by other work) gets EPNP_ERR_UNSUPPORTED; nothing is
-// launched then.  launch = false: only that check (run_lm_amis_split makes it before its LM launch).
+// Cluster-split launches (amis_split_kernel, cost_split_kernel, gn_plus_backward_split_kernel, epnp_init_split_kernel):
+// `ctas` CTAs of T threads for each of B objects; the kernel takes (Args, ctas).  Args holding a KArgs get its launch
+// fields set (prepare_launch).  A device that cannot co-schedule one such cluster (a MIG slice, or SMs taken by other
+// work) gets EPNP_ERR_UNSUPPORTED; nothing is launched then.  launch = false: only that check (run_lm_amis_split makes
+// it before its LM launch).
 inline KArgs& kargs_of(KArgs& a) { return a; }
 inline KArgs& kargs_of(GnBwArgs& g) { return g.k; }
+inline int prepare_launch(KArgs& a) { a.use_tma = tma_ok(a); return device_sms(&a.num_sms); }
+inline int prepare_launch(GnBwArgs& g) { return prepare_launch(g.k); }
+inline int prepare_launch(EpnpInitArgs&) { return EPNP_OK; }
 #if defined(EPNP_SIMT_EMUL) && !defined(SIMT_EMUL_HAS_CLUSTERS)
 // The single-CTA emulator build (tests/simt_emul) cannot run a cluster: every launch is refused.
 template <int T, class Kern, class Args>
-int launch_cluster_per_object(Kern, Args& args, int smem_bytes, int, cudaStream_t, bool = true) {
-    if (kargs_of(args).B == 0) return EPNP_OK;
+int launch_cluster(Kern, Args&, int B, int smem_bytes, int, cudaStream_t, bool = true) {
+    if (B == 0) return EPNP_OK;
     if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
     return EPNP_ERR_UNSUPPORTED;
 }
 #else
 template <int T, class Kern, class Args>
-int launch_cluster_per_object(Kern kern, Args& args, int smem_bytes, int ctas, cudaStream_t stream, bool launch = true) {
-    KArgs& a = kargs_of(args);
-    if (a.B == 0) return EPNP_OK;
+int launch_cluster(Kern kern, Args& args, int B, int smem_bytes, int ctas, cudaStream_t stream, bool launch = true) {
+    if (B == 0) return EPNP_OK;
     if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
     if (e != cudaSuccess) return cuda_fail(e);
@@ -1182,7 +1406,7 @@ int launch_cluster_per_object(Kern kern, Args& args, int smem_bytes, int ctas, c
     attr[0].val.clusterDim.y = 1;
     attr[0].val.clusterDim.z = 1;
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)a.B * (unsigned)ctas);
+    cfg.gridDim = dim3((unsigned)B * (unsigned)ctas);
     cfg.blockDim = dim3(T);
     cfg.dynamicSmemBytes = (size_t)smem_bytes;
     cfg.stream = stream;
@@ -1193,13 +1417,16 @@ int launch_cluster_per_object(Kern kern, Args& args, int smem_bytes, int ctas, c
     if (e != cudaSuccess) return cuda_fail(e);
     if (clusters == 0) return EPNP_ERR_UNSUPPORTED;
     if (!launch) return EPNP_OK;
-    a.use_tma = tma_ok(a);
-    const int rc = device_sms(&a.num_sms);
+    const int rc = prepare_launch(args);
     if (rc != EPNP_OK) return rc;
     e = cudaLaunchKernelEx(&cfg, kern, args, ctas);
     return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
 }
 #endif
+template <int T, class Kern, class Args>
+int launch_cluster_per_object(Kern kern, Args& args, int smem_bytes, int ctas, cudaStream_t stream, bool launch = true) {
+    return launch_cluster<T>(kern, args, kargs_of(args).B, smem_bytes, ctas, stream, launch);
+}
 
 // Shared memory per CTA of a split launch; mc_samples = 0: the cost and GN-plus backward kernels.
 int split_smem_bytes(int dof, int N, int ctas, int mc_samples, int mc_iter) {
@@ -1590,6 +1817,19 @@ int epnp_epnp_init_f32(const float* x3d, const float* x2d, const float* w2d, con
     EPNP_LAUNCH(epnp_init_kernel, B, NT, smem, (cudaStream_t)stream, a);
     e = cudaGetLastError();
     return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+}
+
+int epnp_epnp_init_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                             float conf_quantile, float* pose, int* n_sel, int B, int N, int cluster_ctas, void* stream) {
+    if (!x3d || !x2d || !cam_mats || !pose || B < 0 || N < 4) return EPNP_ERR_BAD_ARG;
+    if (!(conf_quantile >= 0.0f && conf_quantile <= 1.0f)) return EPNP_ERR_BAD_ARG;
+    if (w2d && epnp::min_selected(N, conf_quantile) < 4) return EPNP_ERR_BAD_ARG;
+    const int ctas = split_ctas_for(6, N, 0, 0, cluster_ctas);     // the cost kernel's plan, which bounds this one's
+    if (ctas < 0) return ctas;
+    const int smem_bytes = epnp_split_smem_bytes(split_share(N, ctas));
+    if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
+    EpnpInitArgs a{x3d, x2d, w2d, cam_mats, pose, n_sel, N, conf_quantile};
+    return launch_cluster<EPNP_SPLIT_T>(epnp_init_split_kernel, a, B, smem_bytes, ctas, (cudaStream_t)stream);
 }
 
 int epnp_amis_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,

@@ -11,10 +11,10 @@
                                     or, with EPNP_NATIVE_GN_STEP=1, by the native kernel epnp_gn_plus_backward_f32
 
 Objects with more points than one SM holds (N above epnp_max_points: about 5,400 for the AMIS loop at M = 512, 7,000
-for the cost and the pose_opt_plus backward) take the cluster-split kernels (fused_forward, stacked_cost,
-gn_plus_backward), up to epnp_max_points_split; at or below those limits nothing changes.  The Monte-Carlo cost
-backward kernel streams the points, so it serves both; the pose_opt_plus forward (the LM kernel) streams them too.
-RSLM init, EPnPSolver and the push / host-buffer entry points still refuse objects above the resident limits.
+for the cost, the pose_opt_plus backward and the EPnP initialiser) take the cluster-split kernels (fused_forward,
+stacked_cost, gn_plus_backward, epnp_init), up to epnp_max_points_split; at or below those limits nothing changes.  The
+Monte-Carlo cost backward kernel streams the points, so it serves both; the pose_opt_plus forward (the LM kernel) streams
+them too.  RSLM init and the push / host-buffer entry points still refuse objects above the resident limits.
 
 Gradients w.r.t. poses (pose_init / stacked hypotheses) are not provided: the reference's losses never use
 them (pose_init is the ground truth, lib/train.py:178-180), and asking for them raises.
@@ -48,6 +48,12 @@ def gn_plus_backward(prob, pose, grad_pose_plus, dof, z_min, eps, huber_eps, wan
     split = prob.N > _resident_limit(dof, 0, 0)
     return (native.gn_plus_backward_split if split else native.gn_plus_backward)(
         prob, pose, grad_pose_plus, dof, z_min, eps, huber_eps, want=want)
+
+
+def epnp_init(x3d, x2d, w2d, cam_mats, conf_quantile):
+    """native.epnp_init, or its cluster-split form when the objects' points do not fit one SM."""
+    split = x3d.shape[1] > _resident_limit(6, 0, 0)
+    return (native.epnp_init_split if split else native.epnp_init)(x3d, x2d, w2d, cam_mats, conf_quantile)
 
 
 def _delta_tensor(delta, ref):

@@ -1,5 +1,7 @@
 """EPnPSolver: the EPnP initialisation of the reference's 6DoF test loop (EPro-PnP-6DoF/lib/test.py:178-194) as an
-`init_solver` of LMSolver, executing on the native sm_90a kernel (epnp_epnp_init_f32, one launch, no host round trip).
+`init_solver` of LMSolver, executing on the native sm_90a kernel (epnp_epnp_init_f32, one launch, no host round trip;
+objects larger than one SM holds, such as the 16,384 points of a 128 x 128 coordinate map, take its cluster-split form
+epnp_epnp_init_split_f32, up to epnp_max_points_split(6, 0, 0)).
 
     solver = LMSolver(dof=6, num_iter=3, init_solver=EPnPSolver(conf_quantile=0.8))
     pose_opt = EProPnP6DoF(solver=solver)(x3d, x2d, w2d, camera, cost_fun, fast_mode=True)[0]   # pose_init=None
@@ -13,6 +15,7 @@ import torch
 import torch.nn as nn
 
 from epropnp_b200 import native
+from . import autograd
 from .builder import PNP
 
 
@@ -33,9 +36,9 @@ class EPnPSolver(nn.Module):
     def solve(self, x3d, x2d, w2d, camera, cost_fun, with_cost=False, **kwargs):
         """-> pose (B, 7), None, cost (B) | None.  With with_cost, the cost is evaluate_pnp's at the EPnP pose (what
         LMSolver compares against pose_init under force_init_solve)."""
-        pose = native.epnp_init(x3d.detach(), x2d.detach(), w2d.detach(), camera.cam_mats, self.conf_quantile)
+        pose = autograd.epnp_init(x3d.detach(), x2d.detach(), w2d.detach(), camera.cam_mats, self.conf_quantile)
         cost = None
         if with_cost:
             prob = native.Problem(x3d, x2d, w2d, camera.cam_mats, camera.lb, camera.ub, cost_fun.delta)
-            cost = native.evaluate_cost(prob, pose[None], 6, float(camera.z_min))[0].to(x2d.dtype)
+            cost = autograd.stacked_cost(prob, pose[None], 6, float(camera.z_min))[0].to(x2d.dtype)
         return pose.to(x2d.dtype), None, cost

@@ -119,8 +119,8 @@ def max_points(dof, mc_samples=0, mc_iter=0):
 
 
 def max_points_split(dof, mc_samples=0, mc_iter=0):
-    """Largest N the cluster-split calls take (lm_amis_fused_split with mc_samples > 0, else evaluate_cost_split and
-    gn_plus_backward_split)."""
+    """Largest N the cluster-split calls take (lm_amis_fused_split with mc_samples > 0, else evaluate_cost_split,
+    gn_plus_backward_split and, with dof = 6, epnp_init_split)."""
     return int(lib().epnp_max_points_split(int(dof), int(mc_samples), int(mc_iter)))
 
 
@@ -218,6 +218,18 @@ def epnp_init(x3d, x2d, w2d, cam_mats, conf_quantile=0.8, want_n_sel=False):
     """EPnP initialisation of the 6DoF test-time solve (epnp_epnp_init_f32): per object, the points whose confidence
     mean(w2d, -1) is >= its np.quantile(., conf_quantile) (every point when w2d is None), then EPnP as
     cv2.solvePnP(SOLVEPNP_EPNP) computes it.  -> pose (B, 7) [x y z w i j k], w >= 0 [, n_sel (B) int32]."""
+    return _epnp_init("epnp_epnp_init_f32", (), x3d, x2d, w2d, cam_mats, conf_quantile, want_n_sel)
+
+
+def epnp_init_split(x3d, x2d, w2d, cam_mats, conf_quantile=0.8, want_n_sel=False, cluster_ctas=0):
+    """epnp_init for objects larger than one SM holds (epnp_epnp_init_split_f32): one thread-block cluster of
+    split_ctas(6, N) CTAs per object, or of `cluster_ctas` (that minimum .. 8).  The same kept points for every cluster
+    size; the pose depends on the cluster size (the order of the fp64 sums), not on the batch."""
+    return _epnp_init("epnp_epnp_init_split_f32", (int(cluster_ctas),), x3d, x2d, w2d, cam_mats, conf_quantile,
+                      want_n_sel)
+
+
+def _epnp_init(fn, extra, x3d, x2d, w2d, cam_mats, conf_quantile, want_n_sel):
     _need_cuda(x3d, "x3d")
     if x3d.dim() != 3 or x3d.shape[2] != 3:
         raise ValueError(f"x3d must be (B, N, 3), got {tuple(x3d.shape)}")
@@ -233,9 +245,8 @@ def epnp_init(x3d, x2d, w2d, cam_mats, conf_quantile=0.8, want_n_sel=False):
     if B > 0:
         cam = _cam(cam_mats, B, dev)
         with torch.cuda.device(dev):
-            check(lib().epnp_epnp_init_f32(ptr(x3d), ptr(x2d), ptr(w2d), ptr(cam), ctypes.c_float(conf_quantile),
-                                           ptr(pose), None if n_sel is None else capi.iptr(n_sel), B, N,
-                                           stream_ptr(dev)), "epnp_epnp_init_f32")
+            check(getattr(lib(), fn)(ptr(x3d), ptr(x2d), ptr(w2d), ptr(cam), ctypes.c_float(conf_quantile), ptr(pose),
+                                     None if n_sel is None else capi.iptr(n_sel), B, N, *extra, stream_ptr(dev)), fn)
     return (pose, n_sel) if want_n_sel else pose
 
 
@@ -493,4 +504,4 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
 
 
 __all__ = ["Problem", "adaptive_delta", "cost_backward", "evaluate_cost", "evaluate_cost_split", "evaluate_full", "lm_solve",
-           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "fused_workspace_bytes", "rslm", "epnp_init", "gn_plus_backward", "gn_plus_backward_split", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]
+           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "fused_workspace_bytes", "rslm", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

@@ -181,6 +181,19 @@ int epnp_epnp_init_f32(const float* x3d, const float* x2d, const float* w2d /*[o
                        const float* cam_mats, float conf_quantile, float* pose /*(B,7)*/, int* n_sel /*[opt]*/,
                        int B, int N, void* stream);
 
+/* epnp_epnp_init_f32 for objects of up to epnp_max_points_split(6, 0, 0) points (the dense coordinate maps of the 6DoF
+ * test loop): one cluster of C CTAs per object, each rank holding one range of the points.  The radix-select counts,
+ * the kept counts and the fp64 sums are added over distributed shared memory in rank order, so every rank solves the
+ * same EPnP problem; rank 0 writes pose and n_sel.  The kept set is exactly that of epnp_epnp_init_f32 (the counts
+ * are integers) for every C; the pose depends on C (the order of the fp64 sums over ranks) and never on B or the
+ * object's position in the batch.  cluster_ctas = 0 takes C = epnp_split_ctas(6, N, 0, 0); a caller may ask for any C
+ * from that minimum to 8 (EPNP_ERR_BAD_ARG outside it, EPNP_ERR_TOO_MANY_POINTS when no C fits).  EPNP_ERR_UNSUPPORTED
+ * when the device cannot run one cluster of that size; nothing is launched then.  The other arguments, checks and the
+ * NaN / degenerate-object semantics are those of epnp_epnp_init_f32.                                                 */
+int epnp_epnp_init_split_f32(const float* x3d, const float* x2d, const float* w2d /*[opt] NULL = all points*/,
+                             const float* cam_mats, float conf_quantile, float* pose /*(B,7)*/, int* n_sel /*[opt]*/,
+                             int B, int N, int cluster_ctas, void* stream);
+
 /* LMSolver.solve with a given pose_init (levenberg_marquardt.py:80-190, _lm_iter :192-241, GN
  * fast mode :136-152) plus, when pose_opt_plus != NULL, the extra Gauss-Newton step of
  * LMSolver.forward (:66-68, gn_step :243-253, pose_add :255-265).

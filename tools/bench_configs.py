@@ -264,6 +264,34 @@ def main():
                                 iters=10)
         row["ms_resident"] = timed(lambda: native.gn_plus_backward(prob, p0, gp, 6, 0.01, 1e-5, 1e-10), iters=10)
         out.append(row)
+        # the 6DoF test-time path on the same dense maps: the split EPnP initialiser alone, EPnP + GN(3) through
+        # LMSolver (which takes the split call above the resident limit), and the reference's host loop; and at
+        # N = 4,096 the split EPnP on two CTAs next to the resident kernel
+        from epropnp.epnp import EPnPSolver
+        N = 16 if TOY else 16384
+        for B in bs(32, 256):
+            pc = {k: v.to(dev) for k, v in make_problem(B, N, seed=13, grid2d=True).items()}
+            t = (pc["x3d"], pc["x2d"], pc["w2d"], pc["cam_mats"])
+            camera = PerspectiveCamera(cam_mats=pc["cam_mats"], z_min=0.01)
+            cost_fun = AdaptiveHuberPnPCost(relative_delta=0.1)
+            cost_fun.set_param(pc["x2d"], pc["w2d"])
+            solver = LMSolver(dof=6, num_iter=3, init_solver=EPnPSolver(conf_quantile=0.8))
+            row = dict(config=f"6DoF test-time path: EPnP init (q=0.8) + GN(3), N={N}, cluster-split", B=B,
+                       cluster_ctas=native.split_ctas(6, N), **card)
+            row["ms_epnp_split"] = timed(lambda: native.epnp_init_split(*t, 0.8), iters=10)
+            row["ms_epnp_gn3"] = timed(lambda: solver.solve(pc["x3d"], pc["x2d"], pc["w2d"], camera, cost_fun,
+                                                            fast_mode=True), iters=10)
+            host = host_cv2_epnp_ms(pc, 0.8)
+            if host is not None:
+                row["host_cv2_epnp_ms"] = host
+            out.append(row)
+        B, N4 = b(256), 16 if TOY else 4096
+        pc = {k: v.to(dev) for k, v in make_problem(B, N4, seed=13, grid2d=True).items()}
+        t = (pc["x3d"], pc["x2d"], pc["w2d"], pc["cam_mats"])
+        row = dict(config=f"EPnP init (q=0.8), N={N4}, cluster-split", B=B, cluster_ctas=2, **card)
+        row["ms_split"] = timed(lambda: native.epnp_init_split(*t, 0.8, cluster_ctas=2), iters=10)
+        row["ms_resident"] = timed(lambda: native.epnp_init(*t, 0.8), iters=10)
+        out.append(row)
     for r in out:
         print(json.dumps(r))
 
