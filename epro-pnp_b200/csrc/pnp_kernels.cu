@@ -15,6 +15,7 @@
 //                                    loop, the stacked-pose cost, the pose_opt_plus backward and the EPnP initialiser for
 //                                    objects whose points do not fit one SM: one thread-block CLUSTER of 2..8 CTAs per
 //                                    object, each holding a point range, partial sums added over distributed shared memory.
+//   push_split_kernel                the multi-GPU gather of the split solve: this rank's rows copied into its peers' buffers.
 // No tensor cores: the only contraction is 6-deep, the work is FP32-pipe + MUFU bound (DESIGN.md).
 // Build options: EPNP_PHASE_TIMERS (profiling), EPNP_SIMT_EMUL (g++ build for the test-only CPU emulator).
 #include <cuda_runtime.h>
@@ -1274,6 +1275,44 @@ __global__ void __launch_bounds__(EPNP_SPLIT_T, 1) epnp_init_split_kernel(const 
     cluster_sync();
 }
 
+// The gather of the cluster-split push call (epnp_lm_amis_fused_split_push_f32), launched after the solve on the same
+// stream: this rank's finished rows -- logw (B, M) and pose (B, PD), each one contiguous run -- go to rows
+// [row0, row0 + B) of every peer's full-batch buffers, float4 where the run's length and every address allow.  A copy
+// of what the solve wrote, so the peers hold the single-GPU split result by construction (no second compilation of the
+// AMIS body, DESIGN.md section 5).  Its own loop: the out-of-line push_rows is fitted by ptxas to all its callers, so a
+// new caller could change amis_kernel's code.
+__device__ __forceinline__ void push_run(float* const* peer, int n_peers, size_t dst_off, const float* src, size_t n) {
+    float* dst[EPNP_MAX_PEERS];
+    uintptr_t any = reinterpret_cast<uintptr_t>(src);
+#pragma unroll
+    for (int r = 0; r < EPNP_MAX_PEERS; ++r) {
+        dst[r] = r < n_peers ? peer[r] + dst_off : nullptr;
+        any |= reinterpret_cast<uintptr_t>(dst[r]);
+    }
+    const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+    if ((n & 3) == 0 && (any & 15u) == 0) {
+        for (size_t q = i0; q < n / 4; q += step) {
+            const float4 v = __ldg(reinterpret_cast<const float4*>(src) + q);
+#pragma unroll
+            for (int r = 0; r < EPNP_MAX_PEERS; ++r)
+                if (r < n_peers) reinterpret_cast<float4*>(dst[r])[q] = v;
+        }
+    } else {
+        for (size_t i = i0; i < n; i += step) {
+            const float v = __ldg(src + i);
+#pragma unroll
+            for (int r = 0; r < EPNP_MAX_PEERS; ++r)
+                if (r < n_peers) dst[r][i] = v;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(NT) push_split_kernel(const float* logw, const float* pose, const PushArgs push,
+                                                        const size_t row0, const int B, const int M, const int PD) {
+    push_run(push.logw, push.n, row0 * M, logw, (size_t)B * M);
+    push_run(push.pose, push.n, row0 * PD, pose, (size_t)B * PD);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Host side
 int cuda_fail(cudaError_t e) { g_last_cuda_error = (int)e; return EPNP_ERR_CUDA; }
@@ -1377,7 +1416,7 @@ int launch_amis(KArgs& a, const PushArgs* push, cudaStream_t stream) {
 // `ctas` CTAs of T threads for each of B objects; the kernel takes (Args, ctas).  Args holding a KArgs get its launch
 // fields set (prepare_launch).  A device that cannot co-schedule one such cluster (a MIG slice, or SMs taken by other
 // work) gets EPNP_ERR_UNSUPPORTED; nothing is launched then.  launch = false: only that check (run_lm_amis_split makes
-// it before its LM launch).
+// it before its LM launch).  clusters [opt]: receives how many such clusters the device runs at once.
 inline KArgs& kargs_of(KArgs& a) { return a; }
 inline KArgs& kargs_of(GnBwArgs& g) { return g.k; }
 inline int prepare_launch(KArgs& a) { a.use_tma = tma_ok(a); return device_sms(&a.num_sms); }
@@ -1386,14 +1425,15 @@ inline int prepare_launch(EpnpInitArgs&) { return EPNP_OK; }
 #if defined(EPNP_SIMT_EMUL) && !defined(SIMT_EMUL_HAS_CLUSTERS)
 // The single-CTA emulator build (tests/simt_emul) cannot run a cluster: every launch is refused.
 template <int T, class Kern, class Args>
-int launch_cluster(Kern, Args&, int B, int smem_bytes, int, cudaStream_t, bool = true) {
+int launch_cluster(Kern, Args&, int B, int smem_bytes, int, cudaStream_t, bool = true, int* = nullptr) {
     if (B == 0) return EPNP_OK;
     if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
     return EPNP_ERR_UNSUPPORTED;
 }
 #else
 template <int T, class Kern, class Args>
-int launch_cluster(Kern kern, Args& args, int B, int smem_bytes, int ctas, cudaStream_t stream, bool launch = true) {
+int launch_cluster(Kern kern, Args& args, int B, int smem_bytes, int ctas, cudaStream_t stream, bool launch = true,
+                   int* active = nullptr) {
     if (B == 0) return EPNP_OK;
     if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
@@ -1416,6 +1456,7 @@ int launch_cluster(Kern kern, Args& args, int B, int smem_bytes, int ctas, cudaS
     e = cudaOccupancyMaxActiveClusters(&clusters, kern, &cfg);
     if (e != cudaSuccess) return cuda_fail(e);
     if (clusters == 0) return EPNP_ERR_UNSUPPORTED;
+    if (active) *active = clusters;
     if (!launch) return EPNP_OK;
     const int rc = prepare_launch(args);
     if (rc != EPNP_OK) return rc;
@@ -1424,8 +1465,9 @@ int launch_cluster(Kern kern, Args& args, int B, int smem_bytes, int ctas, cudaS
 }
 #endif
 template <int T, class Kern, class Args>
-int launch_cluster_per_object(Kern kern, Args& args, int smem_bytes, int ctas, cudaStream_t stream, bool launch = true) {
-    return launch_cluster<T>(kern, args, kargs_of(args).B, smem_bytes, ctas, stream, launch);
+int launch_cluster_per_object(Kern kern, Args& args, int smem_bytes, int ctas, cudaStream_t stream, bool launch = true,
+                              int* active = nullptr) {
+    return launch_cluster<T>(kern, args, kargs_of(args).B, smem_bytes, ctas, stream, launch, active);
 }
 
 // Shared memory per CTA of a split launch; mc_samples = 0: the cost and GN-plus backward kernels.
@@ -1516,6 +1558,21 @@ int run_lm_amis_split(KArgs& a, int cluster_ctas, cudaStream_t stream) {
     a.pose_cov_in = a.pose_cov;
     return dof == 6 ? launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<6>, a, smem_bytes, ctas, stream)
                     : launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<4>, a, smem_bytes, ctas, stream);
+}
+
+// What run_lm_amis_split would run B > 0 objects of N points on, checked without launching anything: returns the
+// cluster size C, or the refusal it would give (negative); *wave = the objects the device solves at once (clusters of
+// the AMIS split kernel it co-schedules).  For the host-buffer call, whose refusals come before its first copy.
+int split_lm_amis_plan(const Params& p, int B, int N, int cluster_ctas, int* wave) {
+    const int ctas = split_ctas_for(p.dof, N, p.mc_samples, p.mc_iter, cluster_ctas);
+    if (ctas < 0) return ctas;
+    KArgs a{};
+    a.B = B; a.N = N; a.p = p;
+    const int smem_bytes = split_smem_bytes(p.dof, N, ctas, p.mc_samples, p.mc_iter);
+    const int rc = p.dof == 6
+        ? launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<6>, a, smem_bytes, ctas, nullptr, false, wave)
+        : launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<4>, a, smem_bytes, ctas, nullptr, false, wave);
+    return rc != EPNP_OK ? rc : ctas;
 }
 
 }  // namespace
@@ -1908,15 +1965,14 @@ int epnp_lm_amis_fused_split_f32(const float* x3d, const float* x2d, const float
     return run_lm_amis_split(a, cluster_ctas, (cudaStream_t)stream);
 }
 
-int epnp_lm_amis_fused_push_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
-                                const float* lb, const float* ub, const float* delta, const float* pose_init,
-                                uint64_t seed, uint32_t obj_offset,
-                                float* pose_opt, float* pose_cov, float* cost, float* pose_samples, float* logw,
-                                float* const* peer_logw, float* const* peer_pose, int n_peers,
-                                int B, int N, const EpnpParams* p, void* stream) {
+// The arguments of the push calls as the solve's KArgs and the peer table, or the refusal.
+static int push_args(KArgs& a, PushArgs& push, const float* x3d, const float* x2d, const float* w2d,
+                     const float* cam_mats, const float* lb, const float* ub, const float* delta, const float* pose_init,
+                     uint64_t seed, uint32_t obj_offset,
+                     float* pose_opt, float* pose_cov, float* cost, float* pose_samples, float* logw,
+                     float* const* peer_logw, float* const* peer_pose, int n_peers, int B, int N, const EpnpParams* p) {
     if (!p) return EPNP_ERR_BAD_ARG;
     if (n_peers < 0 || n_peers > EPNP_MAX_PEERS || (n_peers > 0 && (!peer_logw || !peer_pose))) return EPNP_ERR_BAD_ARG;
-    KArgs a{};
     a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
     a.pose_init = pose_init;
     a.seed = seed; a.obj_offset = obj_offset;
@@ -1928,8 +1984,42 @@ int epnp_lm_amis_fused_push_f32(const float* x3d, const float* x2d, const float*
     rc = check_amis_params(*p);
     if (rc != EPNP_OK) return rc;
     if (!pose_init || !pose_opt || !pose_samples || !logw || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
-    PushArgs push{peer_logw, peer_pose, n_peers};
-    return run_lm_amis(a, &push, (cudaStream_t)stream);
+    push = PushArgs{peer_logw, peer_pose, n_peers};
+    return EPNP_OK;
+}
+
+int epnp_lm_amis_fused_push_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                const float* lb, const float* ub, const float* delta, const float* pose_init,
+                                uint64_t seed, uint32_t obj_offset,
+                                float* pose_opt, float* pose_cov, float* cost, float* pose_samples, float* logw,
+                                float* const* peer_logw, float* const* peer_pose, int n_peers,
+                                int B, int N, const EpnpParams* p, void* stream) {
+    KArgs a{};
+    PushArgs push{};
+    const int rc = push_args(a, push, x3d, x2d, w2d, cam_mats, lb, ub, delta, pose_init, seed, obj_offset, pose_opt,
+                             pose_cov, cost, pose_samples, logw, peer_logw, peer_pose, n_peers, B, N, p);
+    return rc != EPNP_OK ? rc : run_lm_amis(a, &push, (cudaStream_t)stream);
+}
+
+int epnp_lm_amis_fused_split_push_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                      const float* lb, const float* ub, const float* delta, const float* pose_init,
+                                      uint64_t seed, uint32_t obj_offset,
+                                      float* pose_opt, float* pose_cov, float* cost, float* pose_samples, float* logw,
+                                      float* const* peer_logw, float* const* peer_pose, int n_peers,
+                                      int B, int N, const EpnpParams* p, int cluster_ctas, void* stream) {
+    KArgs a{};
+    PushArgs push{};
+    int rc = push_args(a, push, x3d, x2d, w2d, cam_mats, lb, ub, delta, pose_init, seed, obj_offset, pose_opt,
+                       pose_cov, cost, pose_samples, logw, peer_logw, peer_pose, n_peers, B, N, p);
+    if (rc != EPNP_OK) return rc;
+    rc = run_lm_amis_split(a, cluster_ctas, (cudaStream_t)stream);
+    if (rc != EPNP_OK || n_peers == 0 || B == 0) return rc;
+    const size_t blocks = ((size_t)B * p->mc_samples + 4 * NT - 1) / (4 * NT);     // one float4 of logw per thread
+    const int grid = blocks < 1024 ? (int)blocks : 1024;
+    EPNP_LAUNCH(push_split_kernel, grid, NT, 0, (cudaStream_t)stream, logw, pose_opt, push, (size_t)obj_offset, B,
+                p->mc_samples, p->dof == 6 ? 7 : 4);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
 }
 
 int epnp_cost_backward_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
@@ -2019,32 +2109,49 @@ struct HostPipe {
 };
 static thread_local HostPipe g_pipe;
 
-int epnp_lm_amis_fused_host_f32(const float* x3d_host, const float* x2d_host, const float* w2d_host,
-                                const float* cam_mats_host, const float* lb_host, const float* ub_host,
-                                const float* delta_host, const float* pose_init_host,
-                                uint64_t seed, uint32_t obj_offset,
-                                float* pose_opt_host, float* pose_cov_host, float* cost_host,
-                                float* pose_samples_host, float* logw_host,
-                                void* workspace, size_t workspace_bytes, int n_chunks,
-                                int B, int N, const EpnpParams* p, void* stream_) {
+// The argument checks both host-buffer calls make first: EPNP_OK or EPNP_ERR_BAD_ARG.
+static int check_host_args(const float* x3d_host, const float* x2d_host, const float* w2d_host,
+                           const float* cam_mats_host, const float* lb_host, const float* ub_host,
+                           const float* delta_host, const float* pose_init_host, float* pose_opt_host, float* logw_host,
+                           void* workspace, size_t workspace_bytes, int B, int N, const EpnpParams* p) {
     if (!p || !workspace || !x3d_host || !x2d_host || !w2d_host || !cam_mats_host || !delta_host || !pose_init_host ||
         !pose_opt_host || !logw_host)
         return EPNP_ERR_BAD_ARG;
     if ((lb_host == nullptr) != (ub_host == nullptr)) return EPNP_ERR_BAD_ARG;
     if (B < 0 || N <= 0) return EPNP_ERR_BAD_ARG;
-    if (B == 0) return EPNP_OK;
+    if (workspace_bytes < ws_layout(B, N, p).total) return EPNP_ERR_BAD_ARG;
+    return EPNP_OK;
+}
+
+// The solve of one chunk: epnp_lm_amis_fused_split_f32's arguments; the resident form ignores cluster_ctas.
+using ChunkSolve = decltype(&epnp_lm_amis_fused_split_f32);
+static int fused_resident_chunk(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                const float* lb, const float* ub, const float* delta, const float* pose_init,
+                                const float* noise_normal, const float* noise_chi2, const float* noise_rot,
+                                uint64_t seed, uint32_t obj_offset,
+                                float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus, float* cost_init,
+                                float* pose_samples, float* logw, float* proposals,
+                                int B, int N, const EpnpParams* p, int, void* stream) {
+    return epnp_lm_amis_fused_f32(x3d, x2d, w2d, cam_mats, lb, ub, delta, pose_init, noise_normal, noise_chi2, noise_rot,
+                                  seed, obj_offset, pose_opt, pose_cov, cost, pose_opt_plus, cost_init, pose_samples, logw,
+                                  proposals, B, N, p, stream);
+}
+
+// The chunked copy-in / solve / copy-out pipeline of the host-buffer calls, after their checks (B > 0): `solve` with
+// `ctas` on every chunk.  n_chunks = 0: cut the batch at whole waves of `wave` objects the device solves at once (a
+// chunk of 1.7 waves costs 2), as few waves per chunk as the 64-chunk limit allows (one chunk when wave = 0);
+// n_chunks >= 1: that many equal chunks.
+static int host_pipeline(ChunkSolve solve, int ctas, int wave,
+                         const float* x3d_host, const float* x2d_host, const float* w2d_host,
+                         const float* cam_mats_host, const float* lb_host, const float* ub_host,
+                         const float* delta_host, const float* pose_init_host,
+                         uint64_t seed, uint32_t obj_offset,
+                         float* pose_opt_host, float* pose_cov_host, float* cost_host,
+                         float* pose_samples_host, float* logw_host,
+                         void* workspace, int n_chunks, int B, int N, const EpnpParams* p, void* stream_) {
     const WsLayout w = ws_layout(B, N, p);
-    if (workspace_bytes < w.total) return EPNP_ERR_BAD_ARG;
-    // n_chunks = 0: cut the batch at whole waves of resident CTAs (a chunk of 1.7 waves costs 2), as few waves per chunk
-    // as the 64-chunk limit allows; n_chunks >= 1: that many equal chunks
     int chunk_objects = 0;
     if (n_chunks == 0) {
-        if (check_amis_params(*p) != EPNP_OK) return EPNP_ERR_BAD_ARG;
-        const int wave = (p->dof == 6)
-            ? (amis_dense(N) ? resident_objects<AMIS_T_DENSE>(amis_kernel<6, AMIS_T_DENSE>, amis_smem_bytes<6>(N, p->mc_samples))
-                             : resident_objects<NT>(amis_kernel<6, NT>, amis_smem_bytes<6>(N, p->mc_samples)))
-            : (amis_dense(N) ? resident_objects<AMIS_T_DENSE>(amis_kernel<4, AMIS_T_DENSE>, amis_smem_bytes<4>(N, p->mc_samples))
-                             : resident_objects<NT>(amis_kernel<4, NT>, amis_smem_bytes<4>(N, p->mc_samples)));
         if (wave > 0) {
             const int waves_per_chunk = (B + 64 * wave - 1) / (64 * wave);
             chunk_objects = wave * waves_per_chunk;
@@ -2086,7 +2193,7 @@ int epnp_lm_amis_fused_host_f32(const float* x3d_host, const float* x2d_host, co
         EPNP_TRY(cudaEventCreateWithFlags(&ev_in[c], cudaEventDisableTiming));
         EPNP_TRY(cudaEventRecord(ev_in[c], g_pipe.in));
         EPNP_TRY(cudaStreamWaitEvent(sk, ev_in[c], 0));
-        rc = epnp_lm_amis_fused_f32(
+        rc = solve(
             (float*)(ws + w.x3d) + (size_t)b0 * N * 3, (float*)(ws + w.x2d) + (size_t)b0 * N * 2,
             (float*)(ws + w.w2d) + (size_t)b0 * N * 2, (float*)(ws + w.cam) + (size_t)b0 * 9,
             lb_host ? (float*)(ws + w.lb) + (size_t)b0 * 2 : nullptr, lb_host ? (float*)(ws + w.ub) + (size_t)b0 * 2 : nullptr,
@@ -2095,7 +2202,7 @@ int epnp_lm_amis_fused_host_f32(const float* x3d_host, const float* x2d_host, co
             (float*)(ws + w.pose_opt) + (size_t)b0 * D, (float*)(ws + w.pose_cov) + (size_t)b0 * dof * dof,
             (float*)(ws + w.cost) + b0, nullptr, nullptr,
             (float*)(ws + w.samples) + (size_t)b0 * M * D, (float*)(ws + w.logw) + (size_t)b0 * M, nullptr,
-            nb, N, p, sk);
+            nb, N, p, ctas, sk);
         if (rc != EPNP_OK) goto done;
         EPNP_TRY(cudaEventCreateWithFlags(&ev_k[c], cudaEventDisableTiming));
         EPNP_TRY(cudaEventRecord(ev_k[c], sk));
@@ -2122,6 +2229,52 @@ done:
     for (int i = 0; i < 3; ++i) if (done[i]) cudaEventDestroy(done[i]);
     if (fork) cudaEventDestroy(fork);
     return rc;
+}
+
+int epnp_lm_amis_fused_host_f32(const float* x3d_host, const float* x2d_host, const float* w2d_host,
+                                const float* cam_mats_host, const float* lb_host, const float* ub_host,
+                                const float* delta_host, const float* pose_init_host,
+                                uint64_t seed, uint32_t obj_offset,
+                                float* pose_opt_host, float* pose_cov_host, float* cost_host,
+                                float* pose_samples_host, float* logw_host,
+                                void* workspace, size_t workspace_bytes, int n_chunks,
+                                int B, int N, const EpnpParams* p, void* stream) {
+    const int rc = check_host_args(x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host, ub_host, delta_host,
+                                   pose_init_host, pose_opt_host, logw_host, workspace, workspace_bytes, B, N, p);
+    if (rc != EPNP_OK || B == 0) return rc;
+    int wave = 0;                               // objects in flight: SMs x resident AMIS CTAs per SM
+    if (n_chunks == 0) {
+        if (check_amis_params(*p) != EPNP_OK) return EPNP_ERR_BAD_ARG;
+        wave = (p->dof == 6)
+            ? (amis_dense(N) ? resident_objects<AMIS_T_DENSE>(amis_kernel<6, AMIS_T_DENSE>, amis_smem_bytes<6>(N, p->mc_samples))
+                             : resident_objects<NT>(amis_kernel<6, NT>, amis_smem_bytes<6>(N, p->mc_samples)))
+            : (amis_dense(N) ? resident_objects<AMIS_T_DENSE>(amis_kernel<4, AMIS_T_DENSE>, amis_smem_bytes<4>(N, p->mc_samples))
+                             : resident_objects<NT>(amis_kernel<4, NT>, amis_smem_bytes<4>(N, p->mc_samples)));
+    }
+    return host_pipeline(fused_resident_chunk, 0, wave, x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host, ub_host,
+                         delta_host, pose_init_host, seed, obj_offset, pose_opt_host, pose_cov_host, cost_host,
+                         pose_samples_host, logw_host, workspace, n_chunks, B, N, p, stream);
+}
+
+int epnp_lm_amis_fused_split_host_f32(const float* x3d_host, const float* x2d_host, const float* w2d_host,
+                                      const float* cam_mats_host, const float* lb_host, const float* ub_host,
+                                      const float* delta_host, const float* pose_init_host,
+                                      uint64_t seed, uint32_t obj_offset,
+                                      float* pose_opt_host, float* pose_cov_host, float* cost_host,
+                                      float* pose_samples_host, float* logw_host,
+                                      void* workspace, size_t workspace_bytes, int n_chunks,
+                                      int B, int N, const EpnpParams* p, int cluster_ctas, void* stream) {
+    int rc = check_host_args(x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host, ub_host, delta_host,
+                             pose_init_host, pose_opt_host, logw_host, workspace, workspace_bytes, B, N, p);
+    if (rc != EPNP_OK || B == 0) return rc;
+    // every refusal of the chunk solves, made here, before the first copy is enqueued
+    if ((p->dof != 4 && p->dof != 6) || check_amis_params(*p) != EPNP_OK || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
+    int wave = 0;                               // objects in flight: co-resident clusters
+    const int ctas = split_lm_amis_plan(*p, B, N, cluster_ctas, &wave);
+    if (ctas < 0) return ctas;
+    return host_pipeline(epnp_lm_amis_fused_split_f32, ctas, wave, x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host,
+                         ub_host, delta_host, pose_init_host, seed, obj_offset, pose_opt_host, pose_cov_host, cost_host,
+                         pose_samples_host, logw_host, workspace, n_chunks, B, N, p, stream);
 }
 
 }  // extern "C"

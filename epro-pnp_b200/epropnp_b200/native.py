@@ -356,6 +356,21 @@ def lm_amis_fused_push(prob: Problem, pose_init, params, pose_opt_out, logw_out,
     also writes this rank's rows into -- lists (<= 8) of tensors / raw pointers, or, for a steady-state loop, the
     peer_table() of each list built once (then `n_peers` = how many entries are in use).  Returns dict(pose_opt, logw,
     pose_samples, cost, pose_cov) of local tensors."""
+    return _fused_push("epnp_lm_amis_fused_push_f32", (), prob, pose_init, params, pose_opt_out, logw_out, peer_logw,
+                       peer_pose, seed, obj_offset, want_cost, want_cov, n_peers)
+
+
+def lm_amis_fused_split_push(prob: Problem, pose_init, params, pose_opt_out, logw_out, peer_logw, peer_pose, seed=0,
+                             obj_offset=0, want_cost=False, want_cov=False, n_peers=None, cluster_ctas=0):
+    """lm_amis_fused_push for objects larger than one SM holds (epnp_lm_amis_fused_split_push_f32): the solve of
+    lm_amis_fused_split (cluster size as there), then one copy kernel that stores this rank's rows into every peer's
+    buffers.  Local and peer rows equal lm_amis_fused_split's bit for bit."""
+    return _fused_push("epnp_lm_amis_fused_split_push_f32", (int(cluster_ctas),), prob, pose_init, params, pose_opt_out,
+                       logw_out, peer_logw, peer_pose, seed, obj_offset, want_cost, want_cov, n_peers)
+
+
+def _fused_push(fn, extra, prob, pose_init, params, pose_opt_out, logw_out, peer_logw, peer_pose, seed, obj_offset,
+                want_cost, want_cov, n_peers):
     D = 7 if params.dof == 6 else 4
     B, M = prob.B, params.mc_samples
     for t, shape in ((pose_opt_out, (B, D)), (logw_out, (B, M))):
@@ -389,12 +404,11 @@ def lm_amis_fused_push(prob: Problem, pose_init, params, pose_opt_out, logw_out,
                cost=prob.empty(B) if want_cost else None,
                pose_cov=prob.empty(B, params.dof, params.dof) if want_cov else None)
     with torch.cuda.device(prob.device):
-        check(lib().epnp_lm_amis_fused_push_f32(*prob.common_ptrs(), ptr(pose_init), ctypes.c_uint64(seed),
-                                                ctypes.c_uint32(obj_offset), ptr(out["pose_opt"]), ptr(out["pose_cov"]),
-                                                ptr(out["cost"]), ptr(out["pose_samples"]), ptr(out["logw"]),
-                                                ctypes.c_void_p(tab_lw.data_ptr()), ctypes.c_void_p(tab_ps.data_ptr()), n,
-                                                B, prob.N, ctypes.byref(params), stream_ptr(prob.device)),
-              "epnp_lm_amis_fused_push_f32")
+        check(getattr(lib(), fn)(*prob.common_ptrs(), ptr(pose_init), ctypes.c_uint64(seed),
+                                 ctypes.c_uint32(obj_offset), ptr(out["pose_opt"]), ptr(out["pose_cov"]),
+                                 ptr(out["cost"]), ptr(out["pose_samples"]), ptr(out["logw"]),
+                                 ctypes.c_void_p(tab_lw.data_ptr()), ctypes.c_void_p(tab_ps.data_ptr()), n,
+                                 B, prob.N, ctypes.byref(params), *extra, stream_ptr(prob.device)), fn)
     if not torch.is_tensor(peer_logw) and tab_lw.is_cuda:
         tab_lw.record_stream(torch.cuda.current_stream(prob.device))       # the kernel reads the tables after we return
         tab_ps.record_stream(torch.cuda.current_stream(prob.device))
@@ -433,6 +447,20 @@ def lm_amis_fused_host(host, params, workspace, n_chunks=8, seed=0, obj_offset=0
     pose_init) of CPU float32 tensors; `workspace` a CUDA uint8 tensor of fused_workspace_bytes().
     Results land in `out` (pinned CPU tensors, allocated when None).  Work is enqueued on the current
     stream of the workspace's device; synchronise that stream before reading `out`."""
+    return _fused_host("epnp_lm_amis_fused_host_f32", (), host, params, workspace, n_chunks, seed, obj_offset, out,
+                       want_samples)
+
+
+def lm_amis_fused_split_host(host, params, workspace, n_chunks=8, seed=0, obj_offset=0, out=None, want_samples=True,
+                             cluster_ctas=0):
+    """lm_amis_fused_host for objects larger than one SM holds (epnp_lm_amis_fused_split_host_f32): every chunk is solved
+    by lm_amis_fused_split (cluster size as there), so the results equal that call's on the same inputs bit for bit.
+    n_chunks = 0 cuts the batch at whole waves of co-resident clusters."""
+    return _fused_host("epnp_lm_amis_fused_split_host_f32", (int(cluster_ctas),), host, params, workspace, n_chunks, seed,
+                       obj_offset, out, want_samples)
+
+
+def _fused_host(fn, extra, host, params, workspace, n_chunks, seed, obj_offset, out, want_samples):
     B, N = host["x3d"].shape[0], host["x3d"].shape[1]
     D = 7 if params.dof == 6 else 4
     M = params.mc_samples
@@ -446,13 +474,12 @@ def lm_amis_fused_host(host, params, workspace, n_chunks=8, seed=0, obj_offset=0
         assert (not t.is_cuda) and t.dtype == torch.float32 and t.is_contiguous(), k
     dev = workspace.device
     with torch.cuda.device(dev):
-        check(lib().epnp_lm_amis_fused_host_f32(
+        check(getattr(lib(), fn)(
             ptr(host["x3d"]), ptr(host["x2d"]), ptr(host["w2d"]), ptr(host["cam_mats"]), ptr(host.get("lb")),
             ptr(host.get("ub")), ptr(host["delta"]), ptr(host["pose_init"]), ctypes.c_uint64(seed),
             ctypes.c_uint32(obj_offset), ptr(out["pose_opt"]), ptr(out["pose_cov"]), ptr(out["cost"]),
             ptr(out.get("pose_samples")), ptr(out["logw"]), ctypes.c_void_p(workspace.data_ptr()),
-            ctypes.c_size_t(workspace.numel()), int(n_chunks), B, N, ctypes.byref(params), stream_ptr(dev)),
-            "epnp_lm_amis_fused_host_f32")
+            ctypes.c_size_t(workspace.numel()), int(n_chunks), B, N, ctypes.byref(params), *extra, stream_ptr(dev)), fn)
     return out
 
 
@@ -504,4 +531,4 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
 
 
 __all__ = ["Problem", "adaptive_delta", "cost_backward", "evaluate_cost", "evaluate_cost_split", "evaluate_full", "lm_solve",
-           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "fused_workspace_bytes", "rslm", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]
+           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "rslm", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

@@ -5,6 +5,8 @@ the (B, M) log-weights); the (B, M, D) pose samples stay sharded unless explicit
 (SURVEY.md section 8e).  The Philox noise is keyed by the GLOBAL object index (`obj_offset`), so a sharded
 run reproduces the single-GPU run bit for bit.
 """
+import functools
+
 import torch
 import torch.distributed as dist
 
@@ -179,6 +181,19 @@ class _DeviceHooks:
         return raw_ipc_open(desc, self.device)     # a raw device pointer (int)
 
 
+@functools.lru_cache(maxsize=None)
+def _resident_limit(dof, mc_samples, mc_iter):
+    from . import native
+    return native.max_points(dof, mc_samples, mc_iter)
+
+
+def _push_call(prob, params):
+    """native.lm_amis_fused_push, or its cluster-split form when the objects' points do not fit one SM."""
+    from . import native
+    split = prob.N > _resident_limit(params.dof, params.mc_samples, params.mc_iter)
+    return native.lm_amis_fused_split_push if split else native.lm_amis_fused_push
+
+
 class _EventWork:
     def __init__(self, event, cur_stream=None):
         self.event, self.cur_stream = event, cur_stream
@@ -192,7 +207,8 @@ class PushGather(_DeviceHooks):
 
     There is no gather step at all: every rank keeps a ring of `depth` FULL-batch result buffers (pose_opt
     (num_obj, D), logw (num_obj, M)), exposed to the other ranks through CUDA IPC once, and the solve kernel itself
-    (native.lm_amis_fused_push -> the AMIS kernel's push epilogue) stores each finished object's rows into slot t mod depth of EVERY
+    (native.lm_amis_fused_push -> the AMIS kernel's push epilogue; for objects above the resident point limit
+    native.lm_amis_fused_split_push, whose copy kernel follows the cluster-split solve) stores each finished object's rows into slot t mod depth of EVERY
     rank's ring -- its own slice directly as the kernel's normal output, the peers' with plain stores over NVLink,
     object by object underneath the remaining CTAs' math.  What is left per batch is one 4-byte all-reduce on a side
     stream ("all ranks' kernels for batch t have finished, so every row of my slot t is in place").
@@ -251,7 +267,6 @@ class PushGather(_DeviceHooks):
     def solve(self, prob, pose_init, params, seed=0, want_cost=False, want_cov=False):
         """Enqueue batch `step`: fused solve with in-kernel push.  Returns (local result dict, PendingGather of the
         full-batch pose_opt / logw)."""
-        from . import native
         t = self.step
         s = t % self.depth
         lo, hi = self.rank * self.per_rank, (self.rank + 1) * self.per_rank
@@ -259,9 +274,9 @@ class PushGather(_DeviceHooks):
         gate = self.met.get(t - (self.depth - self.valid_for))
         if gate is not None:
             cur.wait_event(gate)              # every rank is past its reads of the slot this batch overwrites
-        out = native.lm_amis_fused_push(prob, pose_init, params, self.ring[s]["pose_opt"][lo:hi],
-                                        self.ring[s]["logw"][lo:hi], self.tables[s][0], self.tables[s][1],
-                                        seed=seed, obj_offset=lo, want_cost=want_cost, want_cov=want_cov, n_peers=self.n_peers)
+        out = _push_call(prob, params)(prob, pose_init, params, self.ring[s]["pose_opt"][lo:hi],
+                                       self.ring[s]["logw"][lo:hi], self.tables[s][0], self.tables[s][1],
+                                       seed=seed, obj_offset=lo, want_cost=want_cost, want_cov=want_cov, n_peers=self.n_peers)
         ready = self._new_event()
         ready.record(cur)
         with self._on_stream(self.comm):

@@ -246,7 +246,8 @@ int epnp_lm_amis_fused_f32(const float* x3d, const float* x2d, const float* w2d,
  * Results depend on C (the order in which the ranks' partial costs are added), never on B, the shard or obj_offset;
  * they agree with epnp_lm_amis_fused_f32 to fp32 rounding, not bit for bit.  EPNP_ERR_UNSUPPORTED when the device
  * cannot run one cluster of that size (cudaOccupancyMaxActiveClusters = 0, e.g. a MIG slice); the LM kernel is not
- * launched either then.  There is no push or host-buffer form.                                                   */
+ * launched either then.  Its push and host-buffer forms: epnp_lm_amis_fused_split_push_f32,
+ * epnp_lm_amis_fused_split_host_f32.                                                                              */
 int epnp_lm_amis_fused_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
                                  const float* lb, const float* ub, const float* delta, const float* pose_init,
                                  const float* noise_normal, const float* noise_chi2, const float* noise_rot,
@@ -275,6 +276,19 @@ int epnp_lm_amis_fused_push_f32(const float* x3d, const float* x2d, const float*
                                 float* pose_opt, float* pose_cov, float* cost, float* pose_samples, float* logw,
                                 float* const* peer_logw, float* const* peer_pose, int n_peers,
                                 int B, int N, const EpnpParams* p, void* stream);
+
+/* epnp_lm_amis_fused_push_f32 for objects of up to epnp_max_points_split(dof, M, I) points: the same arguments plus
+ * cluster_ctas (as epnp_lm_amis_fused_split_f32).  The solve is epnp_lm_amis_fused_split_f32's into the local outputs;
+ * then, on the same stream, one copy kernel stores this rank's rows -- pose_opt (B, D) and logw (B, M) -- into rows
+ * [obj_offset, obj_offset + B) of every peer's buffers (nothing is launched after the solve when n_peers = 0).  The
+ * peers therefore hold exactly the local results, which equal epnp_lm_amis_fused_split_f32's bit for bit.  Refusals as
+ * epnp_lm_amis_fused_split_f32's, all before the first launch.                                                    */
+int epnp_lm_amis_fused_split_push_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                      const float* lb, const float* ub, const float* delta, const float* pose_init,
+                                      uint64_t seed, uint32_t obj_offset,
+                                      float* pose_opt, float* pose_cov, float* cost, float* pose_samples, float* logw,
+                                      float* const* peer_logw, float* const* peer_pose, int n_peers,
+                                      int B, int N, const EpnpParams* p, int cluster_ctas, void* stream);
 
 /* Backward of the differentiable outputs of monte_carlo_forward (epropnp.py:108-113: cost_init and the
  * Monte-Carlo costs inside pose_sample_logweights; proposal densities and samples carry no gradient,
@@ -326,6 +340,22 @@ int epnp_lm_amis_fused_host_f32(const float* x3d_host, const float* x2d_host, co
                                 float* pose_samples_host, float* logw_host,
                                 void* workspace, size_t workspace_bytes, int n_chunks,
                                 int B, int N, const EpnpParams* p, void* stream);
+
+/* epnp_lm_amis_fused_host_f32 for objects of up to epnp_max_points_split(dof, M, I) points: the same arguments plus
+ * cluster_ctas; each chunk runs epnp_lm_amis_fused_split_f32 (with obj_offset + the chunk's first object), so the
+ * results equal that call's on the same inputs bit for bit, whatever the chunking.  The workspace is the same
+ * epnp_fused_workspace_bytes(B, N, p).  n_chunks = 0 cuts the batch at whole waves of co-resident clusters
+ * (cudaOccupancyMaxActiveClusters objects), at most 64 chunks.  Every refusal -- EPNP_ERR_TOO_MANY_POINTS above the
+ * split limit, EPNP_ERR_BAD_ARG for a cluster size outside [epnp_split_ctas, 8], EPNP_ERR_UNSUPPORTED where the
+ * cluster cannot be co-scheduled -- comes before any copy is enqueued.                                            */
+int epnp_lm_amis_fused_split_host_f32(const float* x3d_host, const float* x2d_host, const float* w2d_host,
+                                      const float* cam_mats_host, const float* lb_host, const float* ub_host,
+                                      const float* delta_host, const float* pose_init_host,
+                                      uint64_t seed, uint32_t obj_offset,
+                                      float* pose_opt_host, float* pose_cov_host, float* cost_host,
+                                      float* pose_samples_host, float* logw_host,
+                                      void* workspace, size_t workspace_bytes, int n_chunks,
+                                      int B, int N, const EpnpParams* p, int cluster_ctas, void* stream);
 
 #ifdef __cplusplus
 }

@@ -292,6 +292,46 @@ def main():
         row["ms_split"] = timed(lambda: native.epnp_init_split(*t, 0.8, cluster_ctas=2), iters=10)
         row["ms_resident"] = timed(lambda: native.epnp_init(*t, 0.8), iters=10)
         out.append(row)
+        # the host-buffer and push forms of the split solve at out_res = 128: the chunked copy / solve / copy-back
+        # pipeline from pinned host memory next to the device-resident call on the same data and next to one plain
+        # pinned copy of the same 28 N B input bytes (which bound the pipeline sits at); and the split push to 7
+        # stand-in peers on this device next to the plain split call (what the copy kernel after the solve costs)
+        B, N = b(256), 16 if TOY else 16384
+        prob, p0 = setup(B, N, 0.1, grid2d=True)
+        p = native.default_params(6, lm_iter=3, fast_mode=1, z_min=0.01, mc_samples=m(512), mc_iter=2 if TOY else 4)
+        pin = dev.type == "cuda"
+        host = {k: getattr(prob, k).cpu().pin_memory() if pin else getattr(prob, k).cpu()
+                for k in ("x3d", "x2d", "w2d", "delta")}
+        host.update(cam_mats=prob.cam.cpu(), pose_init=p0.cpu().contiguous())
+        ws = torch.empty(native.fused_workspace_bytes(B, N, p), dtype=torch.uint8, device=dev)
+        M, D = p.mc_samples, 7
+        res = dict(pose_opt=torch.empty(B, D, pin_memory=pin), pose_cov=torch.empty(B, 6, 6, pin_memory=pin),
+                   cost=torch.empty(B, pin_memory=pin), logw=torch.empty(B, M, pin_memory=pin),
+                   pose_samples=torch.empty(B, M, D, pin_memory=pin))
+        flat = torch.empty(B * N * 7, pin_memory=pin)
+        flat_dev = torch.empty(B * N * 7, device=dev)
+        row = dict(config=f"host-buffer dense GN(3)+AMIS(4x128), N={N}, cluster-split", B=B,
+                   cluster_ctas=native.split_ctas(6, N, M, p.mc_iter), input_mb=28 * N * B / 1e6, **card)
+        for nc in (0, 8):
+            row[f"ms_host_split_{nc}chunks"] = timed(
+                lambda: native.lm_amis_fused_split_host(host, p, ws, n_chunks=nc, seed=1, out=res), iters=10)
+        row["ms_device_split"] = timed(lambda: native.lm_amis_fused_split(prob, p0, p, seed=1), iters=10)
+        row["ms_h2d_copy"] = timed(lambda: flat_dev.copy_(flat, non_blocking=True), iters=10)
+        row["objects_per_s_host"] = B / min(row["ms_host_split_0chunks"], row["ms_host_split_8chunks"]) * 1e3
+        row["objects_per_s_device"] = B / row["ms_device_split"] * 1e3
+        row["h2d_gbs"] = 28 * N * B / row["ms_h2d_copy"] / 1e6
+        out.append(row)
+        peers_lw = [torch.empty(B, M, device=dev) for _ in range(7)]
+        peers_ps = [torch.empty(B, D, device=dev) for _ in range(7)]
+        tab_lw, tab_ps = native.peer_table(peers_lw, dev), native.peer_table(peers_ps, dev)
+        own_lw, own_ps = torch.empty(B, M, device=dev), torch.empty(B, D, device=dev)
+        row = dict(config=f"split push to 7 stand-in peers, dense GN(3)+AMIS(4x128), N={N}", B=B,
+                   push_bytes_per_peer=B * (M + D) * 4, **card)
+        row["ms_split"] = timed(lambda: native.lm_amis_fused_split(prob, p0, p, seed=1, want_cov=False,
+                                                                   want_cost_init=False), iters=10)
+        row["ms_split_push"] = timed(lambda: native.lm_amis_fused_split_push(prob, p0, p, own_ps, own_lw, tab_lw, tab_ps,
+                                                                             seed=1, n_peers=7), iters=10)
+        out.append(row)
     for r in out:
         print(json.dumps(r))
 
