@@ -82,6 +82,46 @@ __device__ __forceinline__ float log_add_exp(float a, float b) {
     return (lo == -CUDART_INF_F) ? hi : hi + fast_log1p(fast_exp(lo - hi));
 }
 
+// The 6DoF refit's block sums in the resident (T = NT) kernel: block_sum with the transposed butterfly unrolled one
+// template instance per stage, so every stage's trip count is a constant and the W = 16 or 32 values stay in registers.
+// In block_sum's warp_transpose_sum_w the stage count is a loop variable, the inner loops stay partly rolled and the
+// values go through a local-memory copy indexed per lane (LDL / STL on the latency-bound refit chain).  Same adds in the
+// same order, so the same bits.  T != NT keeps block_sum and its code, and so does amis_phase4: its 6-value sums do not reach local memory.
+template <int W, int HALF> __device__ __forceinline__ void amis_transpose_stage(float (&v)[W], int lane) {
+    constexpr int MASK = 32 * HALF / W;     // 16 at the first stage (HALF = W / 2), halving with HALF
+    const bool up = (lane & MASK) != 0;
+#pragma unroll
+    for (int k = 0; k < HALF; ++k) {
+        const float keep = up ? v[k + HALF] : v[k];
+        const float send = up ? v[k] : v[k + HALF];
+        v[k] = keep + __shfl_xor_sync(0xffffffffu, send, MASK);
+    }
+    if constexpr (HALF > 1) amis_transpose_stage<W, HALF / 2>(v, lane);
+}
+template <int K, int T> __device__ __forceinline__ void amis_block_sum(float (&v)[K], float* red, int half) {
+    if constexpr (T != NT) {
+        block_sum<K, T>(v, red, half);
+    } else {
+        static_assert(K > 4 && K <= 32, "amis_block_sum: 5..32 values");
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        float* r = red + half * NT;
+        constexpr int W = K <= 8 ? 8 : (K <= 16 ? 16 : 32);
+        constexpr int SH = W == 8 ? 2 : (W == 16 ? 1 : 0);
+        float w[W];
+#pragma unroll
+        for (int k = 0; k < W; ++k) w[k] = k < K ? v[k] : 0.f;
+        amis_transpose_stage<W, W / 2>(w, lane);
+        float tot = w[0];
+#pragma unroll
+        for (int o = 16 / W; o >= 1; o >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, o);
+        if ((lane & ((1 << SH) - 1)) == 0 && (lane >> SH) < K) r[warp * 32 + (lane >> SH)] = tot;
+        __syncthreads();
+        const float mine = lane < K ? sum_warp_partials<NT>(r, lane) : 0.f;
+#pragma unroll
+        for (int k = 0; k < K; ++k) v[k] = __shfl_sync(0xffffffffu, mine, k);
+    }
+}
+
 // One object's AMIS loop split over a thread-block cluster (amis_split_kernel): this CTA is rank `rank` of `ctas` and
 // holds `npair` pair records of the object.  xbuf: 2 S floats of this CTA's shared memory, the per-sample partial costs
 // of its point range in the half of the current iteration's parity.
@@ -216,7 +256,7 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
 #pragma unroll
                     for (int c = r; c < 4; ++c) { acc[idx] = fmaf(wm * q[r], q[c], acc[idx]); ++idx; }
             }
-            block_sum<15, T>(acc, sh.red, 1);
+            amis_block_sum<15, T>(acc, sh.red, 1);
             inv_sum = 1.0f / acc[0];
             mean[0] = acc[1] * inv_sum; mean[1] = acc[2] * inv_sum; mean[2] = acc[3] * inv_sum;
             const float inv0 = 1.0f / acc[4];
@@ -254,7 +294,7 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
                         for (int c = r; c < 4; ++c) { acc[idx] = fmaf(wm * q[r], q[c], acc[idx]); ++idx; }
                 }
             }
-            block_sum<17, T>(acc, sh.red, 0);
+            amis_block_sum<17, T>(acc, sh.red, 0);
 #pragma unroll
             for (int r = 0; r < 6; ++r) tc[r] = acc[11 + r];
             if (more) {
@@ -280,7 +320,7 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
 #pragma unroll
                     for (int c = r; c < 4; ++c) { acc[idx] = fmaf(wm * q[r], q[c], acc[idx]); ++idx; }
             }
-            block_sum<11, T>(acc, sh.red, (itr + 1) & 1);
+            amis_block_sum<11, T>(acc, sh.red, (itr + 1) & 1);
             const float inv0 = 1.0f / acc[0];
 #pragma unroll
             for (int r = 0; r < 10; ++r) lam10[r] = acc[1 + r] * inv0;
