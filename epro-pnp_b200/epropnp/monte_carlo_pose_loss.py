@@ -12,9 +12,9 @@
 The layer hands out `pose_sample_logweights` (M, B) and `pose_samples` (M, B, D) as transposed views of object-major
 buffers, so each of these is ONE pass over contiguous memory in the native epilogue kernel (epnp_mc_epilogue_f32 /
 epnp_mc_lse_backward_f32) instead of the reference's chain of (M, B) reductions, an advanced-index gather
-`pose_samples[..., [0, 2]]` and a softmax.  The native epilogue is opt-in (`EPNP_NATIVE_MC_EPILOGUE=1`) until its first
-hardware run; the default is the torch composite below, which is the reference's formula verbatim in meaning.  Both
-are outside the hot path: O(M B) work next to the O(M B N) of the solve.
+`pose_samples[..., [0, 2]]` and a softmax.  The native epilogue is the default for CUDA tensors;
+`EPNP_NATIVE_MC_EPILOGUE=0` selects the torch composite below instead, which is the reference's formula verbatim in
+meaning (CPU tensors always take it).  Both are outside the hot path: O(M B) work next to the O(M B N) of the solve.
 """
 import os
 
