@@ -510,9 +510,9 @@ __device__ __noinline__ void push_rows(const float* src, const float* pose, size
     }
 }
 
-// One object per CTA of T threads (blockIdx.x = object).
+// One object per CTA of T threads (blockIdx.x = object).  The body of amis_kernel and amis_seedptr_kernel.
 template <int DOF, int T>
-__global__ void __launch_bounds__(T, T == NT ? AMIS_CTAS_PER_SM : 1) amis_kernel(const KArgs a, const PushArgs push) {
+__device__ __forceinline__ void amis_body(const KArgs& a, const PushArgs& push) {
     EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
     AmisHead<DOF, T>& sh = *reinterpret_cast<AmisHead<DOF, T>*>(smem_raw);
     float* dyn = reinterpret_cast<float*>(smem_raw);
@@ -563,6 +563,21 @@ __global__ void __launch_bounds__(T, T == NT ? AMIS_CTAS_PER_SM : 1) amis_kernel
     }
 }
 
+template <int DOF, int T>
+__global__ void __launch_bounds__(T, T == NT ? AMIS_CTAS_PER_SM : 1) amis_kernel(const KArgs a, const PushArgs push) {
+    amis_body<DOF, T>(a, push);
+}
+
+// amis_kernel with the Philox seed read from device memory at entry, so that a CUDA graph replaying the launch draws
+// from whatever seed the graph (or the caller) wrote there last, instead of the one it was captured with.
+template <int DOF, int T>
+__global__ void __launch_bounds__(T, T == NT ? AMIS_CTAS_PER_SM : 1)
+    amis_seedptr_kernel(const KArgs a, const PushArgs push, const uint64_t* seed) {
+    KArgs s = a;
+    s.seed = *seed;
+    amis_body<DOF, T>(s, push);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Objects whose points do not fit one SM: one object per thread-block CLUSTER of `ctas` CTAs (grid = B * ctas), rank r
 // holding the contiguous point range [r share, (r + 1) share) (split_share).  Every rank runs the whole AMIS control
@@ -603,7 +618,7 @@ __host__ __device__ inline AmisSplitPlan plan_amis_split(int share, int M, int I
 }
 
 template <int DOF>
-__global__ void __launch_bounds__(AMIS_T_DENSE, 1) amis_split_kernel(const KArgs a, const int ctas) {
+__device__ __forceinline__ void amis_split_body(const KArgs& a, const int ctas) {
     constexpr int T = AMIS_T_DENSE;
     EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
     AmisHead<DOF, T>& sh = *reinterpret_cast<AmisHead<DOF, T>*>(smem_raw);
@@ -664,6 +679,24 @@ __global__ void __launch_bounds__(AMIS_T_DENSE, 1) amis_split_kernel(const KArgs
     // Ordering rule 2: a CTA's shared memory disappears when it exits; this barrier keeps every CTA of the cluster alive
     // until no rank can still read its partial costs of the last iteration.
     cluster_sync();
+}
+
+template <int DOF>
+__global__ void __launch_bounds__(AMIS_T_DENSE, 1) amis_split_kernel(const KArgs a, const int ctas) {
+    amis_split_body<DOF>(a, ctas);
+}
+
+// amis_split_kernel with the seed read from device memory at entry (as amis_seedptr_kernel).
+struct SeededKArgs {
+    KArgs k;
+    const uint64_t* seed;
+};
+
+template <int DOF>
+__global__ void __launch_bounds__(AMIS_T_DENSE, 1) amis_split_seedptr_kernel(const SeededKArgs sa, const int ctas) {
+    KArgs s = sa.k;
+    s.seed = *sa.seed;
+    amis_split_body<DOF>(s, ctas);
 }
 
 }  // namespace

@@ -280,13 +280,15 @@ struct RslmDrawArgs {
 
 constexpr uint32_t RSLM_TAG_SUBSET = 0x52534c4du, RSLM_TAG_START = 0x52534c53u;
 
+// The body of rslm_draw_kernel and rslm_draw_seedptr_kernel.  `r` by value: taken by reference, the inlined body
+// compiles to different (validated-kernel-changing) code.
 template <int DOF>
-__global__ void __launch_bounds__(NT) rslm_draw_kernel(const RslmDrawArgs r) {
-    EPNP_DYN_SMEM(unsigned char, smem_raw, 16);
+__device__ __forceinline__ void rslm_draw_body(const RslmDrawArgs r) {
+    EPNP_DYN_SMEM(unsigned char, draw_smem, 16);      // its own name: as a device function it shares the others' scope
     __shared__ float red[2 * NT];
     __shared__ float t0[3];
     __shared__ int counts[NT];
-    float* wbar = reinterpret_cast<float*>(smem_raw);                       // [N]
+    float* wbar = reinterpret_cast<float*>(draw_smem);                       // [N]
     float* keys = wbar + ((r.N + 3) & ~3);                                  // [n][NT]
     int* slots = reinterpret_cast<int*>(keys + (size_t)r.n * NT);           // [n][NT]
     constexpr int PD = Dim<DOF>::POSE;
@@ -437,6 +439,20 @@ __global__ void __launch_bounds__(NT) rslm_draw_kernel(const RslmDrawArgs r) {
         }
         __syncwarp();                       // lane 0 has finished reading the other lanes' lists before they are reused
     }
+}
+
+template <int DOF>
+__global__ void __launch_bounds__(NT) rslm_draw_kernel(const RslmDrawArgs r) {
+    rslm_draw_body<DOF>(r);
+}
+
+// rslm_draw_kernel with the seed read from device memory at entry: a CUDA graph replaying the launch draws new subsets
+// and start orientations whenever the seed there changes.
+template <int DOF>
+__global__ void __launch_bounds__(NT) rslm_draw_seedptr_kernel(const RslmDrawArgs r, const uint64_t* seed) {
+    RslmDrawArgs s = r;
+    s.seed = *seed;
+    rslm_draw_body<DOF>(s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1403,10 +1419,17 @@ template <int DOF> int amis_smem_bytes(int N, int M) {
     return amis_dense(N) ? plan_amis<DOF, AMIS_T_DENSE>(N, M).total_bytes : plan_amis<DOF, NT>(N, M).total_bytes;
 }
 
+// seed_ptr [opt]: the AMIS kernel reads the seed from this device address (amis_seedptr_kernel) instead of a.seed.
 template <int DOF>
-int launch_amis(KArgs& a, const PushArgs* push, cudaStream_t stream) {
+int launch_amis(KArgs& a, const PushArgs* push, cudaStream_t stream, const uint64_t* seed_ptr = nullptr) {
     const int smem_bytes = amis_smem_bytes<DOF>(a.N, a.p.mc_samples);
     const PushArgs none{};
+    if (seed_ptr) {
+        if (amis_dense(a.N))
+            return launch_cta_per_object<AMIS_T_DENSE>(amis_seedptr_kernel<DOF, AMIS_T_DENSE>, a, smem_bytes, stream,
+                                                       push ? *push : none, seed_ptr);
+        return launch_cta_per_object<NT>(amis_seedptr_kernel<DOF, NT>, a, smem_bytes, stream, push ? *push : none, seed_ptr);
+    }
     if (amis_dense(a.N))
         return launch_cta_per_object<AMIS_T_DENSE>(amis_kernel<DOF, AMIS_T_DENSE>, a, smem_bytes, stream, push ? *push : none);
     return launch_cta_per_object<NT>(amis_kernel<DOF, NT>, a, smem_bytes, stream, push ? *push : none);
@@ -1419,8 +1442,10 @@ int launch_amis(KArgs& a, const PushArgs* push, cudaStream_t stream) {
 // it before its LM launch).  clusters [opt]: receives how many such clusters the device runs at once.
 inline KArgs& kargs_of(KArgs& a) { return a; }
 inline KArgs& kargs_of(GnBwArgs& g) { return g.k; }
+inline KArgs& kargs_of(SeededKArgs& s) { return s.k; }
 inline int prepare_launch(KArgs& a) { a.use_tma = tma_ok(a); return device_sms(&a.num_sms); }
 inline int prepare_launch(GnBwArgs& g) { return prepare_launch(g.k); }
+inline int prepare_launch(SeededKArgs& s) { return prepare_launch(s.k); }
 inline int prepare_launch(EpnpInitArgs&) { return EPNP_OK; }
 #if defined(EPNP_SIMT_EMUL) && !defined(SIMT_EMUL_HAS_CLUSTERS)
 // The single-CTA emulator build (tests/simt_emul) cannot run a cluster: every launch is refused.
@@ -1519,7 +1544,8 @@ int check_amis_params(const Params& p) {
 
 // LM kernel, then AMIS kernel, on `stream`.  The covariance travels through a.pose_cov (caller's buffer) or, when the
 // caller did not ask for it, through the first dof^2 floats of each object's -- not yet written -- sample rows.
-int run_lm_amis(KArgs& a, const PushArgs* push, cudaStream_t stream) {
+// seed_ptr [opt]: the AMIS kernel reads its seed from there (launch_amis).
+int run_lm_amis(KArgs& a, const PushArgs* push, cudaStream_t stream, const uint64_t* seed_ptr = nullptr) {
     const int dof = a.p.dof, D = dof == 6 ? 7 : 4;
     if (a.pose_cov) a.cov_stride = dof * dof;
     else {
@@ -1533,11 +1559,26 @@ int run_lm_amis(KArgs& a, const PushArgs* push, cudaStream_t stream) {
     if (rc != EPNP_OK) return rc;
     a.pose_opt_in = a.pose_opt;
     a.pose_cov_in = a.pose_cov;
-    return dof == 6 ? launch_amis<6>(a, push, stream) : launch_amis<4>(a, push, stream);
+    return dof == 6 ? launch_amis<6>(a, push, stream, seed_ptr) : launch_amis<4>(a, push, stream, seed_ptr);
+}
+
+// The launches of run_lm_amis_split on `args` (a KArgs, or a SeededKArgs for the seed-pointer kernel): a device that
+// cannot run the cluster gets no LM launch either.
+template <class Args>
+int lm_amis_split_launches(Args& args, void (*kern)(const Args, const int), int ctas, int smem_bytes, cudaStream_t stream) {
+    KArgs& a = kargs_of(args);
+    int rc = launch_cluster_per_object<AMIS_T_DENSE>(kern, args, smem_bytes, ctas, stream, false);
+    if (rc != EPNP_OK) return rc;
+    rc = a.p.dof == 6 ? launch_lm<6>(a, stream) : launch_lm<4>(a, stream);
+    if (rc != EPNP_OK) return rc;
+    a.pose_opt_in = a.pose_opt;
+    a.pose_cov_in = a.pose_cov;
+    return launch_cluster_per_object<AMIS_T_DENSE>(kern, args, smem_bytes, ctas, stream);
 }
 
 // run_lm_amis with the cluster-split AMIS kernel.  The LM half is the unstaged 8-warp LM kernel, which streams any N.
-int run_lm_amis_split(KArgs& a, int cluster_ctas, cudaStream_t stream) {
+// seed_ptr [opt]: the AMIS kernel reads its seed from there (amis_split_seedptr_kernel).
+int run_lm_amis_split(KArgs& a, int cluster_ctas, cudaStream_t stream, const uint64_t* seed_ptr = nullptr) {
     const int dof = a.p.dof, D = dof == 6 ? 7 : 4;
     const int ctas = split_ctas_for(dof, a.N, a.p.mc_samples, a.p.mc_iter, cluster_ctas);
     if (ctas < 0) return ctas;                  // before anything is launched
@@ -1548,16 +1589,12 @@ int run_lm_amis_split(KArgs& a, int cluster_ctas, cudaStream_t stream) {
         a.cov_stride = a.p.mc_samples * D;
     }
     const int smem_bytes = split_smem_bytes(dof, a.N, ctas, a.p.mc_samples, a.p.mc_iter);
-    // a device that cannot run the cluster gets no LM launch either
-    int rc = dof == 6 ? launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<6>, a, smem_bytes, ctas, stream, false)
-                      : launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<4>, a, smem_bytes, ctas, stream, false);
-    if (rc != EPNP_OK) return rc;
-    rc = dof == 6 ? launch_lm<6>(a, stream) : launch_lm<4>(a, stream);
-    if (rc != EPNP_OK) return rc;
-    a.pose_opt_in = a.pose_opt;
-    a.pose_cov_in = a.pose_cov;
-    return dof == 6 ? launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<6>, a, smem_bytes, ctas, stream)
-                    : launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<4>, a, smem_bytes, ctas, stream);
+    if (seed_ptr) {
+        SeededKArgs sa{a, seed_ptr};
+        return lm_amis_split_launches(sa, dof == 6 ? amis_split_seedptr_kernel<6> : amis_split_seedptr_kernel<4>, ctas,
+                                      smem_bytes, stream);
+    }
+    return lm_amis_split_launches(a, dof == 6 ? amis_split_kernel<6> : amis_split_kernel<4>, ctas, smem_bytes, stream);
 }
 
 // What run_lm_amis_split would run B > 0 objects of N points on, checked without launching anything: returns the
@@ -1836,9 +1873,10 @@ int epnp_rslm_f32(const float* x3d, const float* x2d, const float* w2d, const fl
     return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
 }
 
-int epnp_rslm_draw_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats, const float* t_init,
-                       uint64_t seed, uint32_t obj_offset, int* inds, float* start, float* t_out,
-                       int P, int n, int B, int N, int dof, float eps, void* stream) {
+// epnp_rslm_draw_f32 and, with seed_ptr != NULL, epnp_rslm_draw_seedptr_f32 (the seed then comes from *seed_ptr).
+static int rslm_draw(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats, const float* t_init,
+                     uint64_t seed, const uint64_t* seed_ptr, uint32_t obj_offset, int* inds, float* start, float* t_out,
+                     int P, int n, int B, int N, int dof, float eps, void* stream) {
     if (!w2d || !inds || !start || (dof != 4 && dof != 6) || P <= 0 || n <= 0 || B < 0 || N <= 0 || n > N)
         return EPNP_ERR_BAD_ARG;
     if (!t_init && (!x3d || !x2d || !cam_mats)) return EPNP_ERR_BAD_ARG;
@@ -1847,7 +1885,12 @@ int epnp_rslm_draw_f32(const float* x3d, const float* x2d, const float* w2d, con
     if (smem + 2048 > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
     RslmDrawArgs r{x3d, x2d, w2d, cam_mats, t_init, inds, start, t_out, seed, obj_offset, P, n, B, N, eps};
     cudaError_t e;
-    if (dof == 6) {
+    if (seed_ptr) {
+        const auto kern = dof == 6 ? rslm_draw_seedptr_kernel<6> : rslm_draw_seedptr_kernel<4>;
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return cuda_fail(e);
+        EPNP_LAUNCH(kern, B, NT, smem, (cudaStream_t)stream, r, seed_ptr);
+    } else if (dof == 6) {
         e = cudaFuncSetAttribute(rslm_draw_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return cuda_fail(e);
         EPNP_LAUNCH(rslm_draw_kernel<6>, B, NT, smem, (cudaStream_t)stream, r);
@@ -1858,6 +1901,20 @@ int epnp_rslm_draw_f32(const float* x3d, const float* x2d, const float* w2d, con
     }
     e = cudaGetLastError();
     return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+}
+
+int epnp_rslm_draw_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats, const float* t_init,
+                       uint64_t seed, uint32_t obj_offset, int* inds, float* start, float* t_out,
+                       int P, int n, int B, int N, int dof, float eps, void* stream) {
+    return rslm_draw(x3d, x2d, w2d, cam_mats, t_init, seed, nullptr, obj_offset, inds, start, t_out, P, n, B, N, dof, eps,
+                     stream);
+}
+
+int epnp_rslm_draw_seedptr_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                               const float* t_init, const uint64_t* seed, uint32_t obj_offset, int* inds, float* start,
+                               float* t_out, int P, int n, int B, int N, int dof, float eps, void* stream) {
+    if (!seed) return EPNP_ERR_BAD_ARG;
+    return rslm_draw(x3d, x2d, w2d, cam_mats, t_init, 0, seed, obj_offset, inds, start, t_out, P, n, B, N, dof, eps, stream);
 }
 
 int epnp_epnp_init_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats, float conf_quantile,
@@ -1913,15 +1970,14 @@ int epnp_amis_f32(const float* x3d, const float* x2d, const float* w2d, const fl
     return p->dof == 6 ? launch_amis<6>(a, nullptr, (cudaStream_t)stream) : launch_amis<4>(a, nullptr, (cudaStream_t)stream);
 }
 
-int epnp_lm_amis_fused_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
-                           const float* lb, const float* ub, const float* delta, const float* pose_init,
-                           const float* noise_normal, const float* noise_chi2, const float* noise_rot,
-                           uint64_t seed, uint32_t obj_offset,
-                           float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus, float* cost_init,
-                           float* pose_samples, float* logw, float* proposals,
-                           int B, int N, const EpnpParams* p, void* stream) {
+// The checked KArgs of the fused calls (resident and split, by-value and seed-pointer forms), or the refusal.
+static int fused_args(KArgs& a, const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                      const float* lb, const float* ub, const float* delta, const float* pose_init,
+                      const float* noise_normal, const float* noise_chi2, const float* noise_rot,
+                      uint64_t seed, uint32_t obj_offset,
+                      float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus, float* cost_init,
+                      float* pose_samples, float* logw, float* proposals, int B, int N, const EpnpParams* p) {
     if (!p) return EPNP_ERR_BAD_ARG;
-    KArgs a{};
     a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
     a.pose_init = pose_init;
     a.noise_n3 = noise_normal; a.noise_chi2 = noise_chi2; a.noise_rot = noise_rot;
@@ -1936,7 +1992,36 @@ int epnp_lm_amis_fused_f32(const float* x3d, const float* x2d, const float* w2d,
     if (!pose_init || !pose_opt || !pose_samples || !logw || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
     const bool any = noise_normal || noise_chi2 || noise_rot, all = noise_normal && noise_chi2 && noise_rot;
     if (any && !all) return EPNP_ERR_BAD_ARG;
-    return run_lm_amis(a, nullptr, (cudaStream_t)stream);
+    return EPNP_OK;
+}
+
+int epnp_lm_amis_fused_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                           const float* lb, const float* ub, const float* delta, const float* pose_init,
+                           const float* noise_normal, const float* noise_chi2, const float* noise_rot,
+                           uint64_t seed, uint32_t obj_offset,
+                           float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus, float* cost_init,
+                           float* pose_samples, float* logw, float* proposals,
+                           int B, int N, const EpnpParams* p, void* stream) {
+    KArgs a{};
+    const int rc = fused_args(a, x3d, x2d, w2d, cam_mats, lb, ub, delta, pose_init, noise_normal, noise_chi2, noise_rot,
+                              seed, obj_offset, pose_opt, pose_cov, cost, pose_opt_plus, cost_init, pose_samples, logw,
+                              proposals, B, N, p);
+    return rc != EPNP_OK ? rc : run_lm_amis(a, nullptr, (cudaStream_t)stream);
+}
+
+int epnp_lm_amis_fused_seedptr_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                   const float* lb, const float* ub, const float* delta, const float* pose_init,
+                                   const float* noise_normal, const float* noise_chi2, const float* noise_rot,
+                                   const uint64_t* seed, uint32_t obj_offset,
+                                   float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus, float* cost_init,
+                                   float* pose_samples, float* logw, float* proposals,
+                                   int B, int N, const EpnpParams* p, void* stream) {
+    if (!seed) return EPNP_ERR_BAD_ARG;
+    KArgs a{};
+    const int rc = fused_args(a, x3d, x2d, w2d, cam_mats, lb, ub, delta, pose_init, noise_normal, noise_chi2, noise_rot,
+                              0, obj_offset, pose_opt, pose_cov, cost, pose_opt_plus, cost_init, pose_samples, logw,
+                              proposals, B, N, p);
+    return rc != EPNP_OK ? rc : run_lm_amis(a, nullptr, (cudaStream_t)stream, seed);
 }
 
 int epnp_lm_amis_fused_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
@@ -1946,23 +2031,26 @@ int epnp_lm_amis_fused_split_f32(const float* x3d, const float* x2d, const float
                                  float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus, float* cost_init,
                                  float* pose_samples, float* logw, float* proposals,
                                  int B, int N, const EpnpParams* p, int cluster_ctas, void* stream) {
-    if (!p) return EPNP_ERR_BAD_ARG;
     KArgs a{};
-    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
-    a.pose_init = pose_init;
-    a.noise_n3 = noise_normal; a.noise_chi2 = noise_chi2; a.noise_rot = noise_rot;
-    a.seed = seed; a.obj_offset = obj_offset;
-    a.pose_opt = pose_opt; a.pose_cov = pose_cov; a.cost = cost; a.pose_plus = pose_opt_plus; a.cost_init = cost_init;
-    a.pose_samples = pose_samples; a.logw = logw; a.proposals = proposals; a.B = B; a.N = N; a.p = *p;
-    a.prof = g_prof_buffer;
-    int rc = check_common(a);
-    if (rc != EPNP_OK) return rc;
-    rc = check_amis_params(*p);
-    if (rc != EPNP_OK) return rc;
-    if (!pose_init || !pose_opt || !pose_samples || !logw || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
-    const bool any = noise_normal || noise_chi2 || noise_rot, all = noise_normal && noise_chi2 && noise_rot;
-    if (any && !all) return EPNP_ERR_BAD_ARG;
-    return run_lm_amis_split(a, cluster_ctas, (cudaStream_t)stream);
+    const int rc = fused_args(a, x3d, x2d, w2d, cam_mats, lb, ub, delta, pose_init, noise_normal, noise_chi2, noise_rot,
+                              seed, obj_offset, pose_opt, pose_cov, cost, pose_opt_plus, cost_init, pose_samples, logw,
+                              proposals, B, N, p);
+    return rc != EPNP_OK ? rc : run_lm_amis_split(a, cluster_ctas, (cudaStream_t)stream);
+}
+
+int epnp_lm_amis_fused_split_seedptr_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                         const float* lb, const float* ub, const float* delta, const float* pose_init,
+                                         const float* noise_normal, const float* noise_chi2, const float* noise_rot,
+                                         const uint64_t* seed, uint32_t obj_offset,
+                                         float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus,
+                                         float* cost_init, float* pose_samples, float* logw, float* proposals,
+                                         int B, int N, const EpnpParams* p, int cluster_ctas, void* stream) {
+    if (!seed) return EPNP_ERR_BAD_ARG;
+    KArgs a{};
+    const int rc = fused_args(a, x3d, x2d, w2d, cam_mats, lb, ub, delta, pose_init, noise_normal, noise_chi2, noise_rot,
+                              0, obj_offset, pose_opt, pose_cov, cost, pose_opt_plus, cost_init, pose_samples, logw,
+                              proposals, B, N, p);
+    return rc != EPNP_OK ? rc : run_lm_amis_split(a, cluster_ctas, (cudaStream_t)stream, seed);
 }
 
 // The arguments of the push calls as the solve's KArgs and the peer table, or the refusal.

@@ -105,6 +105,19 @@ def evaluate_pnp(x3d, x2d, w2d, pose, camera, cost_fun,
             _store(out_jacobian, jac) if want_j else None)
 
 
+def philox_seed(seed, device):
+    """The seed of a native Philox draw (AMIS samples, RSLM subsets and starts).  A given seed is used as it is: an int,
+    or a one-element int64 CUDA tensor whose value the kernel reads when it runs.  Without one, a fresh seed: eagerly an
+    int from torch's default CPU generator (torch.manual_seed governs it); while the current stream is being captured
+    into a CUDA graph, a tensor drawn on `device` by torch's CUDA generator, so that every replay of the graph writes a
+    new seed and the kernels draw new samples -- an int would be baked into the graph."""
+    if seed is not None:
+        return seed if torch.is_tensor(seed) and seed.is_cuda else int(seed)
+    if torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing():    # (no CUDA context: no capture)
+        return torch.randint(0, 2 ** 62, (1,), dtype=torch.int64, device=device)
+    return int(torch.randint(0, 2 ** 62, (1,)).item())
+
+
 def pnp_normalize(x3d, pose=None, detach_transformation=True):
     """Centre the 3D points; returns (offset (*, 1, 3), x3d_norm, pose_norm)   (reference common.py:103-127)."""
     src = x3d.detach() if detach_transformation else x3d

@@ -15,8 +15,10 @@ hold (M, B, D) / (M, B) *views* of them so reference call sites (softmax(dim=0),
 [..., [0, 2]] ...) work unchanged.
 
 Extra keyword-only arguments (not in the reference): `amis_noise` = (normal3 (B,M,3), chi2 (B,M),
-rot (B,M,4)) injects the proposals' base noise (parity tests); `amis_seed` fixes the Philox stream.
-Without them a seed is drawn from torch's default CPU generator, so torch.manual_seed() governs it.
+rot (B,M,4)) injects the proposals' base noise (parity tests); `amis_seed` fixes the Philox stream: an int, or a
+one-element int64 CUDA tensor the kernel reads at run time (for CUDA graphs that set the seed before each replay).
+Without them a seed is drawn from torch's default CPU generator, so torch.manual_seed() governs it; while a CUDA graph
+is being captured it is drawn on the device instead, so every replay samples anew (common.philox_seed).
 """
 from abc import ABCMeta, abstractmethod
 
@@ -24,7 +26,7 @@ import torch
 
 from epropnp_b200 import native
 from .builder import PNP, build_pnp
-from .common import evaluate_pnp, pnp_normalize, pnp_denormalize
+from .common import evaluate_pnp, philox_seed, pnp_normalize, pnp_denormalize
 from .distributions import AngularCentralGaussian, MultivariateStudentT, VonMisesUniformMix
 
 # The steps of the AMIS loop the reference exposes as methods of the layer (epropnp.py:65-82).  Here the loop runs inside
@@ -164,7 +166,7 @@ class EProPnPBase(torch.nn.Module, metaclass=ABCMeta):
                                                        force_init_solve, fast_mode)
                 else:
                     start = pose_init
-                seed = int(amis_seed) if amis_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
+                seed = philox_seed(amis_seed, x3d.device)
                 params = self._amis_params(camera, cost_fun, fast_mode)
                 if not differentiable:
                     prob = native.Problem(x3d, x2d, w2d, camera.cam_mats, camera.lb, camera.ub, cost_fun.delta)

@@ -16,7 +16,7 @@ import torch.nn.functional as F
 
 from epropnp_b200 import native
 from .builder import PNP, build_pnp
-from .common import evaluate_pnp, pnp_normalize, pnp_denormalize
+from .common import evaluate_pnp, philox_seed, pnp_normalize, pnp_denormalize
 
 
 def solve_wrapper(b, A):
@@ -223,7 +223,8 @@ class RSLMSolver(LMSolver):
         pair records, scored on all N points, cheapest kept).  The reference's gather of (P*B, n, .) mini-problems, its
         P-fold repeated camera / cost objects and its P*B tiny solves do not exist; run on the same kernels that
         formulation measured slower and was removed.
-        `rslm_seed=` fixes the Philox stream of the native draws."""
+        `rslm_seed=` fixes the Philox stream of the native draws: an int, or a one-element int64 CUDA tensor the kernel
+        reads at run time (common.philox_seed; a graph being captured draws its own on the device)."""
         bs, pn, _ = x2d.size()
         pd = self._pose_dim()
         if bs == 0:
@@ -231,13 +232,17 @@ class RSLMSolver(LMSolver):
         P, n = self.num_proposals, self.num_points
         x3d, x2d, w2d = x3d.detach(), x2d.detach(), w2d.detach()
         if self.draws == 'torch':
+            if torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing():
+                raise RuntimeError(
+                    "RSLMSolver(draws='torch') cannot be captured into a CUDA graph: center_based_init's "
+                    "torch.linalg.solve checks its result on the host, a synchronisation that capture forbids.  "
+                    "draws='native' (the default) is capturable: its kernel reads a seed drawn on the device")
             # weighted subsets without replacement, one row per (proposal, object)
             prob_rows = w2d.mean(dim=-1).unsqueeze(0).expand(P, bs, pn).reshape(P * bs, pn)
             inds = torch.multinomial(prob_rows, n).reshape(P, bs, n)
             start = self._starting_hypotheses(x3d, x2d, camera)
         else:
-            seed = kwargs.get("rslm_seed")
-            seed = int(seed) if seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
+            seed = philox_seed(kwargs.get("rslm_seed"), x2d.device)
             # a subclass that overrides center_based_init keeps its say; otherwise the kernel computes the guess itself
             own_guess = type(self).center_based_init is not RSLMSolver.center_based_init
             t_init = self.center_based_init(x2d, x3d, camera) if own_guess else None

@@ -50,6 +50,7 @@ _SIGNATURES = {
     "epnp_gn_plus_backward_f32": (ctypes.c_int, [_P] * 13 + [_I, _I, _I, _F, _F, _F, _P]),
     "epnp_gn_plus_backward_split_f32": (ctypes.c_int, [_P] * 13 + [_I, _I, _I, _F, _F, _F, _I, _P]),
     "epnp_rslm_draw_f32": (ctypes.c_int, [_P] * 5 + [ctypes.c_uint64, ctypes.c_uint32, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
+    "epnp_rslm_draw_seedptr_f32": (ctypes.c_int, [_P] * 6 + [ctypes.c_uint32, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
     "epnp_rslm_f32": (ctypes.c_int, [_P] * 13 + [_I, _I, _I, _I, ctypes.POINTER(EpnpParams), _P]),
     "epnp_epnp_init_f32": (ctypes.c_int, [_P] * 4 + [_F, _P, _P, _I, _I, _P]),
     "epnp_epnp_init_split_f32": (ctypes.c_int, [_P] * 4 + [_F, _P, _P, _I, _I, _I, _P]),
@@ -59,6 +60,10 @@ _SIGNATURES = {
                                + [_I, _I, ctypes.POINTER(EpnpParams), _P]),
     "epnp_lm_amis_fused_split_f32": (ctypes.c_int, [_P] * 11 + [ctypes.c_uint64, ctypes.c_uint32] + [_P] * 8
                                      + [_I, _I, ctypes.POINTER(EpnpParams), _I, _P]),
+    "epnp_lm_amis_fused_seedptr_f32": (ctypes.c_int, [_P] * 12 + [ctypes.c_uint32] + [_P] * 8
+                                       + [_I, _I, ctypes.POINTER(EpnpParams), _P]),
+    "epnp_lm_amis_fused_split_seedptr_f32": (ctypes.c_int, [_P] * 12 + [ctypes.c_uint32] + [_P] * 8
+                                             + [_I, _I, ctypes.POINTER(EpnpParams), _I, _P]),
     "epnp_lm_amis_fused_push_f32": (ctypes.c_int, [_P] * 8 + [ctypes.c_uint64, ctypes.c_uint32] + [_P] * 5
                                     + [_P, _P, _I, _I, _I, ctypes.POINTER(EpnpParams), _P]),
     "epnp_lm_amis_fused_split_push_f32": (ctypes.c_int, [_P] * 8 + [ctypes.c_uint64, ctypes.c_uint32] + [_P] * 5

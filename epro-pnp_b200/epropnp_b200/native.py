@@ -142,6 +142,18 @@ def evaluate_full(prob: Problem, pose, dof, z_min, huber_eps, clip_jac, want_res
     return res, cost, jac
 
 
+def _seed(fn, seed, device):
+    """The Philox seed argument of `fn`: an int goes by value; a one-element int64 tensor on `device` goes by its device
+    address to fn's *_seedptr_f32 form, whose kernel reads the seed when it starts -- what a CUDA graph needs to draw
+    anew at every replay.  -> (function name, ctypes argument)."""
+    if not torch.is_tensor(seed):
+        return fn, ctypes.c_uint64(seed)
+    if seed.dtype != torch.int64 or seed.numel() != 1 or seed.device != device or not seed.is_contiguous():
+        raise ValueError(f"a seed tensor must be one contiguous int64 element on {device}; got {seed.dtype} "
+                         f"{tuple(seed.shape)} on {seed.device}")
+    return fn.replace("_f32", "_seedptr_f32"), ctypes.c_void_p(seed.data_ptr())
+
+
 def _check_pose(pose, lead, D, what):
     if tuple(pose.shape) != tuple(lead) + (D,):
         raise ValueError(f"{what} must be {tuple(lead) + (D,)}; got {tuple(pose.shape)}")
@@ -169,7 +181,8 @@ def rslm_draw(x3d, x2d, w2d, cam_mats, P, n, dof, eps=1e-5, seed=0, obj_offset=0
     """Everything before the solves of the random-sample initialiser in one launch (epnp_rslm_draw_f32): the
     centre-based translation guess (unless t_init (B, 3) is given -- then x3d / x2d / cam_mats may be None), inds
     (P, B, n) int32 (weighted subsets without replacement, per proposal and object) and start (P, B, D) (that translation
-    + a uniformly random orientation).  -> inds, start [, t (B, 3) with want_t]."""
+    + a uniformly random orientation).  seed: an int, or a one-element int64 tensor on w2d's device that the kernel
+    reads (epnp_rslm_draw_seedptr_f32).  -> inds, start [, t (B, 3) with want_t]."""
     _need_cuda(w2d, "w2d")
     if w2d.dim() != 3 or w2d.shape[-1] != 2:
         raise ValueError(f"w2d must be (B, N, 2), got {tuple(w2d.shape)}")
@@ -190,10 +203,11 @@ def rslm_draw(x3d, x2d, w2d, cam_mats, P, n, dof, eps=1e-5, seed=0, obj_offset=0
     inds = torch.empty(P, B, n, dtype=torch.int32, device=dev)
     start = torch.empty(P, B, D, dtype=torch.float32, device=dev)
     t_out = torch.empty(B, 3, dtype=torch.float32, device=dev) if want_t else None
+    fn, seed_arg = _seed("epnp_rslm_draw_f32", seed, dev)
     with torch.cuda.device(dev):
-        check(lib().epnp_rslm_draw_f32(ptr(x3d), ptr(x2d), ptr(w2d), ptr(cam_mats), ptr(t_init), ctypes.c_uint64(seed),
-                                       ctypes.c_uint32(obj_offset), capi.iptr(inds), ptr(start), ptr(t_out), P, n, B, N, dof,
-                                       ctypes.c_float(eps), stream_ptr(dev)), "epnp_rslm_draw_f32")
+        check(getattr(lib(), fn)(ptr(x3d), ptr(x2d), ptr(w2d), ptr(cam_mats), ptr(t_init), seed_arg,
+                                 ctypes.c_uint32(obj_offset), capi.iptr(inds), ptr(start), ptr(t_out), P, n, B, N, dof,
+                                 ctypes.c_float(eps), stream_ptr(dev)), fn)
     return (inds, start, t_out) if want_t else (inds, start)
 
 
@@ -304,6 +318,8 @@ def amis(prob: Problem, pose_opt, pose_cov, params, noise=None, seed=0, obj_offs
 
 def lm_amis_fused(prob: Problem, pose_init, params, noise=None, seed=0, obj_offset=0, want_cost=False,
                   want_plus=False, want_cost_init=True, want_proposals=False, want_cov=True):
+    """LM solve + AMIS (epnp_lm_amis_fused_f32).  seed: an int, or a one-element int64 tensor on the problem's device
+    that the AMIS kernel reads (epnp_lm_amis_fused_seedptr_f32; outputs equal the int call's with that value)."""
     return _fused("epnp_lm_amis_fused_f32", (), prob, pose_init, params, noise, seed, obj_offset, want_cost, want_plus,
                   want_cost_init, want_proposals, want_cov)
 
@@ -312,7 +328,8 @@ def lm_amis_fused_split(prob: Problem, pose_init, params, noise=None, seed=0, ob
                         want_plus=False, want_cost_init=True, want_proposals=False, want_cov=True, cluster_ctas=0):
     """lm_amis_fused for objects larger than one SM holds (epnp_lm_amis_fused_split_f32): the AMIS loop of each object runs
     on a thread-block cluster of split_ctas(dof, N, M, I) CTAs, or of `cluster_ctas` (that minimum .. 8).  Same outputs;
-    they depend on the cluster size, not on the batch."""
+    they depend on the cluster size, not on the batch.  `seed` as lm_amis_fused's (a tensor takes
+    epnp_lm_amis_fused_split_seedptr_f32)."""
     return _fused("epnp_lm_amis_fused_split_f32", (int(cluster_ctas),), prob, pose_init, params, noise, seed, obj_offset,
                   want_cost, want_plus, want_cost_init, want_proposals, want_cov)
 
@@ -330,9 +347,10 @@ def _fused(fn, extra, prob, pose_init, params, noise, seed, obj_offset, want_cos
                pose_samples=prob.empty(B, M, D), logw=prob.empty(B, M),
                proposals=prob.empty(B, I, 19) if want_proposals else None)
     p3, p2, p4, keep = _noise_ptrs(noise)
+    fn, seed_arg = _seed(fn, seed, prob.device)
     with torch.cuda.device(prob.device):
         check(getattr(lib(), fn)(*prob.common_ptrs(), ptr(pose_init), p3, p2, p4,
-                                 ctypes.c_uint64(seed), ctypes.c_uint32(obj_offset),
+                                 seed_arg, ctypes.c_uint32(obj_offset),
                                  ptr(out["pose_opt"]), ptr(out["pose_cov"]), ptr(out["cost"]),
                                  ptr(out["pose_opt_plus"]), ptr(out["cost_init"]),
                                  ptr(out["pose_samples"]), ptr(out["logw"]), ptr(out["proposals"]),

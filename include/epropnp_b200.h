@@ -154,6 +154,20 @@ int epnp_rslm_draw_f32(const float* x3d, const float* x2d, const float* w2d, con
                        int* inds, float* start, float* t_out,
                        int P, int n, int B, int N, int dof, float eps, void* stream);
 
+/* CUDA-graph capture.  A by-value seed is baked into a captured launch, so every replay of a graph would draw the
+ * same samples.  The *_seedptr_f32 forms below take the seed as `const uint64_t* seed`, a DEVICE address the kernel
+ * reads when it starts; a graph that writes a new seed there (e.g. torch.randint on the device, inside the graph)
+ * draws new samples at every replay.  Arguments, checks and results are otherwise those of the by-value call: given
+ * the value *seed, the outputs equal the by-value call's bit for bit.  EPNP_ERR_BAD_ARG also for seed == NULL.
+ * These and the other device-buffer calls only enqueue kernels on `stream`, so they may be captured.  Not capturable,
+ * and without a seed-pointer form: the host-buffer calls (epnp_lm_amis_fused_host_f32 and its split form run their
+ * own helper streams and events) and the push calls (epnp_lm_amis_fused_push_f32 and its split form write into
+ * IPC-mapped peer buffers that the ranks hand over outside the stream, around an all-reduce).                      */
+int epnp_rslm_draw_seedptr_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                               const float* t_init, const uint64_t* seed, uint32_t obj_offset,
+                               int* inds, float* start, float* t_out,
+                               int P, int n, int B, int N, int dof, float eps, void* stream);
+
 /* RSLMSolver.solve after the hypotheses are drawn (levenberg_marquardt.py:300-353): for every object, P starting
  * poses, each refined by LM / GN on its own n sampled correspondences, scored on all N correspondences, cheapest
  * kept.  Replaces the reference's gather of (P*B, n, .) mini-problems, the P-fold repeated camera / cost objects,
@@ -236,6 +250,14 @@ int epnp_lm_amis_fused_f32(const float* x3d, const float* x2d, const float* w2d,
                            float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus,
                            float* cost_init, float* pose_samples, float* logw, float* proposals,
                            int B, int N, const EpnpParams* p, void* stream);
+/* epnp_lm_amis_fused_f32 with the Philox seed read from device memory (see epnp_rslm_draw_seedptr_f32). */
+int epnp_lm_amis_fused_seedptr_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                   const float* lb, const float* ub, const float* delta, const float* pose_init,
+                                   const float* noise_normal, const float* noise_chi2, const float* noise_rot,
+                                   const uint64_t* seed, uint32_t obj_offset,
+                                   float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus,
+                                   float* cost_init, float* pose_samples, float* logw, float* proposals,
+                                   int B, int N, const EpnpParams* p, void* stream);
 
 /* epnp_lm_amis_fused_f32 for objects of up to epnp_max_points_split(dof, M, I) points (the dense coordinate maps of
  * out_res = 128 and beyond): the same arguments, outputs and noise conventions, plus cluster_ctas.  The LM half is
@@ -255,6 +277,14 @@ int epnp_lm_amis_fused_split_f32(const float* x3d, const float* x2d, const float
                                  float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus,
                                  float* cost_init, float* pose_samples, float* logw, float* proposals,
                                  int B, int N, const EpnpParams* p, int cluster_ctas, void* stream);
+/* epnp_lm_amis_fused_split_f32 with the Philox seed read from device memory (see epnp_rslm_draw_seedptr_f32). */
+int epnp_lm_amis_fused_split_seedptr_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                         const float* lb, const float* ub, const float* delta, const float* pose_init,
+                                         const float* noise_normal, const float* noise_chi2, const float* noise_rot,
+                                         const uint64_t* seed, uint32_t obj_offset,
+                                         float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus,
+                                         float* cost_init, float* pose_samples, float* logw, float* proposals,
+                                         int B, int N, const EpnpParams* p, int cluster_ctas, void* stream);
 
 /* Multi-GPU form of epnp_lm_amis_fused_f32 (one process per GPU, one NVLink / NVSwitch node): the solve AND the gather
  * of its small results in one kernel (the AMIS kernel).  Every CTA, when its object is finished, additionally stores the object's
