@@ -83,7 +83,7 @@ inline void cluster_sync() { simt::cluster_sync(); }
 inline float dsmem_ld(const float* p, int rank) { return *simt::map_shared_rank(p, rank); }
 #else
 // the single-CTA emulator (tests/simt_emul) has no clusters: the split kernels compile, their launches are refused
-// (launch_cluster_per_object), so these never run
+// (launch_cluster), so these never run
 inline int cluster_rank() { return 0; }
 inline void cluster_sync() { std::abort(); }
 inline float dsmem_ld(const float*, int) { std::abort(); }

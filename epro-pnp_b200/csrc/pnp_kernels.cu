@@ -1335,12 +1335,27 @@ int cuda_fail(cudaError_t e) { g_last_cuda_error = (int)e; return EPNP_ERR_CUDA;
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+// The problem fields of a KArgs: correspondences, cameras, bounds [opt] and Huber scales of B objects of N points.
+KArgs problem_args(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats, const float* lb,
+                   const float* ub, const float* delta, int B, int N) {
+    KArgs a{};
+    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
+    a.B = B; a.N = N;
+    return a;
+}
+
 int check_common(const KArgs& a) {
     if (!a.x3d || !a.x2d || !a.w2d || !a.cam || !a.delta) return EPNP_ERR_BAD_ARG;
     if ((a.lb == nullptr) != (a.ub == nullptr)) return EPNP_ERR_BAD_ARG;
     if (a.B < 0 || a.N <= 0) return EPNP_ERR_BAD_ARG;
     if (a.p.dof != 4 && a.p.dof != 6) return EPNP_ERR_BAD_ARG;
     return EPNP_OK;
+}
+
+// f(std::integral_constant<int, 6>{}) for dof = 6, else the <4> form: the DOF instantiation of a kernel or plan.
+template <class F>
+auto by_dof(int dof, F f) {
+    return dof == 6 ? f(std::integral_constant<int, 6>{}) : f(std::integral_constant<int, 4>{});
 }
 
 int device_sms(int* sms) {
@@ -1353,40 +1368,54 @@ int device_sms(int* sms) {
 
 bool tma_ok(const KArgs& a) { return (a.N % 4 == 0) && aligned16(a.x3d) && aligned16(a.x2d) && aligned16(a.w2d); }
 
+// The launch fields of a KArgs: the loader's TMA switch and the SM count.
+int prepare_launch(KArgs& a) { a.use_tma = tma_ok(a); return device_sms(&a.num_sms); }
+
+// The shared-memory check and launch fields of a launch that holds each object's points in one CTA.
+int prepare_resident(KArgs& a, int smem_bytes) {
+    if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
+    return prepare_launch(a);
+}
+
+// What a launch sets on its kernel first: nothing, the dynamic shared-memory size, or that size and the full shared
+// memory carve-out of the SM (which several resident CTAs of nearly 228 KB between them need).  Which kernels ask for
+// the carve-out is a tuning choice, made at each launch.
+enum class SmemAttr { none, size, size_and_carveout };
+
+template <class Kern>
+cudaError_t set_smem_attr(Kern kern, int smem_bytes, SmemAttr attr) {
+    if (attr == SmemAttr::none) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+    if (e != cudaSuccess || attr == SmemAttr::size) return e;
+    return cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+}
+
+// A plain (non-cluster) launch of `grid` CTAs of `block` threads: the kernel's attributes, the launch, its error.
+template <class Kern, class... Args>
+int launch_plain(Kern kern, int grid, int block, int smem_bytes, SmemAttr attr, cudaStream_t stream, Args... args) {
+    cudaError_t e = set_smem_attr(kern, smem_bytes, attr);
+    if (e != cudaSuccess) return cuda_fail(e);
+    EPNP_LAUNCH(kern, grid, block, smem_bytes, stream, args...);
+    e = cudaGetLastError();
+    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+}
+
 // One CTA of NT threads per object (grid = B): the hardware scheduler hands CTAs to SMs as slots free up, the CTAs'
 // serial and parallel phases de-synchronise and there is no lock-step tail, as a persistent grid would have.
 template <int T = NT, class Kern, class... Extra>
 int launch_cta_per_object(Kern kern, KArgs& a, int smem_bytes, cudaStream_t stream, Extra... extra) {
     if (a.B == 0) return EPNP_OK;
-    if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
-    a.use_tma = tma_ok(a);
-    int rc = device_sms(&a.num_sms);
+    const int rc = prepare_resident(a, smem_bytes);
     if (rc != EPNP_OK) return rc;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-    if (e != cudaSuccess) return cuda_fail(e);
-    // several resident CTAs need (nearly) the whole 228 KB of the SM as shared memory: ask for the full carve-out
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    if (e != cudaSuccess) return cuda_fail(e);
-    EPNP_LAUNCH(kern, a.B, T, smem_bytes, stream, a, extra...);
-    e = cudaGetLastError();
-    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+    return launch_plain(kern, a.B, T, smem_bytes, SmemAttr::size_and_carveout, stream, a, extra...);
 }
 
 // LM / GN solve: one CTA of WARPS warps per object (one warp unless the point set is long).  Outputs: a.pose_opt,
 // a.pose_cov [opt] (stride a.cov_stride), a.cost [opt], a.pose_plus [opt], a.cost_init [opt].
 template <int DOF, bool STAGED, int WARPS>
 int launch_lm_as(KArgs& a, cudaStream_t stream) {
-    const int smem_bytes = lm_smem_bytes<DOF, WARPS>(a.N, STAGED);
-    cudaError_t e;
-    if (STAGED) {
-        e = cudaFuncSetAttribute(lm_warp_kernel<DOF, STAGED, WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-        if (e != cudaSuccess) return cuda_fail(e);
-        e = cudaFuncSetAttribute(lm_warp_kernel<DOF, STAGED, WARPS>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-        if (e != cudaSuccess) return cuda_fail(e);
-    }
-    EPNP_LAUNCH((lm_warp_kernel<DOF, STAGED, WARPS>), a.B, 32 * WARPS, smem_bytes, stream, a);
-    e = cudaGetLastError();
-    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+    return launch_plain(lm_warp_kernel<DOF, STAGED, WARPS>, a.B, 32 * WARPS, lm_smem_bytes<DOF, WARPS>(a.N, STAGED),
+                        STAGED ? SmemAttr::size_and_carveout : SmemAttr::none, stream, a);
 }
 
 // Warps per object: a function of N ONLY, so that an object's result does not depend on how large a batch (or which
@@ -1394,24 +1423,23 @@ int launch_lm_as(KArgs& a, cudaStream_t stream) {
 // (N >= 2048: 16+ points per lane even with 8 warps) get 8 warps, everything else one.
 int lm_warps_per_object(int N) { return N >= 2048 ? 8 : 1; }
 
-template <int DOF>
 int launch_lm(KArgs& a, cudaStream_t stream) {
     if (a.B == 0) return EPNP_OK;
-    a.use_tma = tma_ok(a);
-    int rc = device_sms(&a.num_sms);
+    const int rc = prepare_launch(a);
     if (rc != EPNP_OK) return rc;
-    const bool staged = a.N <= LM_STAGE_MAX_N;
-    const int w = lm_warps_per_object(a.N);
-    if (staged) {
-        switch (w) {
-            case 1: return launch_lm_as<DOF, true, 1>(a, stream);
-            default: return launch_lm_as<DOF, true, 8>(a, stream);
-        }
-    }
-    switch (w) {
-        case 1: return launch_lm_as<DOF, false, 1>(a, stream);
-        default: return launch_lm_as<DOF, false, 8>(a, stream);
-    }
+    const bool staged = a.N <= LM_STAGE_MAX_N, one_warp = lm_warps_per_object(a.N) == 1;
+    return by_dof(a.p.dof, [&](auto D) {
+        if (staged) return one_warp ? launch_lm_as<D, true, 1>(a, stream) : launch_lm_as<D, true, 8>(a, stream);
+        return one_warp ? launch_lm_as<D, false, 1>(a, stream) : launch_lm_as<D, false, 8>(a, stream);
+    });
+}
+
+// The LM launch of the fused calls; its pose and covariance are the AMIS kernel's inputs.
+int launch_lm_for_amis(KArgs& a, cudaStream_t stream) {
+    const int rc = launch_lm(a, stream);
+    a.pose_opt_in = a.pose_opt;
+    a.pose_cov_in = a.pose_cov;
+    return rc;
 }
 
 inline bool amis_dense(int N) { return N >= AMIS_DENSE_MIN_N; }
@@ -1419,20 +1447,22 @@ template <int DOF> int amis_smem_bytes(int N, int M) {
     return amis_dense(N) ? plan_amis<DOF, AMIS_T_DENSE>(N, M).total_bytes : plan_amis<DOF, NT>(N, M).total_bytes;
 }
 
+// f(std::integral_constant<int, T>{}) with T the threads per CTA of the resident AMIS kernel for N points.
+template <class F>
+int by_amis_threads(int N, F f) {
+    return amis_dense(N) ? f(std::integral_constant<int, AMIS_T_DENSE>{}) : f(std::integral_constant<int, NT>{});
+}
+
 // seed_ptr [opt]: the AMIS kernel reads the seed from this device address (amis_seedptr_kernel) instead of a.seed.
-template <int DOF>
 int launch_amis(KArgs& a, const PushArgs* push, cudaStream_t stream, const uint64_t* seed_ptr = nullptr) {
-    const int smem_bytes = amis_smem_bytes<DOF>(a.N, a.p.mc_samples);
-    const PushArgs none{};
-    if (seed_ptr) {
-        if (amis_dense(a.N))
-            return launch_cta_per_object<AMIS_T_DENSE>(amis_seedptr_kernel<DOF, AMIS_T_DENSE>, a, smem_bytes, stream,
-                                                       push ? *push : none, seed_ptr);
-        return launch_cta_per_object<NT>(amis_seedptr_kernel<DOF, NT>, a, smem_bytes, stream, push ? *push : none, seed_ptr);
-    }
-    if (amis_dense(a.N))
-        return launch_cta_per_object<AMIS_T_DENSE>(amis_kernel<DOF, AMIS_T_DENSE>, a, smem_bytes, stream, push ? *push : none);
-    return launch_cta_per_object<NT>(amis_kernel<DOF, NT>, a, smem_bytes, stream, push ? *push : none);
+    const PushArgs pa = push ? *push : PushArgs{};
+    return by_dof(a.p.dof, [&](auto D) {
+        const int smem_bytes = amis_smem_bytes<D>(a.N, a.p.mc_samples);
+        return by_amis_threads(a.N, [&](auto T) {
+            if (seed_ptr) return launch_cta_per_object<T>(amis_seedptr_kernel<D, T>, a, smem_bytes, stream, pa, seed_ptr);
+            return launch_cta_per_object<T>(amis_kernel<D, T>, a, smem_bytes, stream, pa);
+        });
+    });
 }
 
 // Cluster-split launches (amis_split_kernel, cost_split_kernel, gn_plus_backward_split_kernel, epnp_init_split_kernel):
@@ -1441,9 +1471,7 @@ int launch_amis(KArgs& a, const PushArgs* push, cudaStream_t stream, const uint6
 // work) gets EPNP_ERR_UNSUPPORTED; nothing is launched then.  launch = false: only that check (run_lm_amis_split makes
 // it before its LM launch).  clusters [opt]: receives how many such clusters the device runs at once.
 inline KArgs& kargs_of(KArgs& a) { return a; }
-inline KArgs& kargs_of(GnBwArgs& g) { return g.k; }
 inline KArgs& kargs_of(SeededKArgs& s) { return s.k; }
-inline int prepare_launch(KArgs& a) { a.use_tma = tma_ok(a); return device_sms(&a.num_sms); }
 inline int prepare_launch(GnBwArgs& g) { return prepare_launch(g.k); }
 inline int prepare_launch(SeededKArgs& s) { return prepare_launch(s.k); }
 inline int prepare_launch(EpnpInitArgs&) { return EPNP_OK; }
@@ -1461,9 +1489,7 @@ int launch_cluster(Kern kern, Args& args, int B, int smem_bytes, int ctas, cudaS
                    int* active = nullptr) {
     if (B == 0) return EPNP_OK;
     if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-    if (e != cudaSuccess) return cuda_fail(e);
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    cudaError_t e = set_smem_attr(kern, smem_bytes, SmemAttr::size_and_carveout);
     if (e != cudaSuccess) return cuda_fail(e);
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -1489,18 +1515,12 @@ int launch_cluster(Kern kern, Args& args, int B, int smem_bytes, int ctas, cudaS
     return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
 }
 #endif
-template <int T, class Kern, class Args>
-int launch_cluster_per_object(Kern kern, Args& args, int smem_bytes, int ctas, cudaStream_t stream, bool launch = true,
-                              int* active = nullptr) {
-    return launch_cluster<T>(kern, args, kargs_of(args).B, smem_bytes, ctas, stream, launch, active);
-}
 
 // Shared memory per CTA of a split launch; mc_samples = 0: the cost and GN-plus backward kernels.
 int split_smem_bytes(int dof, int N, int ctas, int mc_samples, int mc_iter) {
     const int share = split_share(N, ctas);
     if (mc_samples == 0) return plan_cost_split(share).total_bytes;
-    return dof == 6 ? plan_amis_split<6>(share, mc_samples, mc_iter).a.total_bytes
-                    : plan_amis_split<4>(share, mc_samples, mc_iter).a.total_bytes;
+    return by_dof(dof, [&](auto D) { return plan_amis_split<D>(share, mc_samples, mc_iter).a.total_bytes; });
 }
 
 // The automatic cluster size: the smallest C >= 2 whose largest rank share fits, 0 when even 8 do not.  A function of
@@ -1530,8 +1550,7 @@ int resident_objects(Kern kern, int smem_bytes) {
     int sms = 0, occ = 0;
     if ((size_t)smem_bytes > SMEM_LIMIT) return 0;
     if (device_sms(&sms) != EPNP_OK) return 0;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes) != cudaSuccess) return 0;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100) != cudaSuccess) return 0;
+    if (set_smem_attr(kern, smem_bytes, SmemAttr::size_and_carveout) != cudaSuccess) return 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, T, smem_bytes) != cudaSuccess) return 0;
     return sms * occ;
 }
@@ -1542,24 +1561,37 @@ int check_amis_params(const Params& p) {
     return EPNP_OK;
 }
 
-// LM kernel, then AMIS kernel, on `stream`.  The covariance travels through a.pose_cov (caller's buffer) or, when the
-// caller did not ask for it, through the first dof^2 floats of each object's -- not yet written -- sample rows.
-// seed_ptr [opt]: the AMIS kernel reads its seed from there (launch_amis).
-int run_lm_amis(KArgs& a, const PushArgs* push, cudaStream_t stream, const uint64_t* seed_ptr = nullptr) {
+// The checks every AMIS call (epnp_amis_f32, the fused and the push calls) makes of its KArgs: the problem, the AMIS
+// parameters, the sample outputs, and the noise tables, which come all three or not at all.
+int check_amis_call(const KArgs& a) {
+    if (check_common(a) != EPNP_OK || check_amis_params(a.p) != EPNP_OK) return EPNP_ERR_BAD_ARG;
+    if (!a.pose_samples || !a.logw) return EPNP_ERR_BAD_ARG;
+    const bool any = a.noise_n3 || a.noise_chi2 || a.noise_rot, all = a.noise_n3 && a.noise_chi2 && a.noise_rot;
+    return any && !all ? EPNP_ERR_BAD_ARG : EPNP_OK;
+}
+
+// The covariance of the fused calls travels from the LM to the AMIS kernel through a.pose_cov (caller's buffer) or,
+// when the caller did not ask for it, through the first dof^2 floats of each object's -- not yet written -- sample rows.
+int route_cov(KArgs& a) {
     const int dof = a.p.dof, D = dof == 6 ? 7 : 4;
-    if (a.pose_cov) a.cov_stride = dof * dof;
-    else {
-        if (a.p.mc_samples * D < dof * dof) return EPNP_ERR_BAD_ARG;
-        a.pose_cov = a.pose_samples;
-        a.cov_stride = a.p.mc_samples * D;
+    if (a.pose_cov) {
+        a.cov_stride = dof * dof;
+        return EPNP_OK;
     }
-    if ((size_t)(dof == 6 ? amis_smem_bytes<6>(a.N, a.p.mc_samples) : amis_smem_bytes<4>(a.N, a.p.mc_samples)) > SMEM_LIMIT)
-        return EPNP_ERR_TOO_MANY_POINTS;        // before anything is launched
-    int rc = dof == 6 ? launch_lm<6>(a, stream) : launch_lm<4>(a, stream);
+    if (a.p.mc_samples * D < dof * dof) return EPNP_ERR_BAD_ARG;
+    a.pose_cov = a.pose_samples;
+    a.cov_stride = a.p.mc_samples * D;
+    return EPNP_OK;
+}
+
+// LM kernel, then AMIS kernel, on `stream`.  seed_ptr [opt]: the AMIS kernel reads its seed from there (launch_amis).
+int run_lm_amis(KArgs& a, const PushArgs* push, cudaStream_t stream, const uint64_t* seed_ptr = nullptr) {
+    int rc = route_cov(a);
     if (rc != EPNP_OK) return rc;
-    a.pose_opt_in = a.pose_opt;
-    a.pose_cov_in = a.pose_cov;
-    return dof == 6 ? launch_amis<6>(a, push, stream, seed_ptr) : launch_amis<4>(a, push, stream, seed_ptr);
+    if ((size_t)by_dof(a.p.dof, [&](auto D) { return amis_smem_bytes<D>(a.N, a.p.mc_samples); }) > SMEM_LIMIT)
+        return EPNP_ERR_TOO_MANY_POINTS;        // before anything is launched
+    rc = launch_lm_for_amis(a, stream);
+    return rc != EPNP_OK ? rc : launch_amis(a, push, stream, seed_ptr);
 }
 
 // The launches of run_lm_amis_split on `args` (a KArgs, or a SeededKArgs for the seed-pointer kernel): a device that
@@ -1567,34 +1599,26 @@ int run_lm_amis(KArgs& a, const PushArgs* push, cudaStream_t stream, const uint6
 template <class Args>
 int lm_amis_split_launches(Args& args, void (*kern)(const Args, const int), int ctas, int smem_bytes, cudaStream_t stream) {
     KArgs& a = kargs_of(args);
-    int rc = launch_cluster_per_object<AMIS_T_DENSE>(kern, args, smem_bytes, ctas, stream, false);
+    int rc = launch_cluster<AMIS_T_DENSE>(kern, args, a.B, smem_bytes, ctas, stream, false);
     if (rc != EPNP_OK) return rc;
-    rc = a.p.dof == 6 ? launch_lm<6>(a, stream) : launch_lm<4>(a, stream);
-    if (rc != EPNP_OK) return rc;
-    a.pose_opt_in = a.pose_opt;
-    a.pose_cov_in = a.pose_cov;
-    return launch_cluster_per_object<AMIS_T_DENSE>(kern, args, smem_bytes, ctas, stream);
+    rc = launch_lm_for_amis(a, stream);
+    return rc != EPNP_OK ? rc : launch_cluster<AMIS_T_DENSE>(kern, args, a.B, smem_bytes, ctas, stream);
 }
 
 // run_lm_amis with the cluster-split AMIS kernel.  The LM half is the unstaged 8-warp LM kernel, which streams any N.
 // seed_ptr [opt]: the AMIS kernel reads its seed from there (amis_split_seedptr_kernel).
 int run_lm_amis_split(KArgs& a, int cluster_ctas, cudaStream_t stream, const uint64_t* seed_ptr = nullptr) {
-    const int dof = a.p.dof, D = dof == 6 ? 7 : 4;
+    const int dof = a.p.dof;
     const int ctas = split_ctas_for(dof, a.N, a.p.mc_samples, a.p.mc_iter, cluster_ctas);
     if (ctas < 0) return ctas;                  // before anything is launched
-    if (a.pose_cov) a.cov_stride = dof * dof;
-    else {
-        if (a.p.mc_samples * D < dof * dof) return EPNP_ERR_BAD_ARG;
-        a.pose_cov = a.pose_samples;
-        a.cov_stride = a.p.mc_samples * D;
-    }
+    const int rc = route_cov(a);
+    if (rc != EPNP_OK) return rc;
     const int smem_bytes = split_smem_bytes(dof, a.N, ctas, a.p.mc_samples, a.p.mc_iter);
-    if (seed_ptr) {
+    return by_dof(dof, [&](auto D) {
+        if (!seed_ptr) return lm_amis_split_launches(a, amis_split_kernel<D>, ctas, smem_bytes, stream);
         SeededKArgs sa{a, seed_ptr};
-        return lm_amis_split_launches(sa, dof == 6 ? amis_split_seedptr_kernel<6> : amis_split_seedptr_kernel<4>, ctas,
-                                      smem_bytes, stream);
-    }
-    return lm_amis_split_launches(a, dof == 6 ? amis_split_kernel<6> : amis_split_kernel<4>, ctas, smem_bytes, stream);
+        return lm_amis_split_launches(sa, amis_split_seedptr_kernel<D>, ctas, smem_bytes, stream);
+    });
 }
 
 // What run_lm_amis_split would run B > 0 objects of N points on, checked without launching anything: returns the
@@ -1603,12 +1627,11 @@ int run_lm_amis_split(KArgs& a, int cluster_ctas, cudaStream_t stream, const uin
 int split_lm_amis_plan(const Params& p, int B, int N, int cluster_ctas, int* wave) {
     const int ctas = split_ctas_for(p.dof, N, p.mc_samples, p.mc_iter, cluster_ctas);
     if (ctas < 0) return ctas;
-    KArgs a{};
-    a.B = B; a.N = N; a.p = p;
+    KArgs unused{};                             // launch = false: launch_cluster does not read the kernel's arguments
     const int smem_bytes = split_smem_bytes(p.dof, N, ctas, p.mc_samples, p.mc_iter);
-    const int rc = p.dof == 6
-        ? launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<6>, a, smem_bytes, ctas, nullptr, false, wave)
-        : launch_cluster_per_object<AMIS_T_DENSE>(amis_split_kernel<4>, a, smem_bytes, ctas, nullptr, false, wave);
+    const int rc = by_dof(p.dof, [&](auto D) {
+        return launch_cluster<AMIS_T_DENSE>(amis_split_kernel<D>, unused, B, smem_bytes, ctas, nullptr, false, wave);
+    });
     return rc != EPNP_OK ? rc : ctas;
 }
 
@@ -1652,9 +1675,9 @@ int epnp_max_points(int dof, int mc_samples, int mc_iter) {
     while (lo + 4 <= hi) {                   // largest multiple of 4 that fits
         const int mid = ((lo + hi) / 2) / 4 * 4;
         if (mid == lo) break;
-        int bytes;
-        if (amis) bytes = (dof == 6) ? amis_smem_bytes<6>(mid, mc_samples) : amis_smem_bytes<4>(mid, mc_samples);
-        else bytes = (dof == 6) ? plan_obj<6>(mid).total_bytes : plan_obj<4>(mid).total_bytes;
+        const int bytes = by_dof(dof, [&](auto D) {
+            return amis ? amis_smem_bytes<D>(mid, mc_samples) : plan_obj<D>(mid).total_bytes;
+        });
         if ((size_t)bytes <= SMEM_LIMIT) lo = mid; else hi = mid;
     }
     return lo;
@@ -1681,9 +1704,8 @@ int epnp_adaptive_delta_f32(const float* x2d, const float* w2d, float relative_d
                             void* stream) {
     if (!x2d || !w2d || !delta || B < 0 || N <= 0) return EPNP_ERR_BAD_ARG;
     if (B == 0) return EPNP_OK;
-    EPNP_LAUNCH(adaptive_delta_kernel, B, NT, 0, (cudaStream_t)stream, x2d, w2d, relative_delta, delta, N);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+    return launch_plain(adaptive_delta_kernel, B, NT, 0, SmemAttr::none, (cudaStream_t)stream, x2d, w2d, relative_delta,
+                        delta, N);
 }
 
 int epnp_mc_epilogue_f32(const float* logw, const float* pose_samples, const float* pose_opt, const float* cost_target,
@@ -1692,77 +1714,76 @@ int epnp_mc_epilogue_f32(const float* logw, const float* pose_samples, const flo
     if (!lse && !loss && !weights && !score_te) return EPNP_ERR_BAD_ARG;
     if (score_te && (!pose_samples || !pose_opt)) return EPNP_ERR_BAD_ARG;
     if (B == 0) return EPNP_OK;
-    if (dof == 6)
-        EPNP_LAUNCH(mc_epilogue_kernel<7>, B, NT, 0, (cudaStream_t)stream, logw, pose_samples, pose_opt, cost_target, lse, loss,
-                    weights, score_te, M);
-    else
-        EPNP_LAUNCH(mc_epilogue_kernel<4>, B, NT, 0, (cudaStream_t)stream, logw, pose_samples, pose_opt, cost_target, lse, loss,
-                    weights, score_te, M);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+    const auto run = [&](auto kern) {
+        return launch_plain(kern, B, NT, 0, SmemAttr::none, (cudaStream_t)stream, logw, pose_samples, pose_opt,
+                            cost_target, lse, loss, weights, score_te, M);
+    };
+    return dof == 6 ? run(mc_epilogue_kernel<7>) : run(mc_epilogue_kernel<4>);
 }
 
 int epnp_mc_lse_backward_f32(const float* logw, const float* lse, const float* grad_lse, float* grad_logw, int B, int M,
                              void* stream) {
     if (!logw || !lse || !grad_lse || !grad_logw || B < 0 || M <= 0) return EPNP_ERR_BAD_ARG;
     if (B == 0) return EPNP_OK;
-    EPNP_LAUNCH(mc_lse_backward_kernel, B, NT, 0, (cudaStream_t)stream, logw, lse, grad_lse, grad_logw, M);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+    return launch_plain(mc_lse_backward_kernel, B, NT, 0, SmemAttr::none, (cudaStream_t)stream, logw, lse, grad_lse,
+                        grad_logw, M);
+}
+
+// The checked KArgs of epnp_evaluate_cost_f32 and its split form, or the refusal.
+static int cost_args(KArgs& a, const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                     const float* lb, const float* ub, const float* delta, const float* poses, float* cost,
+                     int S, int B, int N, int dof, float z_min) {
+    a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
+    a.poses = poses; a.cost_out = cost; a.S_eval = S;
+    epnp_default_params(&a.p, dof);
+    a.p.z_min = z_min;
+    const int rc = check_common(a);
+    if (rc != EPNP_OK) return rc;
+    return (!poses || !cost || S < 0) ? EPNP_ERR_BAD_ARG : EPNP_OK;
 }
 
 int epnp_evaluate_cost_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
                            const float* lb, const float* ub, const float* delta, const float* poses, float* cost,
                            int S, int B, int N, int dof, float z_min, void* stream) {
-    KArgs a{};
-    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
-    a.poses = poses; a.cost_out = cost; a.S_eval = S; a.B = B; a.N = N;
-    epnp_default_params(&a.p, dof);
-    a.p.z_min = z_min;
-    int rc = check_common(a);
-    if (rc != EPNP_OK) return rc;
-    if (!poses || !cost || S < 0) return EPNP_ERR_BAD_ARG;
-    if (S == 0) return EPNP_OK;
-    if (dof == 6) return launch_cta_per_object(cost_kernel<6>, a, plan_obj<6>(N).total_bytes, (cudaStream_t)stream);
-    return launch_cta_per_object(cost_kernel<4>, a, plan_obj<4>(N).total_bytes, (cudaStream_t)stream);
+    KArgs a;
+    const int rc = cost_args(a, x3d, x2d, w2d, cam_mats, lb, ub, delta, poses, cost, S, B, N, dof, z_min);
+    if (rc != EPNP_OK || S == 0) return rc;
+    return by_dof(dof, [&](auto D) {
+        return launch_cta_per_object(cost_kernel<D>, a, plan_obj<D>(N).total_bytes, (cudaStream_t)stream);
+    });
 }
 
 int epnp_evaluate_cost_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
                                  const float* lb, const float* ub, const float* delta, const float* poses, float* cost,
                                  int S, int B, int N, int dof, float z_min, int cluster_ctas, void* stream) {
-    KArgs a{};
-    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
-    a.poses = poses; a.cost_out = cost; a.S_eval = S; a.B = B; a.N = N;
-    epnp_default_params(&a.p, dof);
-    a.p.z_min = z_min;
-    int rc = check_common(a);
+    KArgs a;
+    const int rc = cost_args(a, x3d, x2d, w2d, cam_mats, lb, ub, delta, poses, cost, S, B, N, dof, z_min);
     if (rc != EPNP_OK) return rc;
-    if (!poses || !cost || S < 0) return EPNP_ERR_BAD_ARG;
     const int ctas = split_ctas_for(dof, N, 0, 0, cluster_ctas);
     if (ctas < 0) return ctas;
     if (S == 0) return EPNP_OK;
     const int smem_bytes = split_smem_bytes(dof, N, ctas, 0, 0);
-    if (dof == 6) return launch_cluster_per_object<COST_SPLIT_TILE>(cost_split_kernel<6>, a, smem_bytes, ctas, (cudaStream_t)stream);
-    return launch_cluster_per_object<COST_SPLIT_TILE>(cost_split_kernel<4>, a, smem_bytes, ctas, (cudaStream_t)stream);
+    return by_dof(dof, [&](auto D) {
+        return launch_cluster<COST_SPLIT_TILE>(cost_split_kernel<D>, a, B, smem_bytes, ctas, (cudaStream_t)stream);
+    });
 }
 
 int epnp_evaluate_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
                       const float* lb, const float* ub, const float* delta, const float* pose,
                       float* residual, float* jac, float* cost, int clip_jac,
                       int B, int N, int dof, float z_min, float huber_eps, void* stream) {
-    KArgs a{};
-    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
-    a.poses = pose; a.B = B; a.N = N;
+    KArgs a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
+    a.poses = pose;
     epnp_default_params(&a.p, dof);
     a.p.z_min = z_min;
-    int rc = check_common(a);
+    const int rc = check_common(a);
     if (rc != EPNP_OK) return rc;
     if (!pose) return EPNP_ERR_BAD_ARG;
     if (B == 0) return EPNP_OK;
-    if (dof == 6) EPNP_LAUNCH(evaluate_full_kernel<6>, B, NT, 0, (cudaStream_t)stream, a, residual, jac, cost, clip_jac, huber_eps);
-    else EPNP_LAUNCH(evaluate_full_kernel<4>, B, NT, 0, (cudaStream_t)stream, a, residual, jac, cost, clip_jac, huber_eps);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+    return by_dof(dof, [&](auto D) {
+        return launch_plain(evaluate_full_kernel<D>, B, NT, 0, SmemAttr::none, (cudaStream_t)stream, a, residual, jac,
+                            cost, clip_jac, huber_eps);
+    });
 }
 
 int epnp_lm_solve_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
@@ -1770,15 +1791,30 @@ int epnp_lm_solve_f32(const float* x3d, const float* x2d, const float* w2d, cons
                       float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus, float* cost_init,
                       int B, int N, const EpnpParams* p, void* stream) {
     if (!p) return EPNP_ERR_BAD_ARG;
-    KArgs a{};
-    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
+    KArgs a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
     a.pose_init = pose_init; a.pose_opt = pose_opt; a.pose_cov = pose_cov; a.cost = cost;
-    a.pose_plus = pose_opt_plus; a.cost_init = cost_init; a.B = B; a.N = N; a.p = *p;
-    int rc = check_common(a);
+    a.pose_plus = pose_opt_plus; a.cost_init = cost_init; a.p = *p;
+    const int rc = check_common(a);
     if (rc != EPNP_OK) return rc;
     if (!pose_init || !pose_opt || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
     a.cov_stride = p->dof * p->dof;
-    return p->dof == 6 ? launch_lm<6>(a, (cudaStream_t)stream) : launch_lm<4>(a, (cudaStream_t)stream);
+    return launch_lm(a, (cudaStream_t)stream);
+}
+
+// The checked arguments of epnp_gn_plus_backward_f32 and its split form, or the refusal.
+static int gn_bw_args(GnBwArgs& g, const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                      const float* lb, const float* ub, const float* delta, const float* pose,
+                      const float* grad_pose_plus, float* grad_x3d, float* grad_x2d, float* grad_w2d,
+                      float* grad_delta, int B, int N, int dof, float z_min, float eps, float huber_eps) {
+    KArgs& a = g.k;
+    a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
+    a.poses = pose;
+    epnp_default_params(&a.p, dof);
+    a.p.z_min = z_min; a.p.eps = eps; a.p.huber_eps = huber_eps;
+    g.gplus = grad_pose_plus; g.gx3d = grad_x3d; g.gx2d = grad_x2d; g.gw2d = grad_w2d; g.gdelta = grad_delta;
+    const int rc = check_common(a);
+    if (rc != EPNP_OK) return rc;
+    return (!pose || !grad_pose_plus) ? EPNP_ERR_BAD_ARG : EPNP_OK;
 }
 
 int epnp_gn_plus_backward_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
@@ -1787,33 +1823,15 @@ int epnp_gn_plus_backward_f32(const float* x3d, const float* x2d, const float* w
                               float* grad_delta, int B, int N, int dof, float z_min, float eps, float huber_eps,
                               void* stream) {
     GnBwArgs g{};
-    KArgs& a = g.k;
-    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
-    a.poses = pose; a.B = B; a.N = N;
-    epnp_default_params(&a.p, dof);
-    a.p.z_min = z_min; a.p.eps = eps; a.p.huber_eps = huber_eps;
-    g.gplus = grad_pose_plus; g.gx3d = grad_x3d; g.gx2d = grad_x2d; g.gw2d = grad_w2d; g.gdelta = grad_delta;
-    int rc = check_common(a);
-    if (rc != EPNP_OK) return rc;
-    if (!pose || !grad_pose_plus) return EPNP_ERR_BAD_ARG;
-    if (B == 0) return EPNP_OK;
-    const int smem_bytes = (dof == 6) ? plan_obj<6>(N).total_bytes : plan_obj<4>(N).total_bytes;
-    if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
-    a.use_tma = tma_ok(a);
-    rc = device_sms(&a.num_sms);
-    if (rc != EPNP_OK) return rc;
-    cudaError_t e;
-    if (dof == 6) {
-        e = cudaFuncSetAttribute(gn_plus_backward_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-        if (e != cudaSuccess) return cuda_fail(e);
-        EPNP_LAUNCH(gn_plus_backward_kernel<6>, B, NT, smem_bytes, (cudaStream_t)stream, g);
-    } else {
-        e = cudaFuncSetAttribute(gn_plus_backward_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-        if (e != cudaSuccess) return cuda_fail(e);
-        EPNP_LAUNCH(gn_plus_backward_kernel<4>, B, NT, smem_bytes, (cudaStream_t)stream, g);
-    }
-    e = cudaGetLastError();
-    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+    const int rc = gn_bw_args(g, x3d, x2d, w2d, cam_mats, lb, ub, delta, pose, grad_pose_plus, grad_x3d, grad_x2d,
+                              grad_w2d, grad_delta, B, N, dof, z_min, eps, huber_eps);
+    if (rc != EPNP_OK || B == 0) return rc;
+    return by_dof(dof, [&](auto D) {
+        const int smem_bytes = plan_obj<D>(N).total_bytes;
+        const int rc = prepare_resident(g.k, smem_bytes);
+        if (rc != EPNP_OK) return rc;
+        return launch_plain(gn_plus_backward_kernel<D>, B, NT, smem_bytes, SmemAttr::size, (cudaStream_t)stream, g);
+    });
 }
 
 int epnp_gn_plus_backward_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
@@ -1822,21 +1840,15 @@ int epnp_gn_plus_backward_split_f32(const float* x3d, const float* x2d, const fl
                                     float* grad_delta, int B, int N, int dof, float z_min, float eps, float huber_eps,
                                     int cluster_ctas, void* stream) {
     GnBwArgs g{};
-    KArgs& a = g.k;
-    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
-    a.poses = pose; a.B = B; a.N = N;
-    epnp_default_params(&a.p, dof);
-    a.p.z_min = z_min; a.p.eps = eps; a.p.huber_eps = huber_eps;
-    g.gplus = grad_pose_plus; g.gx3d = grad_x3d; g.gx2d = grad_x2d; g.gw2d = grad_w2d; g.gdelta = grad_delta;
-    int rc = check_common(a);
+    const int rc = gn_bw_args(g, x3d, x2d, w2d, cam_mats, lb, ub, delta, pose, grad_pose_plus, grad_x3d, grad_x2d,
+                              grad_w2d, grad_delta, B, N, dof, z_min, eps, huber_eps);
     if (rc != EPNP_OK) return rc;
-    if (!pose || !grad_pose_plus) return EPNP_ERR_BAD_ARG;
     const int ctas = split_ctas_for(dof, N, 0, 0, cluster_ctas);
     if (ctas < 0) return ctas;
     const int smem_bytes = split_smem_bytes(dof, N, ctas, 0, 0);
-    if (dof == 6)
-        return launch_cluster_per_object<GNBW_SPLIT_T>(gn_plus_backward_split_kernel<6>, g, smem_bytes, ctas, (cudaStream_t)stream);
-    return launch_cluster_per_object<GNBW_SPLIT_T>(gn_plus_backward_split_kernel<4>, g, smem_bytes, ctas, (cudaStream_t)stream);
+    return by_dof(dof, [&](auto D) {
+        return launch_cluster<GNBW_SPLIT_T>(gn_plus_backward_split_kernel<D>, g, B, smem_bytes, ctas, (cudaStream_t)stream);
+    });
 }
 
 int epnp_rslm_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
@@ -1845,32 +1857,20 @@ int epnp_rslm_f32(const float* x3d, const float* x2d, const float* w2d, const fl
                   int P, int n, int B, int N, const EpnpParams* p, void* stream) {
     if (!p) return EPNP_ERR_BAD_ARG;
     RslmArgs r{};
-    KArgs& a = r.k;
-    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
-    a.B = B; a.N = N; a.p = *p;
+    r.k = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
+    r.k.p = *p;
     r.inds = inds; r.start = start; r.pose_best = pose_best; r.cost_best = cost_best;
     r.pose_all = pose_all; r.cost_all = cost_all; r.P = P; r.n = n;
-    int rc = check_common(a);
+    const int rc = check_common(r.k);
     if (rc != EPNP_OK) return rc;
     if (!inds || !start || !pose_best || !cost_best || P <= 0 || n <= 0 || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
     if (B == 0) return EPNP_OK;
-    const int smem_bytes = (p->dof == 6) ? plan_obj<6>(N).total_bytes : plan_obj<4>(N).total_bytes;
-    if ((size_t)smem_bytes > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
-    a.use_tma = tma_ok(a);
-    rc = device_sms(&a.num_sms);
-    if (rc != EPNP_OK) return rc;
-    cudaError_t e;
-    if (p->dof == 6) {
-        e = cudaFuncSetAttribute(rslm_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-        if (e != cudaSuccess) return cuda_fail(e);
-        EPNP_LAUNCH(rslm_kernel<6>, B, NT, smem_bytes, (cudaStream_t)stream, r);
-    } else {
-        e = cudaFuncSetAttribute(rslm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-        if (e != cudaSuccess) return cuda_fail(e);
-        EPNP_LAUNCH(rslm_kernel<4>, B, NT, smem_bytes, (cudaStream_t)stream, r);
-    }
-    e = cudaGetLastError();
-    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+    return by_dof(p->dof, [&](auto D) {
+        const int smem_bytes = plan_obj<D>(N).total_bytes;
+        const int rc = prepare_resident(r.k, smem_bytes);
+        if (rc != EPNP_OK) return rc;
+        return launch_plain(rslm_kernel<D>, B, NT, smem_bytes, SmemAttr::size, (cudaStream_t)stream, r);
+    });
 }
 
 // epnp_rslm_draw_f32 and, with seed_ptr != NULL, epnp_rslm_draw_seedptr_f32 (the seed then comes from *seed_ptr).
@@ -1883,24 +1883,12 @@ static int rslm_draw(const float* x3d, const float* x2d, const float* w2d, const
     if (B == 0) return EPNP_OK;
     const size_t smem = (size_t)((N + 3) & ~3) * sizeof(float) + (size_t)n * NT * (sizeof(float) + sizeof(int));
     if (smem + 2048 > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
-    RslmDrawArgs r{x3d, x2d, w2d, cam_mats, t_init, inds, start, t_out, seed, obj_offset, P, n, B, N, eps};
-    cudaError_t e;
-    if (seed_ptr) {
-        const auto kern = dof == 6 ? rslm_draw_seedptr_kernel<6> : rslm_draw_seedptr_kernel<4>;
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return cuda_fail(e);
-        EPNP_LAUNCH(kern, B, NT, smem, (cudaStream_t)stream, r, seed_ptr);
-    } else if (dof == 6) {
-        e = cudaFuncSetAttribute(rslm_draw_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return cuda_fail(e);
-        EPNP_LAUNCH(rslm_draw_kernel<6>, B, NT, smem, (cudaStream_t)stream, r);
-    } else {
-        e = cudaFuncSetAttribute(rslm_draw_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return cuda_fail(e);
-        EPNP_LAUNCH(rslm_draw_kernel<4>, B, NT, smem, (cudaStream_t)stream, r);
-    }
-    e = cudaGetLastError();
-    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+    const RslmDrawArgs r{x3d, x2d, w2d, cam_mats, t_init, inds, start, t_out, seed, obj_offset, P, n, B, N, eps};
+    const cudaStream_t s = (cudaStream_t)stream;
+    return by_dof(dof, [&](auto D) {
+        if (seed_ptr) return launch_plain(rslm_draw_seedptr_kernel<D>, B, NT, (int)smem, SmemAttr::size, s, r, seed_ptr);
+        return launch_plain(rslm_draw_kernel<D>, B, NT, (int)smem, SmemAttr::size, s, r);
+    });
 }
 
 int epnp_rslm_draw_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats, const float* t_init,
@@ -1924,13 +1912,8 @@ int epnp_epnp_init_f32(const float* x3d, const float* x2d, const float* w2d, con
     if (N > epnp_max_points(6, 0, 0)) return EPNP_ERR_TOO_MANY_POINTS;
     if (w2d && epnp::min_selected(N, conf_quantile) < 4) return EPNP_ERR_BAD_ARG;
     if (B == 0) return EPNP_OK;
-    const int smem = epnp_init_smem_bytes(N);
-    cudaError_t e = cudaFuncSetAttribute(epnp_init_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return cuda_fail(e);
     const EpnpInitArgs a{x3d, x2d, w2d, cam_mats, pose, n_sel, N, conf_quantile};
-    EPNP_LAUNCH(epnp_init_kernel, B, NT, smem, (cudaStream_t)stream, a);
-    e = cudaGetLastError();
-    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+    return launch_plain(epnp_init_kernel, B, NT, epnp_init_smem_bytes(N), SmemAttr::size, (cudaStream_t)stream, a);
 }
 
 int epnp_epnp_init_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
@@ -1952,22 +1935,17 @@ int epnp_amis_f32(const float* x3d, const float* x2d, const float* w2d, const fl
                   uint64_t seed, uint32_t obj_offset, float* pose_samples, float* logw, float* proposals,
                   int B, int N, const EpnpParams* p, void* stream) {
     if (!p) return EPNP_ERR_BAD_ARG;
-    KArgs a{};
-    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
+    KArgs a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
     a.pose_opt_in = pose_opt; a.pose_cov_in = pose_cov;
     a.noise_n3 = noise_normal; a.noise_chi2 = noise_chi2; a.noise_rot = noise_rot;
     a.seed = seed; a.obj_offset = obj_offset;
-    a.pose_samples = pose_samples; a.logw = logw; a.proposals = proposals; a.B = B; a.N = N; a.p = *p;
+    a.pose_samples = pose_samples; a.logw = logw; a.proposals = proposals; a.p = *p;
     a.prof = g_prof_buffer;
-    int rc = check_common(a);
+    const int rc = check_amis_call(a);
     if (rc != EPNP_OK) return rc;
-    rc = check_amis_params(*p);
-    if (rc != EPNP_OK) return rc;
-    if (!pose_opt || !pose_cov || !pose_samples || !logw) return EPNP_ERR_BAD_ARG;
-    const bool any = noise_normal || noise_chi2 || noise_rot, all = noise_normal && noise_chi2 && noise_rot;
-    if (any && !all) return EPNP_ERR_BAD_ARG;
+    if (!pose_opt || !pose_cov) return EPNP_ERR_BAD_ARG;
     a.cov_stride = p->dof * p->dof;
-    return p->dof == 6 ? launch_amis<6>(a, nullptr, (cudaStream_t)stream) : launch_amis<4>(a, nullptr, (cudaStream_t)stream);
+    return launch_amis(a, nullptr, (cudaStream_t)stream);
 }
 
 // The checked KArgs of the fused calls (resident and split, by-value and seed-pointer forms), or the refusal.
@@ -1978,21 +1956,16 @@ static int fused_args(KArgs& a, const float* x3d, const float* x2d, const float*
                       float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus, float* cost_init,
                       float* pose_samples, float* logw, float* proposals, int B, int N, const EpnpParams* p) {
     if (!p) return EPNP_ERR_BAD_ARG;
-    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
+    a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
     a.pose_init = pose_init;
     a.noise_n3 = noise_normal; a.noise_chi2 = noise_chi2; a.noise_rot = noise_rot;
     a.seed = seed; a.obj_offset = obj_offset;
     a.pose_opt = pose_opt; a.pose_cov = pose_cov; a.cost = cost; a.pose_plus = pose_opt_plus; a.cost_init = cost_init;
-    a.pose_samples = pose_samples; a.logw = logw; a.proposals = proposals; a.B = B; a.N = N; a.p = *p;
+    a.pose_samples = pose_samples; a.logw = logw; a.proposals = proposals; a.p = *p;
     a.prof = g_prof_buffer;
-    int rc = check_common(a);
+    const int rc = check_amis_call(a);
     if (rc != EPNP_OK) return rc;
-    rc = check_amis_params(*p);
-    if (rc != EPNP_OK) return rc;
-    if (!pose_init || !pose_opt || !pose_samples || !logw || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
-    const bool any = noise_normal || noise_chi2 || noise_rot, all = noise_normal && noise_chi2 && noise_rot;
-    if (any && !all) return EPNP_ERR_BAD_ARG;
-    return EPNP_OK;
+    return (!pose_init || !pose_opt || p->lm_iter < 0) ? EPNP_ERR_BAD_ARG : EPNP_OK;
 }
 
 int epnp_lm_amis_fused_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
@@ -2061,17 +2034,15 @@ static int push_args(KArgs& a, PushArgs& push, const float* x3d, const float* x2
                      float* const* peer_logw, float* const* peer_pose, int n_peers, int B, int N, const EpnpParams* p) {
     if (!p) return EPNP_ERR_BAD_ARG;
     if (n_peers < 0 || n_peers > EPNP_MAX_PEERS || (n_peers > 0 && (!peer_logw || !peer_pose))) return EPNP_ERR_BAD_ARG;
-    a.x3d = x3d; a.x2d = x2d; a.w2d = w2d; a.cam = cam_mats; a.lb = lb; a.ub = ub; a.delta = delta;
+    a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
     a.pose_init = pose_init;
     a.seed = seed; a.obj_offset = obj_offset;
     a.pose_opt = pose_opt; a.pose_cov = pose_cov; a.cost = cost;
-    a.pose_samples = pose_samples; a.logw = logw; a.B = B; a.N = N; a.p = *p;
+    a.pose_samples = pose_samples; a.logw = logw; a.p = *p;
     a.prof = g_prof_buffer;
-    int rc = check_common(a);
+    const int rc = check_amis_call(a);
     if (rc != EPNP_OK) return rc;
-    rc = check_amis_params(*p);
-    if (rc != EPNP_OK) return rc;
-    if (!pose_init || !pose_opt || !pose_samples || !logw || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
+    if (!pose_init || !pose_opt || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
     push = PushArgs{peer_logw, peer_pose, n_peers};
     return EPNP_OK;
 }
@@ -2104,10 +2075,8 @@ int epnp_lm_amis_fused_split_push_f32(const float* x3d, const float* x2d, const 
     if (rc != EPNP_OK || n_peers == 0 || B == 0) return rc;
     const size_t blocks = ((size_t)B * p->mc_samples + 4 * NT - 1) / (4 * NT);     // one float4 of logw per thread
     const int grid = blocks < 1024 ? (int)blocks : 1024;
-    EPNP_LAUNCH(push_split_kernel, grid, NT, 0, (cudaStream_t)stream, logw, pose_opt, push, (size_t)obj_offset, B,
-                p->mc_samples, p->dof == 6 ? 7 : 4);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+    return launch_plain(push_split_kernel, grid, NT, 0, SmemAttr::none, (cudaStream_t)stream, logw, pose_opt, push,
+                        (size_t)obj_offset, B, p->mc_samples, p->dof == 6 ? 7 : 4);
 }
 
 int epnp_cost_backward_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
@@ -2127,20 +2096,13 @@ int epnp_cost_backward_f32(const float* x3d, const float* x2d, const float* w2d,
     a.gx3d = grad_x3d; a.gx2d = grad_x2d; a.gw2d = grad_w2d; a.gdelta = grad_delta;
     a.B = B; a.N = N; a.z_min = z_min;
     const int smem = (BW_POSE_TILE * 13 + 2 * NW * 32) * 4;
-    cudaError_t e;
-    int dev = 0, sms = 0;
-    if ((e = cudaGetDevice(&dev)) != cudaSuccess) return cuda_fail(e);
-    if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return cuda_fail(e);
+    int sms = 0;
+    const int rc = device_sms(&sms);
+    if (rc != EPNP_OK) return rc;
     const int grid = B < sms * 4 ? B : sms * 4;
-    if (dof == 6) {
-        if ((e = cudaFuncSetAttribute(cost_backward_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return cuda_fail(e);
-        EPNP_LAUNCH(cost_backward_kernel<6>, grid, NT, smem, (cudaStream_t)stream, a);
-    } else {
-        if ((e = cudaFuncSetAttribute(cost_backward_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return cuda_fail(e);
-        EPNP_LAUNCH(cost_backward_kernel<4>, grid, NT, smem, (cudaStream_t)stream, a);
-    }
-    e = cudaGetLastError();
-    return e == cudaSuccess ? EPNP_OK : cuda_fail(e);
+    return by_dof(dof, [&](auto D) {
+        return launch_plain(cost_backward_kernel<D>, grid, NT, smem, SmemAttr::size, (cudaStream_t)stream, a);
+    });
 }
 
 // ---- host-buffer entry point: chunked H2D -> fused kernel -> D2H on two internal streams
@@ -2333,11 +2295,11 @@ int epnp_lm_amis_fused_host_f32(const float* x3d_host, const float* x2d_host, co
     int wave = 0;                               // objects in flight: SMs x resident AMIS CTAs per SM
     if (n_chunks == 0) {
         if (check_amis_params(*p) != EPNP_OK) return EPNP_ERR_BAD_ARG;
-        wave = (p->dof == 6)
-            ? (amis_dense(N) ? resident_objects<AMIS_T_DENSE>(amis_kernel<6, AMIS_T_DENSE>, amis_smem_bytes<6>(N, p->mc_samples))
-                             : resident_objects<NT>(amis_kernel<6, NT>, amis_smem_bytes<6>(N, p->mc_samples)))
-            : (amis_dense(N) ? resident_objects<AMIS_T_DENSE>(amis_kernel<4, AMIS_T_DENSE>, amis_smem_bytes<4>(N, p->mc_samples))
-                             : resident_objects<NT>(amis_kernel<4, NT>, amis_smem_bytes<4>(N, p->mc_samples)));
+        wave = by_dof(p->dof, [&](auto D) {
+            return by_amis_threads(N, [&](auto T) {
+                return resident_objects<T>(amis_kernel<D, T>, amis_smem_bytes<D>(N, p->mc_samples));
+            });
+        });
     }
     return host_pipeline(fused_resident_chunk, 0, wave, x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host, ub_host,
                          delta_host, pose_init_host, seed, obj_offset, pose_opt_host, pose_cov_host, cost_host,
