@@ -1555,6 +1555,11 @@ int resident_objects(Kern kern, int smem_bytes) {
     return sms * occ;
 }
 
+// Fast mode takes the covariance, cost and cost_init from its Gauss-Newton steps' evaluations (each before its step):
+// with lm_iter = 0 nothing evaluates, so none of the three has a value (the reference's has none either).  The calls
+// that would return one refuse instead.
+bool fast_mode_without_steps(const Params& p) { return p.fast_mode != 0 && p.lm_iter == 0; }
+
 int check_amis_params(const Params& p) {
     if (p.mc_iter <= 0 || p.mc_iter > MAX_ITER || p.mc_samples <= 0 || p.mc_samples % p.mc_iter != 0) return EPNP_ERR_BAD_ARG;
     if (p.acg_mle_iter < 0) return EPNP_ERR_BAD_ARG;
@@ -1797,6 +1802,7 @@ int epnp_lm_solve_f32(const float* x3d, const float* x2d, const float* w2d, cons
     const int rc = check_common(a);
     if (rc != EPNP_OK) return rc;
     if (!pose_init || !pose_opt || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
+    if (fast_mode_without_steps(*p) && (pose_cov || cost || cost_init)) return EPNP_ERR_BAD_ARG;
     a.cov_stride = p->dof * p->dof;
     return launch_lm(a, (cudaStream_t)stream);
 }
@@ -1965,7 +1971,7 @@ static int fused_args(KArgs& a, const float* x3d, const float* x2d, const float*
     a.prof = g_prof_buffer;
     const int rc = check_amis_call(a);
     if (rc != EPNP_OK) return rc;
-    return (!pose_init || !pose_opt || p->lm_iter < 0) ? EPNP_ERR_BAD_ARG : EPNP_OK;
+    return (!pose_init || !pose_opt || p->lm_iter < 0 || fast_mode_without_steps(*p)) ? EPNP_ERR_BAD_ARG : EPNP_OK;
 }
 
 int epnp_lm_amis_fused_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
@@ -2042,7 +2048,7 @@ static int push_args(KArgs& a, PushArgs& push, const float* x3d, const float* x2
     a.prof = g_prof_buffer;
     const int rc = check_amis_call(a);
     if (rc != EPNP_OK) return rc;
-    if (!pose_init || !pose_opt || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
+    if (!pose_init || !pose_opt || p->lm_iter < 0 || fast_mode_without_steps(*p)) return EPNP_ERR_BAD_ARG;
     push = PushArgs{peer_logw, peer_pose, n_peers};
     return EPNP_OK;
 }
@@ -2318,7 +2324,8 @@ int epnp_lm_amis_fused_split_host_f32(const float* x3d_host, const float* x2d_ho
                              pose_init_host, pose_opt_host, logw_host, workspace, workspace_bytes, B, N, p);
     if (rc != EPNP_OK || B == 0) return rc;
     // every refusal of the chunk solves, made here, before the first copy is enqueued
-    if ((p->dof != 4 && p->dof != 6) || check_amis_params(*p) != EPNP_OK || p->lm_iter < 0) return EPNP_ERR_BAD_ARG;
+    if ((p->dof != 4 && p->dof != 6) || check_amis_params(*p) != EPNP_OK || p->lm_iter < 0 || fast_mode_without_steps(*p))
+        return EPNP_ERR_BAD_ARG;
     int wave = 0;                               // objects in flight: co-resident clusters
     const int ctas = split_lm_amis_plan(*p, B, N, cluster_ctas, &wave);
     if (ctas < 0) return ctas;

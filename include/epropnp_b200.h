@@ -212,7 +212,11 @@ int epnp_epnp_init_split_f32(const float* x3d, const float* x2d, const float* w2
  * fast mode :136-152) plus, when pose_opt_plus != NULL, the extra Gauss-Newton step of
  * LMSolver.forward (:66-68, gn_step :243-253, pose_add :255-265).
  *   pose_opt (B, D); pose_cov [opt] (B, dof, dof) = inverse(J^T J + eps I); cost [opt] (B);
- *   cost_init [opt] (B) = cost at pose_init (what monte_carlo_forward returns, epropnp.py:121-124) */
+ *   cost_init [opt] (B) = cost at pose_init (what monte_carlo_forward returns, epropnp.py:121-124)
+ * In fast mode pose_cov, cost and cost_init come from the evaluation before a Gauss-Newton step, so fast_mode != 0
+ * with lm_iter = 0 returns EPNP_ERR_BAD_ARG (for any B) when any of the three is requested; pose_opt alone (= pose_init)
+ * and pose_opt_plus stay allowed.  The fused calls (resident, split, seed-pointer, push and host-buffer forms) always
+ * compute the covariance and refuse that combination outright.                                                     */
 int epnp_lm_solve_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
                       const float* lb, const float* ub, const float* delta, const float* pose_init,
                       float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus,

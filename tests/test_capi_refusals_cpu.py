@@ -135,6 +135,8 @@ PARAMS_OR_DOF = {n for n in ALL if _has(n, "dof") or _params_call(n)}
 BOUNDED = {n for n in ALL if _has(n, "lb")}
 AMIS = {n for n in ALL if _amis(n)}
 LM = {n for n in ALL if _params_call(n) and n != "epnp_amis_f32"}
+FUSED = {n for n in AMIS if n != "epnp_amis_f32"}
+FAST0 = {"p.fast_mode": 1, "p.lm_iter": 0}
 NOISE = {n for n in ALL if _has(n, "noise_n")}
 SPLIT = {n for n in ALL if _split(n)}
 PUSH = {n for n in ALL if "push" in n}
@@ -156,6 +158,17 @@ CASES = [
     ("I>8", AMIS, {"p.mc_iter": 16}, (BAD_ARG, BAD_ARG), {n: (BAD_ARG, OK) for n in HOST}),
     ("acg_mle_iter<0", AMIS, {"p.acg_mle_iter": -1}, (BAD_ARG, BAD_ARG), {n: (BAD_ARG, OK) for n in HOST}),
     ("lm_iter<0", LM, {"p.lm_iter": -1}, (BAD_ARG, BAD_ARG), {n: (BAD_ARG, OK) for n in HOST}),
+    # fast mode with no Gauss-Newton step has no covariance, cost or cost_init to return
+    ("fast_no_steps", FUSED, FAST0, (BAD_ARG, BAD_ARG), {n: (BAD_ARG, OK) for n in HOST}),
+    ("fast_no_steps_all_outputs", {"epnp_lm_solve_f32"}, FAST0, (BAD_ARG, BAD_ARG), {}),
+    ("fast_no_steps_cov", {"epnp_lm_solve_f32"}, dict(FAST0, cost=None, pose_plus=None, cost_init=None),
+     (BAD_ARG, BAD_ARG), {}),
+    ("fast_no_steps_cost", {"epnp_lm_solve_f32"}, dict(FAST0, pose_cov=None, pose_plus=None, cost_init=None),
+     (BAD_ARG, BAD_ARG), {}),
+    ("fast_no_steps_cost_init", {"epnp_lm_solve_f32"}, dict(FAST0, pose_cov=None, cost=None, pose_plus=None),
+     (BAD_ARG, BAD_ARG), {}),
+    ("fast_no_steps_pose_only", {"epnp_lm_solve_f32"}, dict(FAST0, pose_cov=None, cost=None, cost_init=None),
+     (None, OK), {}),
     ("noise_normal_only", NOISE, {"noise_chi2": None, "noise_rot": None}, (BAD_ARG, BAD_ARG), {}),
     ("noise_rot_missing", NOISE, {"noise_rot": None}, (BAD_ARG, BAD_ARG), {}),
     ("cluster=1", SPLIT, {"cluster_ctas": 1}, (BAD_ARG, BAD_ARG), {n: (BAD_ARG, OK) for n in HOST}),
