@@ -10,6 +10,8 @@
 //                                    4 points per thread between block barriers (DESIGN.md section 4).
 //   cost_kernel, evaluate_full_kernel, rslm_draw_kernel, rslm_kernel, cost_backward_kernel, gn_plus_backward_kernel, adaptive_delta_kernel,
 //   mc_epilogue_kernel, mc_lse_backward_kernel      the steps either side of the path (CTA per object).
+//   cost_pose_backward_kernel, cost_pose_backward_split_kernel    the cost's gradient with respect to stacked poses: thread per
+//                                    pose over the resident points; the split form on cost_split_kernel's clusters.
 //   epnp_init_kernel (pnp_epnp.cuh)  EPnP initialiser with the confidence-quantile point selection, fp64, CTA per object.
 //   amis_split_kernel (pnp_amis.cuh), cost_split_kernel, gn_plus_backward_split_kernel, epnp_init_split_kernel   the AMIS
 //                                    loop, the stacked-pose cost, the pose_opt_plus backward and the EPnP initialiser for
@@ -820,6 +822,196 @@ __global__ void __launch_bounds__(NT, 4) cost_backward_kernel(const BwArgs a) {
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Backward of the cost with respect to the POSE: grad_pose[b, p] = grad[b, p] * d cost(pose[b, p]) / d pose[b, p] for
+// stacked poses given object-major.  The shape of the work is cost_kernel's: one CTA per object, its points resident as
+// pair records, thread <-> pose, every thread sweeping all points as shared-memory broadcasts.  Each thread owns its
+// output row: no atomics, no cross-thread sum, so a row depends on nothing but its object and its pose.
+// Per point the sweep takes the forward chain of pair_cost_backward and stops at h = d cost / d (xh, yh, zh), the
+// gradient in homogeneous image coordinates K x_cam (zero where the reference's autograd gives zero: no gradient
+// through a depth clamped at z_min, none through a coordinate clamped at lb / ub, none at s = 0; rho' = 1 up to delta,
+// delta / s above).  It accumulates 12 sums per pose, the same for both DOF: sum h (3) and sum h x3d^T (3 x 3).  After
+// the sweep d cost / d t = K^T sum h, G = d cost / d R = K^T sum h x3d^T, and the rotation parameters get <G, dR/dq_k>
+// for the four raw components of the un-normalised quat_to_rot (not a tangent vector), or <G, dR/dyaw>.
+struct PoseBwArgs {
+    KArgs k;                    // correspondences, camera, bounds, delta, poses = (B, P, D) object-major, p.z_min
+    const float* grad;          // (B, P)  dL/d cost
+    float* gpose;               // (B, P, D)
+    int P;
+};
+
+template <bool BOUNDED>
+__device__ __forceinline__ void pair_pose_grad(const float (&P)[12], const Cam& cam, float delta, const float4 q0,
+                                               const float4 q1, const float4 q2, const float4 q3, float2 (&h)[12]) {
+    const float2 X = make_float2(q0.x, q0.y), Y = make_float2(q0.z, q0.w), Z = make_float2(q1.x, q1.y);
+    const float2 nu = make_float2(q1.z, q1.w), nv = make_float2(q2.x, q2.y);
+    const float2 wu = make_float2(q2.z, q2.w), wv = make_float2(q3.x, q3.y);
+    const float2 xh = v2fma(splat(P[0]), X, v2fma(splat(P[1]), Y, v2fma(splat(P[2]), Z, splat(P[3]))));
+    const float2 yh = v2fma(splat(P[4]), X, v2fma(splat(P[5]), Y, v2fma(splat(P[6]), Z, splat(P[7]))));
+    const float2 zh = v2fma(splat(P[8]), X, v2fma(splat(P[9]), Y, v2fma(splat(P[10]), Z, splat(P[11]))));
+    const float2 iz = make_float2(FastRcp()(fmaxf(zh.x, cam.z_min)), FastRcp()(fmaxf(zh.y, cam.z_min)));
+    const float2 px = v2mul(xh, iz), py = v2mul(yh, iz);
+    float2 pxc = px, pyc = py;
+    if (BOUNDED) {
+        pxc.x = fminf(fmaxf(px.x, cam.lbx), cam.ubx); pxc.y = fminf(fmaxf(px.y, cam.lbx), cam.ubx);
+        pyc.x = fminf(fmaxf(py.x, cam.lby), cam.uby); pyc.y = fminf(fmaxf(py.y, cam.lby), cam.uby);
+    }
+    const float2 rx = v2mul(v2add(pxc, nu), wu), ry = v2mul(v2add(pyc, nv), wv);
+    const float2 s2 = v2fma(rx, rx, v2mul(ry, ry));
+    const float2 rs = make_float2(FastRsqrt()(fmaxf(s2.x, 1e-30f)), FastRsqrt()(fmaxf(s2.y, 1e-30f)));
+    const float2 s = v2mul(s2, rs);
+    const float2 k = make_float2(s.x <= delta ? 1.f : delta * rs.x, s.y <= delta ? 1.f : delta * rs.y);    // rho'
+    float2 gpx = v2mul(v2mul(k, rx), wu), gpy = v2mul(v2mul(k, ry), wv);
+    if (BOUNDED) {
+        gpx.x = (pxc.x == px.x) ? gpx.x : 0.f; gpx.y = (pxc.y == px.y) ? gpx.y : 0.f;
+        gpy.x = (pyc.x == py.x) ? gpy.x : 0.f; gpy.y = (pyc.y == py.y) ? gpy.y : 0.f;
+    }
+    const float2 gxh = v2mul(gpx, iz), gyh = v2mul(gpy, iz);
+    const float2 tz = v2fma(gxh, px, v2mul(gyh, py));
+    const float2 gzh = make_float2(zh.x >= cam.z_min ? -tz.x : 0.f, zh.y >= cam.z_min ? -tz.y : 0.f);
+    h[0] = v2add(h[0], gxh); h[1] = v2add(h[1], gyh); h[2] = v2add(h[2], gzh);
+    h[3] = v2fma(gxh, X, h[3]); h[4] = v2fma(gxh, Y, h[4]); h[5] = v2fma(gxh, Z, h[5]);
+    h[6] = v2fma(gyh, X, h[6]); h[7] = v2fma(gyh, Y, h[7]); h[8] = v2fma(gyh, Z, h[8]);
+    h[9] = v2fma(gzh, X, h[9]); h[10] = v2fma(gzh, Y, h[10]); h[11] = v2fma(gzh, Z, h[11]);
+}
+
+// hs = the 12 sums of `pose` over the pair records [0, npair)
+template <int DOF>
+__device__ __forceinline__ void pose_grad_sums(const float* pts, int npair, const float* pose, const Cam& cam,
+                                               float delta, float (&hs)[12]) {
+    float R[9], P[12];
+    pose_to_rot<DOF>(pose, R);
+    make_proj(cam.k, R, pose, P);
+    float2 h[12];
+#pragma unroll
+    for (int k = 0; k < 12; ++k) h[k] = splat(0.f);
+    const float4* q = reinterpret_cast<const float4*>(pts);
+    if (cam.bounded) {
+        for (int j = 0; j < npair; ++j) pair_pose_grad<true>(P, cam, delta, q[4 * j], q[4 * j + 1], q[4 * j + 2], q[4 * j + 3], h);
+    } else {
+        for (int j = 0; j < npair; ++j) pair_pose_grad<false>(P, cam, delta, q[4 * j], q[4 * j + 1], q[4 * j + 2], q[4 * j + 3], h);
+    }
+#pragma unroll
+    for (int k = 0; k < 12; ++k) hs[k] = h[k].x + h[k].y;
+}
+
+// The contraction after the sweep: out[0..D) = up * d cost / d pose from the 12 sums.
+template <int DOF>
+__device__ __forceinline__ void pose_grad_contract(const float (&hs)[12], const float* pose, const Cam& cam, float up,
+                                                   float* out) {
+    const float* K = cam.k;
+    float G[9];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        out[i] = up * (K[i] * hs[0] + K[3 + i] * hs[1] + K[6 + i] * hs[2]);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) G[i * 3 + c] = K[i] * hs[3 + c] + K[3 + i] * hs[6 + c] + K[6 + i] * hs[9 + c];
+    }
+    if (DOF == 6) {
+        // dR/dw = 2 [w -z y; z w -x; -y x w]   dR/dx = 2 [x y z; y -x -w; z w -x]
+        // dR/dy = 2 [-y x w; x y z; -w z -y]   dR/dz = 2 [-z -w x; w -z y; x y z]      (quat_to_rot, q = [w x y z])
+        const float w = pose[3], x = pose[4], y = pose[5], z = pose[6];
+        const float a01 = G[1] + G[3], a02 = G[2] + G[6], a12 = G[5] + G[7];        // symmetric parts
+        const float d10 = G[3] - G[1], d02 = G[2] - G[6], d21 = G[7] - G[5];        // antisymmetric parts
+        out[3] = 2.f * up * (w * (G[0] + G[4] + G[8]) + x * d21 + y * d02 + z * d10);
+        out[4] = 2.f * up * (x * (G[0] - G[4] - G[8]) + w * d21 + y * a01 + z * a02);
+        out[5] = 2.f * up * (y * (G[4] - G[0] - G[8]) + w * d02 + x * a01 + z * a12);
+        out[6] = 2.f * up * (z * (G[8] - G[0] - G[4]) + w * d10 + x * a02 + y * a12);
+    } else {
+        // R = [c 0 s; 0 1 0; -s 0 c]: dR/dyaw = [-s 0 c; 0 0 0; -c 0 -s]
+        float sn, cs;
+        sincosf(pose[3], &sn, &cs);
+        out[3] = up * (cs * (G[2] - G[6]) - sn * (G[0] + G[8]));
+    }
+}
+
+template <int DOF>
+__global__ void __launch_bounds__(NT, 4) cost_pose_backward_kernel(const PoseBwArgs g) {
+    EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
+    ObjHead<DOF>& sh = *reinterpret_cast<ObjHead<DOF>*>(smem_raw);
+    float* dyn = reinterpret_cast<float*>(smem_raw);
+    const KArgs& a = g.k;
+    const ObjPlan pl = plan_obj<DOF>(a.N);
+    float* pts = dyn + pl.pts;
+    constexpr int PD = Dim<DOF>::POSE;
+    const int obj = blockIdx.x;
+    Loader ld(a, sh.bar, dyn + pl.stage);
+    ld.load_object(obj, pts);
+    const Cam cam = load_cam(a, obj);
+    const float delta = __ldg(a.delta + obj);
+    for (int p = threadIdx.x; p < g.P; p += NT) {
+        const size_t row = (size_t)obj * g.P + p;
+        float pose[PD], hs[12], out[PD];
+#pragma unroll
+        for (int k = 0; k < PD; ++k) pose[k] = __ldg(a.poses + row * PD + k);
+        pose_grad_sums<DOF>(pts, (a.N + 1) >> 1, pose, cam, delta, hs);
+        pose_grad_contract<DOF>(hs, pose, cam, __ldg(g.grad + row), out);
+#pragma unroll
+        for (int k = 0; k < PD; ++k) g.gpose[row * PD + k] = out[k];
+    }
+}
+
+// cost_pose_backward_kernel for objects too large for one SM, on cost_split_kernel's plan and cluster size: rank r
+// holds the points [r share, (r + 1) share) and sweeps them for a tile of COST_SPLIT_TILE poses (one per thread).  The
+// 12 sums of a pose cross ranks through the staging ring, which is free once the points are loaded and holds them for
+// POSE_BW_PASS poses: the tile is exchanged pass by pass -- the pass's threads write their sums, a cluster barrier,
+// rank 0 adds the ranks' sums in rank order 0 .. ctas - 1 through distributed shared memory, contracts and stores, a
+// second barrier frees the slot.  The gradient depends on ctas (the order of that sum), never on B.
+constexpr int POSE_BW_PASS = 128;
+static_assert(12 * POSE_BW_PASS <= 2 * STAGE_FLOATS, "a pass's sums must fit the staging ring");
+static_assert(COST_SPLIT_TILE % POSE_BW_PASS == 0, "whole passes per tile");
+
+template <int DOF>
+__global__ void __launch_bounds__(COST_SPLIT_TILE, 1) cost_pose_backward_split_kernel(const PoseBwArgs g, const int ctas) {
+    EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
+    float* dyn = reinterpret_cast<float*>(smem_raw);
+    constexpr int PD = Dim<DOF>::POSE, TILE = COST_SPLIT_TILE;
+    const KArgs& a = g.k;
+    const int share = split_share(a.N, ctas);
+    const CostSplitPlan pl = plan_cost_split(share);
+    const int rank = cluster_rank(), obj = blockIdx.x / ctas, tid = threadIdx.x;
+    const int p0 = min(a.N, rank * share), p1 = min(a.N, p0 + share);
+    float* pts = dyn + pl.pts;
+    float* slot = dyn + pl.stage;                       // [12][POSE_BW_PASS]
+    Loader ld(a, reinterpret_cast<uint64_t*>(smem_raw), dyn + pl.stage);
+    ld.load_range<TILE>(obj, pts, p0, p1);
+    const Cam cam = load_cam(a, obj);
+    const float delta = __ldg(a.delta + obj);
+    const int npair = (p1 - p0 + 1) >> 1;
+    for (int t0 = 0; t0 < g.P; t0 += TILE) {
+        const int p = t0 + tid;
+        const size_t row = (size_t)obj * g.P + (p < g.P ? p : 0);
+        float pose[PD], hs[12];
+#pragma unroll
+        for (int k = 0; k < PD; ++k) pose[k] = __ldg(a.poses + row * PD + k);
+        if (p < g.P) pose_grad_sums<DOF>(pts, npair, pose, cam, delta, hs);
+        const int in_tile = min(TILE, g.P - t0);
+        for (int q0 = 0; q0 < in_tile; q0 += POSE_BW_PASS) {
+            const bool mine = tid >= q0 && tid < q0 + POSE_BW_PASS && p < g.P;
+            float* x = slot + (tid - q0);
+            if (mine) {
+#pragma unroll
+                for (int k = 0; k < 12; ++k) x[k * POSE_BW_PASS] = hs[k];
+            }
+            cluster_sync();
+            if (rank == 0 && mine) {
+                float sum[12], out[PD];
+#pragma unroll
+                for (int k = 0; k < 12; ++k) {
+                    float v = dsmem_ld(x + k * POSE_BW_PASS, 0);
+                    for (int r = 1; r < ctas; ++r) v += dsmem_ld(x + k * POSE_BW_PASS, r);
+                    sum[k] = v;
+                }
+                pose_grad_contract<DOF>(sum, pose, cam, __ldg(g.grad + row), out);
+#pragma unroll
+                for (int k = 0; k < PD; ++k) g.gpose[row * PD + k] = out[k];
+                SPLIT_AUDIT_STORES(PD);
+            }
+            cluster_sync();                             // the slot is read: the next pass may write it, or a CTA leave
+        }
+    }
+}
+
 // AdaptiveHuberPnPCost.set_param: delta = mean(w2d) * sqrt(var_x + var_y) * relative_delta
 __global__ void __launch_bounds__(NT) adaptive_delta_kernel(const float* x2d, const float* w2d, float rel,
                                                           float* delta, int N) {
@@ -1473,6 +1665,7 @@ int launch_amis(KArgs& a, const PushArgs* push, cudaStream_t stream, const uint6
 inline KArgs& kargs_of(KArgs& a) { return a; }
 inline KArgs& kargs_of(SeededKArgs& s) { return s.k; }
 inline int prepare_launch(GnBwArgs& g) { return prepare_launch(g.k); }
+inline int prepare_launch(PoseBwArgs& g) { return prepare_launch(g.k); }
 inline int prepare_launch(SeededKArgs& s) { return prepare_launch(s.k); }
 inline int prepare_launch(EpnpInitArgs&) { return EPNP_OK; }
 #if defined(EPNP_SIMT_EMUL) && !defined(SIMT_EMUL_HAS_CLUSTERS)
@@ -2108,6 +2301,54 @@ int epnp_cost_backward_f32(const float* x3d, const float* x2d, const float* w2d,
     const int grid = B < sms * 4 ? B : sms * 4;
     return by_dof(dof, [&](auto D) {
         return launch_plain(cost_backward_kernel<D>, grid, NT, smem, SmemAttr::size, (cudaStream_t)stream, a);
+    });
+}
+
+// The checked arguments of epnp_cost_pose_backward_f32 and its split form, or the refusal.
+static int pose_bw_args(PoseBwArgs& g, const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                        const float* lb, const float* ub, const float* delta, const float* poses, const float* grad,
+                        float* grad_pose, int P, int B, int N, int dof, float z_min) {
+    KArgs& a = g.k;
+    a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
+    a.poses = poses;
+    epnp_default_params(&a.p, dof);
+    a.p.z_min = z_min;
+    g.grad = grad; g.gpose = grad_pose; g.P = P;
+    const int rc = check_common(a);
+    if (rc != EPNP_OK) return rc;
+    return (!poses || !grad || !grad_pose || P < 0) ? EPNP_ERR_BAD_ARG : EPNP_OK;
+}
+
+int epnp_cost_pose_backward_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                const float* lb, const float* ub, const float* delta, const float* poses,
+                                const float* grad, float* grad_pose, int P, int B, int N, int dof, float z_min,
+                                void* stream) {
+    PoseBwArgs g{};
+    const int rc = pose_bw_args(g, x3d, x2d, w2d, cam_mats, lb, ub, delta, poses, grad, grad_pose, P, B, N, dof, z_min);
+    if (rc != EPNP_OK || P == 0 || B == 0) return rc;
+    return by_dof(dof, [&](auto D) {
+        const int smem_bytes = plan_obj<D>(N).total_bytes;
+        const int rc = prepare_resident(g.k, smem_bytes);
+        if (rc != EPNP_OK) return rc;
+        return launch_plain(cost_pose_backward_kernel<D>, B, NT, smem_bytes, SmemAttr::size_and_carveout,
+                            (cudaStream_t)stream, g);
+    });
+}
+
+int epnp_cost_pose_backward_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                      const float* lb, const float* ub, const float* delta, const float* poses,
+                                      const float* grad, float* grad_pose, int P, int B, int N, int dof, float z_min,
+                                      int cluster_ctas, void* stream) {
+    PoseBwArgs g{};
+    const int rc = pose_bw_args(g, x3d, x2d, w2d, cam_mats, lb, ub, delta, poses, grad, grad_pose, P, B, N, dof, z_min);
+    if (rc != EPNP_OK) return rc;
+    const int ctas = split_ctas_for(dof, N, 0, 0, cluster_ctas);
+    if (ctas < 0) return ctas;
+    if (P == 0) return EPNP_OK;
+    const int smem_bytes = split_smem_bytes(dof, N, ctas, 0, 0);
+    return by_dof(dof, [&](auto D) {
+        return launch_cluster<COST_SPLIT_TILE>(cost_pose_backward_split_kernel<D>, g, B, smem_bytes, ctas,
+                                               (cudaStream_t)stream);
     });
 }
 

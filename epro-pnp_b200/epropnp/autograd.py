@@ -1,10 +1,11 @@
 """Autograd bridge for the differentiable outputs of the layer (reference epropnp.py:108-113):
 
     cost_init                       d/d(x3d, x2d, w2d, delta)   native kernel (epnp_cost_backward_f32)
+                                    d/d pose_init               native kernel (epnp_cost_pose_backward_f32)
     pose_sample_logweights          = -cost(samples) - mixture density; only the cost term carries gradient
                                     (samples and proposals are built under no_grad, epropnp.py:139-140,172-179)
                                     -> same native kernel, upstream gradient -dL/dlogw
-    evaluate_pnp(out_cost=True)     same kernel
+    evaluate_pnp(out_cost=True)     the same two kernels (correspondences / delta, poses)
     pose_opt_plus                   one un-damped Gauss-Newton step at the (detached) solution; differentiated
                                     by torch autograd through `PerspectiveCamera.project` + `HuberPnPCost.compute`
                                     (a single evaluation, levenberg_marquardt.py:243-253 -- not the iterated path),
@@ -14,10 +15,11 @@ Objects with more points than one SM holds (N above epnp_max_points: about 5,400
 for the cost, the pose_opt_plus backward and the EPnP initialiser) take the cluster-split kernels (fused_forward,
 stacked_cost, gn_plus_backward, epnp_init), up to epnp_max_points_split; at or below those limits nothing changes.  The
 Monte-Carlo cost backward kernel streams the points, so it serves both; the pose_opt_plus forward (the LM kernel) streams
-them too.  RSLM init and the push / host-buffer entry points still refuse objects above the resident limits.
+them too; the pose backward has a split form of its own (native.cost_pose_backward chooses).  RSLM init and the
+push / host-buffer entry points still refuse objects above the resident limits.
 
-Gradients w.r.t. poses (pose_init / stacked hypotheses) are not provided: the reference's losses never use
-them (pose_init is the ground truth, lib/train.py:178-180), and asking for them raises.
+Gradients w.r.t. poses (pose_init, stacked hypotheses) are those of the rotation the forward calls use, with respect to
+the raw pose components; pose_opt, the samples and the solver's start carry none (reference epropnp.py:139-140).
 """
 import functools
 
@@ -94,6 +96,7 @@ class _MonteCarloForward(torch.autograd.Function):
         ctx.in_like = (x3d, x2d, w2d, delta if torch.is_tensor(delta) else None)
         ctx.needs = (x3d.requires_grad, x2d.requires_grad, w2d.requires_grad,
                      torch.is_tensor(delta) and delta.requires_grad)
+        ctx.pose_like = cost_init_pose if cost_init_pose is not None and cost_init_pose.requires_grad else None
         cost = out["cost"] if want_cost else x3d.new_zeros(0)
         ci = cost_init if cost_init is not None else x3d.new_zeros(0)
         dt = x3d.dtype
@@ -112,14 +115,19 @@ class _MonteCarloForward(torch.autograd.Function):
         if ctx.cost_init_pose is not None and g_cost_init is not None and g_cost_init.numel() == B:
             poses_b = ctx.cost_init_pose.reshape(B, 1, -1)
             grad_b = g_cost_init.reshape(B, 1)
-        grads = native.cost_backward(prob, ctx.dof, ctx.z_min, ctx.samples, -g_logw.contiguous(), poses_b, grad_b,
-                                     want=ctx.needs)
+        grads = (None,) * 4
+        if any(ctx.needs):
+            grads = native.cost_backward(prob, ctx.dof, ctx.z_min, ctx.samples, -g_logw.contiguous(), poses_b, grad_b,
+                                         want=ctx.needs)
         gx3d, gx2d, gw2d, gdel = _grads_to(ctx.in_like, grads)
-        return gx3d, gx2d, gw2d, gdel, None, None, None, None, None, None, None, None, None, None
+        gpose = None
+        if ctx.pose_like is not None and poses_b is not None:
+            gpose = _pose_grad_to(ctx.pose_like, native.cost_pose_backward(prob, ctx.dof, ctx.z_min, poses_b, grad_b)[:, 0])
+        return gx3d, gx2d, gw2d, gdel, None, None, None, None, gpose, None, None, None, None, None
 
 
 class _CostOnly(torch.autograd.Function):
-    """evaluate_pnp(out_cost=True) with gradients w.r.t. the correspondences / delta."""
+    """evaluate_pnp(out_cost=True) with gradients w.r.t. the correspondences / delta and the poses (S, B, D)."""
 
     @staticmethod
     def forward(ctx, x3d, x2d, w2d, delta, cam_mats, lb, ub, poses, dof, z_min):
@@ -131,39 +139,43 @@ class _CostOnly(torch.autograd.Function):
         ctx.in_like = (x3d, x2d, w2d, delta if torch.is_tensor(delta) else None)
         ctx.needs = (x3d.requires_grad, x2d.requires_grad, w2d.requires_grad,
                      torch.is_tensor(delta) and delta.requires_grad)
+        ctx.pose_like = poses if poses.requires_grad else None
         return cost.to(x3d.dtype)
 
     @staticmethod
     def backward(ctx, g_cost):
-        grads = native.cost_backward(ctx.prob, ctx.dof, ctx.z_min, ctx.poses, g_cost.transpose(0, 1).contiguous(),
-                                     want=ctx.needs)
+        g_cost = g_cost.transpose(0, 1).contiguous()                            # object-major (B, S)
+        grads = (None,) * 4
+        if any(ctx.needs):
+            grads = native.cost_backward(ctx.prob, ctx.dof, ctx.z_min, ctx.poses, g_cost, want=ctx.needs)
         gx3d, gx2d, gw2d, gdel = _grads_to(ctx.in_like, grads)
-        return gx3d, gx2d, gw2d, gdel, None, None, None, None, None, None
+        gpose = None
+        if ctx.pose_like is not None:
+            gpose = _pose_grad_to(ctx.pose_like,
+                                  native.cost_pose_backward(ctx.prob, ctx.dof, ctx.z_min, ctx.poses, g_cost).transpose(0, 1))
+        return gx3d, gx2d, gw2d, gdel, None, None, None, gpose, None, None
 
 
-def _no_pose_grad(pose):
-    if torch.is_tensor(pose) and pose.requires_grad:
-        raise NotImplementedError("gradients with respect to poses are not provided by the native EPro-PnP path "
-                                  "(detach the pose; the reference's losses never differentiate through it)")
+def _pose_grad_to(like, g):
+    """Native pose gradient -> dtype and shape of the pose tensor it belongs to."""
+    return g.to(like.dtype).reshape(like.shape)
 
 
 def evaluate_cost_autograd(x3d, x2d, w2d, pose, camera, cost_fun):
-    """cost (*, B) of pose hypotheses with autograd w.r.t. x3d / x2d / w2d / cost_fun.delta."""
-    _no_pose_grad(pose)
+    """cost (*, B) of pose hypotheses with autograd w.r.t. x3d / x2d / w2d / cost_fun.delta / pose."""
     dof = 4 if pose.size(-1) == 4 else 6
     lead = pose.shape[:-1]
     B = x3d.shape[0]
     cost = _CostOnly.apply(x3d, x2d, w2d, _delta_tensor(cost_fun.delta, x2d), camera.cam_mats, camera.lb, camera.ub,
-                           pose.detach().reshape(-1, B, pose.size(-1)), dof, float(camera.z_min))
+                           pose.reshape(-1, B, pose.size(-1)), dof, float(camera.z_min))
     return cost.reshape(lead)
 
 
 def monte_carlo_autograd(x3d, x2d, w2d, camera, cost_fun, pose_start, pose_init, params, noise, seed, want_cost):
     """-> pose_opt, cost | None, pose_samples (B,M,D), logw (B,M) [differentiable], cost_init | None [differentiable]."""
-    _no_pose_grad(pose_init)
     pose_opt, cost, samples, logw, cost_init = _MonteCarloForward.apply(
         x3d, x2d, w2d, _delta_tensor(cost_fun.delta, x2d), camera.cam_mats, camera.lb, camera.ub, pose_start.detach(),
-        None if pose_init is None else pose_init.detach(), params, noise, seed, bool(want_cost), float(camera.z_min))
+        pose_init, params, noise, seed, bool(want_cost), float(camera.z_min))
     return pose_opt, (cost if want_cost else None), samples, logw, (cost_init if pose_init is not None else None)
 
 

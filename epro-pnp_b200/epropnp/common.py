@@ -62,9 +62,11 @@ def evaluate_pnp(x3d, x2d, w2d, pose, camera, cost_fun,
     if kwargs:
         raise TypeError(f"unexpected arguments {sorted(kwargs)}")
     if _needs_grad(x3d, x2d, w2d, pose, getattr(cost_fun, "delta", None)):
-        if out_jacobian is not False or out_residual is not False or pose.requires_grad:
-            # differentiable residual / Jacobian, or gradients w.r.t. the pose (LMSolver.gn_step under autograd,
-            # reference common.py:67-100): the torch composite of the same two methods the reference calls
+        native_pose_grad = x3d.is_cuda and x3d.dtype == pose.dtype == torch.float32
+        if out_jacobian is not False or out_residual is not False or (pose.requires_grad and not native_pose_grad):
+            # differentiable residual / Jacobian (LMSolver.gn_step under autograd, reference common.py:67-100), or
+            # gradients w.r.t. the pose of CPU / float64 tensors: the torch composite of the same two methods the
+            # reference calls
             x2d_proj, jac_cam = camera.project(x3d, pose, out_jac=(out_jacobian is not False), clip_jac=clip_jac)
             residual, cost, jac = cost_fun.compute(x2d_proj, x2d, w2d, jac_cam=jac_cam, out_residual=(out_residual is not False),
                                                    out_cost=(out_cost is not False), out_jacobian=(out_jacobian is not False))

@@ -140,7 +140,8 @@ class EProPnPBase(torch.nn.Module, metaclass=ABCMeta):
             raise TypeError(f"unexpected arguments {sorted(kwargs)}")
         delta = cost_fun.delta
         differentiable = torch.is_grad_enabled() and (any(t.requires_grad for t in (x3d, x2d, w2d)) or
-                                                      (torch.is_tensor(delta) and delta.requires_grad))
+                                                      (torch.is_tensor(delta) and delta.requires_grad) or
+                                                      (pose_init is not None and pose_init.requires_grad))
         if self.normalize:
             transform, x3d, pose_init = pnp_normalize(x3d, pose_init, detach_transformation=True)
         assert x3d.dim() == x2d.dim() == w2d.dim() == 3
@@ -189,7 +190,7 @@ class EProPnPBase(torch.nn.Module, metaclass=ABCMeta):
             tie = x3d.sum(dim=(1, 2)) + x2d.sum(dim=(1, 2)) + w2d.sum(dim=(1, 2))             # (0,), connected
             logw = x3d.reshape(self.mc_samples, 0) + x2d.reshape(self.mc_samples, 0) + w2d.reshape(self.mc_samples, 0)
             if cost_init is not None:
-                cost_init = cost_init + tie
+                cost_init = cost_init + tie + pose_init.sum(dim=1)
             if pose_opt_plus is not None:
                 pose_opt_plus = pose_opt_plus + tie[:, None]
 

@@ -456,6 +456,26 @@ def cost_backward(prob: Problem, dof, z_min, poses_a, grad_a, poses_b=None, grad
     return gx3d, gx2d, gw2d, gdel
 
 
+def cost_pose_backward(prob: Problem, dof, z_min, poses, grad, cluster_ctas=0):
+    """grad[b, p] * d cost(poses[b, p]) / d poses[b, p] for object-major poses (B, P, D) and grad (B, P) -> (B, P, D)
+    (epnp_cost_pose_backward_f32; above max_points(dof) its cluster-split form, `cluster_ctas` as evaluate_cost_split)."""
+    D = 7 if dof == 6 else 4
+    P = poses.shape[1]
+    _check_pose(poses, (prob.B, P), D, "poses")
+    if tuple(grad.shape) != (prob.B, P):
+        raise ValueError(f"grad must be {(prob.B, P)}; got {tuple(grad.shape)}")
+    poses, grad = _f32c(poses), _f32c(grad)
+    out = prob.empty(prob.B, P, D)
+    args = (*prob.common_ptrs(), ptr(poses), ptr(grad), ptr(out), P, prob.B, prob.N, int(dof), ctypes.c_float(z_min))
+    with torch.cuda.device(prob.device):
+        if prob.N > max_points(dof):
+            check(lib().epnp_cost_pose_backward_split_f32(*args, int(cluster_ctas), stream_ptr(prob.device)),
+                  "epnp_cost_pose_backward_split_f32")
+        else:
+            check(lib().epnp_cost_pose_backward_f32(*args, stream_ptr(prob.device)), "epnp_cost_pose_backward_f32")
+    return out
+
+
 def fused_workspace_bytes(B, N, params):
     return int(lib().epnp_fused_workspace_bytes(B, N, ctypes.byref(params)))
 

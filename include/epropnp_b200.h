@@ -339,6 +339,30 @@ int epnp_cost_backward_f32(const float* x3d, const float* x2d, const float* w2d,
                            float* grad_x3d, float* grad_x2d, float* grad_w2d, float* grad_delta,
                            int B, int N, int dof, float z_min, void* stream);
 
+/* Backward of the same costs with respect to the POSE (the reference's evaluate_pnp is differentiable there too:
+ * common.py:30-36, camera.py:21-30; cost_init of monte_carlo_forward with a predicted pose_init, epropnp.py:121-124):
+ *   grad_pose[b, p] = grad[b, p] * d cost(poses[b, p]) / d poses[b, p]
+ * for poses (B, P, D) given object-major with grad (B, P); grad_pose (B, P, D).  D = 7: [x y z w i j k], the gradient
+ * with respect to the four RAW components of the un-normalised quaternion whose rotation the forward calls use
+ * (R = (ww + ii - jj - kk ...), not a tangent vector; on unit quaternions it differs from the reference's
+ * differentiable branch 1 - 2 (jj + kk) ... only along q itself); D = 4: [x y z yaw].  Same clamps as above: no gradient
+ * through a depth clamped at z_min or a coordinate clamped at lb / ub.  One thread per pose, no atomics: a row depends
+ * on its object and its pose only.  P = 0 or B = 0 writes nothing.                                              */
+int epnp_cost_pose_backward_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                const float* lb, const float* ub, const float* delta, const float* poses,
+                                const float* grad, float* grad_pose, int P, int B, int N, int dof, float z_min,
+                                void* stream);
+
+/* epnp_cost_pose_backward_f32 for objects of up to epnp_max_points_split(dof, 0, 0) points, on the clusters of
+ * epnp_evaluate_cost_split_f32: each rank sweeps its own range of the points, rank 0 adds the ranks' partial sums in
+ * rank order and writes the rows.  cluster_ctas as there (0: epnp_split_ctas(dof, N, 0, 0); EPNP_ERR_BAD_ARG outside
+ * [that minimum, 8]; EPNP_ERR_TOO_MANY_POINTS when no C fits); the gradient depends on C and never on B.
+ * EPNP_ERR_UNSUPPORTED when the device cannot run one cluster of that size; nothing is launched then.           */
+int epnp_cost_pose_backward_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                      const float* lb, const float* ub, const float* delta, const float* poses,
+                                      const float* grad, float* grad_pose, int P, int B, int N, int dof, float z_min,
+                                      int cluster_ctas, void* stream);
+
 /* Epilogue on the AMIS outputs -- the step AFTER the path in every caller of monte_carlo_forward (one pass over the
  * object-major log-weights instead of a dozen torch ops on (M, B) views):
  *   lse (B)        = logsumexp_m logw[b, m]      -- `loss_pred` of MonteCarloPoseLoss.forward
