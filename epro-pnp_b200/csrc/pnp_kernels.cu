@@ -251,6 +251,97 @@ __global__ void __launch_bounds__(NT, 2) rslm_kernel(const RslmArgs r) {
     }
 }
 
+// The RSLM initialiser for objects too large for one SM (epnp_rslm_split_f32) is three launches: this kernel refines
+// the hypotheses, cost_split_kernel scores them on all N points on the object's cluster, rslm_select_kernel keeps the
+// cheapest.  Here one thread per (hypothesis, object) -- thread t = h B + obj, grid over P B -- runs rslm_kernel's
+// iterations on the n sampled correspondences read straight from the object's global rows (nothing is staged: a
+// hypothesis touches n points, not N), and writes pose_all.  A hypothesis' pose is bit-identical to rslm_kernel's:
+// the iterations below are rslm_kernel's, spelled out again because sharing one inlined body changes rslm_kernel<4>'s
+// register allocation (its SASS is pinned).
+
+// One object's rows of x3d / x2d / w2d in global memory.
+struct GlobalRowPoints { const float *x3d, *x2d, *w2d; };
+
+// eval_subset on points read from global memory: the same floats go into point_normal_eq_rows as from a pair record
+// (store_point keeps -u and -v; the negation is exact).
+template <int DOF, bool CLIP>
+__device__ __forceinline__ void eval_subset(const GlobalRowPoints& g, const int* idx, int n, const float* pose,
+                                            const Cam& cam, float delta, float huber_eps, float* acc) {
+    constexpr int NP = Dim<DOF>::NV - 1;
+    float R[9];
+    pose_to_rot<DOF>(pose, R);
+    V2 acc2[NP];
+#pragma unroll
+    for (int i = 0; i < NP; ++i) acc2[i] = v2splat(0.f);
+    const V2 kuv[3] = {v2(cam.k[0], cam.k[3]), v2(cam.k[1], cam.k[4]), v2(cam.k[2], cam.k[5])};
+    float cost = 0.f;
+    for (int i = 0; i < n; ++i) {
+        const int j = __ldg(idx + i);
+        point_normal_eq_rows<DOF, CLIP>(R, pose, cam, kuv, delta, huber_eps, __ldg(g.x3d + 3 * j), __ldg(g.x3d + 3 * j + 1),
+                                        __ldg(g.x3d + 3 * j + 2), -__ldg(g.x2d + 2 * j), -__ldg(g.x2d + 2 * j + 1),
+                                        __ldg(g.w2d + 2 * j), __ldg(g.w2d + 2 * j + 1), acc2, cost);
+    }
+#pragma unroll
+    for (int i = 0; i < NP; ++i) acc[i] = acc2[i].x + acc2[i].y;
+    acc[NP] = cost;
+}
+
+template <int DOF>
+__global__ void __launch_bounds__(NT) rslm_refine_kernel(const RslmArgs r) {
+    const KArgs& a = r.k;
+    constexpr int PD = Dim<DOF>::POSE;
+    const Params& p = a.p;
+    const size_t t = (size_t)blockIdx.x * NT + threadIdx.x;
+    if (t >= (size_t)r.P * a.B) return;
+    const int obj = (int)(t % (size_t)a.B);
+    const size_t row = (size_t)obj * a.N;
+    const GlobalRowPoints pts{a.x3d + row * 3, a.x2d + row * 2, a.w2d + row * 2};
+    const int* idx = r.inds + t * r.n;
+    const Cam cam = load_cam(a, obj);
+    const float delta = __ldg(a.delta + obj);
+    LMState<DOF> s;
+#pragma unroll
+    for (int i = 0; i < PD; ++i) s.pose[i] = __ldg(r.start + t * PD + i);
+    s.radius = p.initial_radius;
+    s.shrink = 2.0f;
+    float acc[Dim<DOF>::NV];
+    if (!p.fast_mode) {
+        eval_subset<DOF, true>(pts, idx, r.n, s.pose, cam, delta, p.huber_eps, acc);
+        lm_adopt<DOF>(s, acc);
+        if (p.lm_iter > 0) lm_propose<DOF>(s, p);
+        for (int k = 0; k < p.lm_iter; ++k) {
+            eval_subset<DOF, true>(pts, idx, r.n, s.pose_new, cam, delta, p.huber_eps, acc);
+            lm_update<DOF>(s, acc, p);
+            if (k + 1 < p.lm_iter) lm_propose<DOF>(s, p);
+        }
+    } else {
+        for (int k = 0; k < p.lm_iter; ++k) {
+            eval_subset<DOF, false>(pts, idx, r.n, s.pose, cam, delta, p.huber_eps, acc);
+            gn_advance<DOF>(s.pose, acc, p.eps, s.pose);
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < PD; ++i) r.pose_all[t * PD + i] = s.pose[i];
+}
+
+// The winner of each object over h = 0 .. P-1 by cheaper_hypothesis (torch.min's order), one thread per object:
+// pose_best and cost_best are copies of its pose_all / cost_all row.
+template <int DOF>
+__global__ void __launch_bounds__(NT) rslm_select_kernel(const RslmArgs r) {
+    constexpr int PD = Dim<DOF>::POSE;
+    const int B = r.k.B, obj = blockIdx.x * NT + threadIdx.x;
+    if (obj >= B) return;
+    int w = 0;
+    float wc = r.cost_all[obj];
+    for (int h = 1; h < r.P; ++h) {
+        const float c = r.cost_all[(size_t)h * B + obj];
+        if (cheaper_hypothesis(c, h, wc, w)) { wc = c; w = h; }
+    }
+#pragma unroll
+    for (int i = 0; i < PD; ++i) r.pose_best[(size_t)obj * PD + i] = r.pose_all[((size_t)w * B + obj) * PD + i];
+    r.cost_best[obj] = wc;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Everything RSLMSolver.solve does before its solves (levenberg_marquardt.py:283-324), one CTA per object:
 //   * the centre-based translation guess (center_based_init, :283-298): rays = K^-1 [u v 1] dehomogenised, direction =
@@ -2069,6 +2160,38 @@ int epnp_rslm_f32(const float* x3d, const float* x2d, const float* w2d, const fl
         const int rc = prepare_resident(r.k, smem_bytes);
         if (rc != EPNP_OK) return rc;
         return launch_plain(rslm_kernel<D>, B, NT, smem_bytes, SmemAttr::size, (cudaStream_t)stream, r);
+    });
+}
+
+int epnp_rslm_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                        const float* lb, const float* ub, const float* delta, const int* inds, const float* start,
+                        float* pose_best, float* cost_best, float* pose_all, float* cost_all,
+                        int P, int n, int B, int N, const EpnpParams* p, int cluster_ctas, void* stream) {
+    if (!p) return EPNP_ERR_BAD_ARG;
+    RslmArgs r{};
+    r.k = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
+    r.k.p = *p;
+    r.inds = inds; r.start = start; r.pose_best = pose_best; r.cost_best = cost_best;
+    r.pose_all = pose_all; r.cost_all = cost_all; r.P = P; r.n = n;
+    const int rc = check_common(r.k);
+    if (rc != EPNP_OK) return rc;
+    if (!inds || !start || !pose_best || !cost_best || !pose_all || !cost_all || P <= 0 || n <= 0 || p->lm_iter < 0)
+        return EPNP_ERR_BAD_ARG;
+    const int ctas = split_ctas_for(p->dof, N, 0, 0, cluster_ctas);
+    if (ctas < 0) return ctas;
+    if (B == 0) return EPNP_OK;
+    KArgs score = r.k;                          // cost_split_kernel on the P refined poses of every object
+    score.poses = pose_all; score.cost_out = cost_all; score.S_eval = P;
+    const int smem_bytes = split_smem_bytes(p->dof, N, ctas, 0, 0);
+    const cudaStream_t s = (cudaStream_t)stream;
+    const int rows = (int)(((size_t)P * B + NT - 1) / NT);
+    return by_dof(p->dof, [&](auto D) {
+        // a device that cannot run the scoring cluster gets no launch at all
+        int rc = launch_cluster<COST_SPLIT_TILE>(cost_split_kernel<D>, score, B, smem_bytes, ctas, s, false);
+        if (rc == EPNP_OK) rc = launch_plain(rslm_refine_kernel<D>, rows, NT, 0, SmemAttr::none, s, r);
+        if (rc == EPNP_OK) rc = launch_cluster<COST_SPLIT_TILE>(cost_split_kernel<D>, score, B, smem_bytes, ctas, s);
+        if (rc == EPNP_OK) rc = launch_plain(rslm_select_kernel<D>, (B + NT - 1) / NT, NT, 0, SmemAttr::none, s, r);
+        return rc;
     });
 }
 

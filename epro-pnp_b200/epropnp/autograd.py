@@ -15,8 +15,9 @@ Objects with more points than one SM holds (N above epnp_max_points: about 5,400
 for the cost, the pose_opt_plus backward and the EPnP initialiser) take the cluster-split kernels (fused_forward,
 stacked_cost, gn_plus_backward, epnp_init), up to epnp_max_points_split; at or below those limits nothing changes.  The
 Monte-Carlo cost backward kernel streams the points, so it serves both; the pose_opt_plus forward (the LM kernel) streams
-them too; the pose backward has a split form of its own (native.cost_pose_backward chooses).  RSLM init and the
-push / host-buffer entry points still refuse objects above the resident limits.
+them too; the pose backward has a split form of its own (native.cost_pose_backward chooses).  RSLM init takes its split
+form (rslm_solve) only when the solver was built with RSLMSolver(cluster_split=True), up to min(epnp_max_points_split,
+the native draw's own limit: 53,504 points at n = 16); by default it refuses objects above the resident limit.
 
 Gradients w.r.t. poses (pose_init, stacked hypotheses) are those of the rotation the forward calls use, with respect to
 the raw pose components; pose_opt, the samples and the solver's start carry none (reference epropnp.py:139-140).
@@ -50,6 +51,13 @@ def gn_plus_backward(prob, pose, grad_pose_plus, dof, z_min, eps, huber_eps, wan
     split = prob.N > _resident_limit(dof, 0, 0)
     return (native.gn_plus_backward_split if split else native.gn_plus_backward)(
         prob, pose, grad_pose_plus, dof, z_min, eps, huber_eps, want=want)
+
+
+def rslm_solve(prob, inds, start, params, allow_split):
+    """native.rslm, or, when `allow_split` is set and the objects' points do not fit one SM, its cluster-split form.
+    Without `allow_split` such objects are refused as before (RSLMSolver's cluster_split keyword)."""
+    split = allow_split and prob.N > _resident_limit(params.dof, 0, 0)
+    return (native.rslm_split if split else native.rslm)(prob, inds, start, params)
 
 
 def epnp_init(x3d, x2d, w2d, cam_mats, conf_quantile):

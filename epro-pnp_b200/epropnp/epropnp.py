@@ -7,8 +7,9 @@ densities -> log-weights -> proposal refit) run per object inside one CTA with t
 resident in shared memory.  The reference's materialised (S, B, N, 3) intermediates, its per-iteration
 host Cholesky round trips and its ~10^3 op launches do not exist here.  Objects with more correspondences than one
 SM holds (N > epnp_max_points(dof, M, I), e.g. the 16,384 of a 128 x 128 coordinate map) run the same loop on a
-thread-block cluster of 2-8 CTAs (epnp_lm_amis_fused_split_f32); the RSLM initialiser still refuses those with its
-shared-memory error, so they need pose_init with force_init_solve=False.
+thread-block cluster of 2-8 CTAs (epnp_lm_amis_fused_split_f32).  The RSLM initialiser refuses those with its
+shared-memory error unless it was built as RSLMSolver(..., cluster_split=True), which solves them on the cluster-split
+initialiser (epnp_rslm_split_f32); without it they need pose_init with force_init_solve=False.
 
 Layout note: the kernel writes object-major (B, M, D) / (B, M) buffers; the tuples returned below
 hold (M, B, D) / (M, B) *views* of them so reference call sites (softmax(dim=0), logsumexp(dim=0),

@@ -6,7 +6,8 @@ What runs where:
     the optional extra GN step are ONE kernel launch (epnp_lm_solve_f32): no per-iteration launches,
     no host round trips, no materialised (B, 2N, 6) Jacobian;
   * RSLMSolver: two launches -- the random subsets / start orientations (epnp_rslm_draw_f32), then refining and
-    scoring all P hypotheses of every object (epnp_rslm_f32).
+    scoring all P hypotheses of every object (epnp_rslm_f32); with cluster_split=True, objects too large for one SM
+    take epnp_rslm_split_f32 instead (refine, score on a thread-block cluster, select: three launches).
 """
 import math
 
@@ -15,6 +16,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from epropnp_b200 import native
+from .autograd import rslm_solve
 from .builder import PNP, build_pnp
 from .common import evaluate_pnp, philox_seed, pnp_normalize, pnp_denormalize
 
@@ -172,17 +174,24 @@ class LMSolver(nn.Module):
 class RSLMSolver(LMSolver):
     """Random-sample LM: a RANSAC-like initialiser for ambiguous problems (levenberg_marquardt.py:268-353)."""
 
-    def __init__(self, num_points=16, num_proposals=64, num_iter=3, draws='native', **kwargs):
+    def __init__(self, num_points=16, num_proposals=64, num_iter=3, draws='native', cluster_split=False, **kwargs):
         """draws='native' (default): the weighted subsets and start orientations come from one kernel launch
         (epnp_rslm_draw_f32, Philox keyed by a seed taken from torch's default generator, so torch.manual_seed governs
         it); draws='torch': torch.multinomial / randn / rand exactly as the reference calls them (:306-324) -- the same
-        distribution from torch's own streams, for code that replays or compares them (the parity tests do)."""
+        distribution from torch's own streams, for code that replays or compares them (the parity tests do).
+
+        cluster_split=True lets objects with more points than one SM holds (above epnp_max_points(dof, 0, 0): 7,000 in
+        6DoF) be solved by the cluster-split initialiser (epnp_rslm_split_f32) instead of being refused.  Objects at or
+        below that limit take the resident kernel either way.  The largest N is then epnp_max_points_split(dof, 0, 0)
+        (55,232 in 6DoF) with draws='torch', and with draws='native' the smaller of that and the draw kernel's own
+        shared-memory limit, 4 N + 8 n 128 + 2 KB <= 227 KB (53,504 points at n = 16)."""
         super(RSLMSolver, self).__init__(num_iter=num_iter, **kwargs)
         self.num_points = num_points
         self.num_proposals = num_proposals
         if draws not in ('native', 'torch'):
             raise ValueError(f"draws must be 'native' or 'torch', got {draws!r}")
         self.draws = draws
+        self.cluster_split = bool(cluster_split)
 
     def center_based_init(self, x2d, x3d, camera, eps=1e-6):
         """Translation guess from the spread of the 2D points vs the 3D points (:283-298)."""
@@ -249,5 +258,6 @@ class RSLMSolver(LMSolver):
             inds, start = native.rslm_draw(x3d, x2d, w2d, camera.cam_mats, P, n, self.dof, eps=self.eps, seed=seed,
                                            t_init=t_init)
         prob = native.Problem(x3d, x2d, w2d, camera.cam_mats, camera.lb, camera.ub, cost_fun.delta)
-        out = native.rslm(prob, inds, start, self.native_params(camera, cost_fun, kwargs.get("fast_mode", False)))
+        out = rslm_solve(prob, inds, start, self.native_params(camera, cost_fun, kwargs.get("fast_mode", False)),
+                         allow_split=self.cluster_split)
         return out["pose"].to(x2d.dtype), None, out["cost"].to(x2d.dtype)

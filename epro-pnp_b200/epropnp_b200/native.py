@@ -228,6 +228,26 @@ def rslm(prob: Problem, inds, start, params, want_all=False):
     return out
 
 
+def rslm_split(prob: Problem, inds, start, params, want_all=False, cluster_ctas=0):
+    """rslm for objects larger than one SM holds (epnp_rslm_split_f32): the hypotheses are refined one thread each
+    (pose_all bit-identical to rslm's), scored by evaluate_cost_split on a thread-block cluster of split_ctas(dof, N)
+    CTAs per object, or of `cluster_ctas` (that minimum .. 8), and the cheapest is kept.  Same return dict as rslm."""
+    D = 7 if params.dof == 6 else 4
+    P, B, n = inds.shape
+    assert B == prob.B and start.shape == (P, B, D)
+    inds32 = inds.detach().to(device=prob.device, dtype=torch.int32).contiguous()
+    start = _f32c(start)
+    out = dict(pose=prob.empty(B, D), cost=prob.empty(B), pose_all=prob.empty(P, B, D), cost_all=prob.empty(P, B))
+    with torch.cuda.device(prob.device):
+        check(lib().epnp_rslm_split_f32(*prob.common_ptrs(), capi.iptr(inds32), ptr(start), ptr(out["pose"]),
+                                        ptr(out["cost"]), ptr(out["pose_all"]), ptr(out["cost_all"]), P, n, B, prob.N,
+                                        ctypes.byref(params), int(cluster_ctas), stream_ptr(prob.device)),
+              "epnp_rslm_split_f32")
+    if not want_all:
+        out["pose_all"] = out["cost_all"] = None
+    return out
+
+
 def epnp_init(x3d, x2d, w2d, cam_mats, conf_quantile=0.8, want_n_sel=False):
     """EPnP initialisation of the 6DoF test-time solve (epnp_epnp_init_f32): per object, the points whose confidence
     mean(w2d, -1) is >= its np.quantile(., conf_quantile) (every point when w2d is None), then EPnP as
@@ -569,4 +589,4 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
 
 
 __all__ = ["Problem", "adaptive_delta", "cost_backward", "evaluate_cost", "evaluate_cost_split", "evaluate_full", "lm_solve",
-           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "rslm", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]
+           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "rslm", "rslm_split", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

@@ -180,6 +180,22 @@ int epnp_rslm_f32(const float* x3d, const float* x2d, const float* w2d, const fl
                   float* pose_best, float* cost_best, float* pose_all, float* cost_all,
                   int P, int n, int B, int N, const EpnpParams* p, void* stream);
 
+/* epnp_rslm_f32 for objects of up to epnp_max_points_split(dof, 0, 0) points, as three launches on `stream`: one
+ * thread per (hypothesis, object) refines the hypothesis on its n correspondences, read from the object's rows in
+ * global memory (pose_all: bit-identical to epnp_rslm_f32's for the same inds / start); epnp_evaluate_cost_split_f32's
+ * kernel scores the P poses on all N points on the object's cluster (cost_all: bit-identical to that call on pose_all
+ * with the same C and params->z_min); one thread per object keeps the cheapest (torch.min's order: a NaN cost wins,
+ * then the smaller cost, then the earlier hypothesis) in pose_best / cost_best.  The costs, and so a winner between
+ * nearly equal hypotheses, depend on C (the order of the ranks' partial sums), never on B.
+ *   pose_all (P, B, D) and cost_all (P, B) are REQUIRED: they carry the results from one launch to the next.
+ *   cluster_ctas as epnp_evaluate_cost_split_f32's (0: epnp_split_ctas(dof, N, 0, 0); EPNP_ERR_BAD_ARG outside [that
+ *   minimum, 8]; EPNP_ERR_TOO_MANY_POINTS when no C fits, for any B).  EPNP_ERR_UNSUPPORTED when the device cannot
+ *   run one cluster of that size; nothing is launched then.                                                       */
+int epnp_rslm_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                        const float* lb, const float* ub, const float* delta, const int* inds, const float* start,
+                        float* pose_best, float* cost_best, float* pose_all, float* cost_all,
+                        int P, int n, int B, int N, const EpnpParams* p, int cluster_ctas, void* stream);
+
 /* EPnP initialisation of the 6DoF test-time solve (EPro-PnP-6DoF/lib/test.py:178-194): per object,
  *   conf_i = (w2d[i,0] + w2d[i,1]) / 2, the points with conf_i >= np.quantile(conf, conf_quantile) (NumPy 2.x
  *   'linear', evaluated in fp32 as NumPy does for a float32 row; ties kept) -> cv2.solvePnP(..., SOLVEPNP_EPNP)

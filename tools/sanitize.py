@@ -66,6 +66,8 @@ for dof, N, B, bounded in ((6, 64, 5, False), (6, 130, 3, True), (6, 51, 4, Fals
         check(f"{tag}: drawn subsets in range and distinct",
               di.min() >= 0 and di.max() < N and (di.sort(-1).values[..., 1:] != di.sort(-1).values[..., :-1]).all())
         native.rslm(prob, di, ds, native.default_params(dof, lm_iter=2))
+        bounded = native.Problem(d["x3d"], d["x2d"], d["w2d"], d["cam_mats"], 0.0, 640.0, prob.delta)
+        native.rslm_split(bounded, di, ds, native.default_params(dof, lm_iter=2), want_all=True, cluster_ctas=2)
         native.gn_plus_backward(prob, out["pose_opt"], torch.randn(B, D, device=dev), dof, 0.1, 1e-5, 1e-10)
     torch.cuda.synchronize()
     check(f"dof={dof} N={N}: finite log-weights", torch.isfinite(out["logw"]).all())
