@@ -1,5 +1,7 @@
 // pnp_amis.cuh -- the adaptive-multiple-importance-sampling loop of EProPnPBase.monte_carlo_forward
-// (epropnp.py:132-182; 6DoF proposals :288-342, 4DoF :199-260) as a CTA-PER-OBJECT kernel.
+// (epropnp.py:132-182; 6DoF proposals :288-342, 4DoF :199-260) as a CTA-PER-OBJECT kernel.  One loop, amis_loop, serves
+// both pose families, the resident and the cluster-split kernels; the families differ only in the draw, the proposal
+// density, the refit and the proposal dump.
 //
 //   * the object's correspondences are pulled from HBM once (TMA ring -> 64-byte pair records in shared memory);
 //   * one thread owns one sample of an iteration: draws it (injected noise or Philox), sweeps all N points with the
@@ -86,7 +88,7 @@ __device__ __forceinline__ float log_add_exp(float a, float b) {
 // template instance per stage, so every stage's trip count is a constant and the W = 16 or 32 values stay in registers.
 // In block_sum's warp_transpose_sum_w the stage count is a loop variable, the inner loops stay partly rolled and the
 // values go through a local-memory copy indexed per lane (LDL / STL on the latency-bound refit chain).  Same adds in the
-// same order, so the same bits.  T != NT keeps block_sum and its code, and so does amis_phase4: its 6-value sums do not reach local memory.
+// same order, so the same bits.  T != NT keeps block_sum and its code, and so does the 4DoF refit: its 6-value sums do not reach local memory.
 template <int W, int HALF> __device__ __forceinline__ void amis_transpose_stage(float (&v)[W], int lane) {
     constexpr int MASK = 32 * HALF / W;     // 16 at the first stage (HALF = W / 2), halving with HALF
     const bool up = (lane & MASK) != 0;
@@ -130,14 +132,23 @@ struct SplitCtx {
     int rank, ctas, npair;
 };
 
+__device__ __forceinline__ float proposal_logpdf(const Proposal6& pr, const float* q) { return proposal_logpdf6(pr, q); }
+__device__ __forceinline__ float proposal_logpdf(const Proposal4& pr, const float* q) { return proposal_logpdf4(pr, q); }
+
 // ------------------------------------------------------------------------------------------------
-// AMIS loop for the resident object, 6DoF.  sh.prop[0] holds the first proposal (the kernel fitted it to the LM solution).
+// The AMIS loop of one object, either pose family.  sh.prop[0] holds the first proposal (the kernel fitted it to the LM
+// solution).  Where the families differ, each keeps the form its kernels were validated with (a common form, such as
+// the 6DoF register copy of a sample in the 4DoF sweep, compiles them differently).  4DoF (EProPnP4DoF,
+// epropnp.py:199-260): the yaw proposal is 0.75 von Mises + 0.25 uniform, and injected noise_rot (B, M) holds the yaw
+// draws themselves (the reference samples them with numpy on the host, distributions.py:61-72, so there is no base
+// noise to replay).
 // SPLIT: the cluster form (sc describes the CTA's share); every rank draws the same samples and, after the exchange of
 // the partial costs, holds the same costs, so each runs the same refits; rank 0 alone writes the outputs.
-template <int T, bool SPLIT = false>
-__device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts4, float* smp, float* cst, float* logp,
-                            float* cpart, const Cam& cam, float delta, int obj, const SplitCtx sc = SplitCtx{}) {
+template <int DOF, int T, bool SPLIT>
+__device__ void amis_loop(const KArgs& a, AmisHead<DOF, T>& sh, const float* pts4, float* smp, float* cst, float* logp,
+                          float* cpart, const Cam& cam, float delta, int obj, const SplitCtx sc = SplitCtx{}) {
     constexpr int PARTS = T / NT;           // threads sweeping one sample (1: the thread that drew it)
+    constexpr int PD = Dim<DOF>::POSE;
     const Params& p = a.p;
     const int tid = threadIdx.x;
     const int M = p.mc_samples, I = p.mc_iter, S = M / I;
@@ -152,24 +163,31 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
         for (int s = tid; s < S; s += NT) {
             if (PARTS > 1 && tid >= NT) break;
             const int m = i * S + s;
-            float n3[3], n4[4], chi2;
+            float n3[3], n4[4], chi2, q[PD];        // n4: the rotation's base noise (6DoF)
             if (injected) {
                 const size_t g = (size_t)obj * M + m;
                 n3[0] = __ldg(a.noise_n3 + g * 3); n3[1] = __ldg(a.noise_n3 + g * 3 + 1); n3[2] = __ldg(a.noise_n3 + g * 3 + 2);
                 chi2 = __ldg(a.noise_chi2 + g);
-                n4[0] = __ldg(a.noise_rot + g * 4); n4[1] = __ldg(a.noise_rot + g * 4 + 1);
-                n4[2] = __ldg(a.noise_rot + g * 4 + 2); n4[3] = __ldg(a.noise_rot + g * 4 + 3);
-            } else {
+                if constexpr (DOF == 6) {
+                    n4[0] = __ldg(a.noise_rot + g * 4); n4[1] = __ldg(a.noise_rot + g * 4 + 1);
+                    n4[2] = __ldg(a.noise_rot + g * 4 + 2); n4[3] = __ldg(a.noise_rot + g * 4 + 3);
+                } else {
+                    q[3] = __ldg(a.noise_rot + g);
+                }
+            } else if constexpr (DOF == 6) {
                 draw_base_noise(a.seed, a.obj_offset + (uint32_t)obj, (uint32_t)m, n3, chi2, n4);
+            } else {
+                draw_base_noise_t(a.seed, a.obj_offset + (uint32_t)obj, (uint32_t)m, n3, chi2);
+                q[3] = draw_yaw(a.seed, a.obj_offset + (uint32_t)obj, (uint32_t)m, s, S, sh.prop[i].mode, sh.prop[i].kappa);
             }
-            float q[7];
-            proposal_draw6(sh.prop[i], n3, chi2, n4, q);
+            if constexpr (DOF == 6) proposal_draw6(sh.prop[i], n3, chi2, n4, q);
+            else draw_translation(sh.prop[i].mu, sh.prop[i].lt, n3, chi2, q);
 #pragma unroll
-            for (int k = 0; k < 7; ++k) smp[m * 7 + k] = q[k];
-            if constexpr (PARTS == 1) cst[m] = pose_cost_pairs<6>(pts4, 0, (a.N + 1) >> 1, q, cam, delta, sh.box);
+            for (int k = 0; k < PD; ++k) smp[m * PD + k] = q[k];
+            if constexpr (PARTS == 1) cst[m] = pose_cost_pairs<DOF>(pts4, 0, (a.N + 1) >> 1, q, cam, delta, sh.box);
             RunningLse l;
-            l.start(proposal_logpdf6(sh.prop[0], q));
-            for (int j = 1; j <= i; ++j) l.add(proposal_logpdf6(sh.prop[j], q));
+            l.start(proposal_logpdf(sh.prop[0], q));
+            for (int j = 1; j <= i; ++j) l.add(proposal_logpdf(sh.prop[j], q));
             logp[m] = l.value();
         }
         if constexpr (PARTS > 1) {
@@ -178,10 +196,14 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
             const int j0 = (int)((long long)npair * part / PARTS) & ~3, j1 = part + 1 == PARTS ? npair : ((int)((long long)npair * (part + 1) / PARTS) & ~3);
             for (int s = tid % NT; s < S; s += NT) {
                 const int m = i * S + s;
-                float q[7];
+                if constexpr (DOF == 6) {
+                    float q[7];
 #pragma unroll
-                for (int k = 0; k < 7; ++k) q[k] = smp[m * 7 + k];
-                cpart[part * M + m] = pose_cost_pairs<6>(pts4, j0, j1, q, cam, delta, sh.box);
+                    for (int k = 0; k < 7; ++k) q[k] = smp[m * 7 + k];
+                    cpart[part * M + m] = pose_cost_pairs<6>(pts4, j0, j1, q, cam, delta, sh.box);
+                } else {
+                    cpart[part * M + m] = pose_cost_pairs<4>(pts4, j0, j1, smp + m * 4, cam, delta, sh.box);
+                }
             }
             __syncthreads();
             for (int s = tid; s < S; s += T) {
@@ -196,21 +218,20 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
                 // One cluster barrier per iteration: the half (i & 1) of xbuf is written again at iteration i + 2, after
                 // the barrier of iteration i + 1, which every rank reaches only once its reads below are done.
                 cluster_sync();
-                for (int s = tid; s < S; s += T) {
-                    const float* x = sc.xbuf + (i & 1) * S + s;
-                    float c = dsmem_ld(x, 0);
-                    for (int r = 1; r < sc.ctas; ++r) c += dsmem_ld(x, r);
-                    cst[i * S + s] = c;
-                }
+                for (int s = tid; s < S; s += T) cst[i * S + s] = sum_ranks(sc.xbuf + (i & 1) * S + s, sc.ctas);
             }
         }
         PH_MARK(a, PH_DRAW_SWEEP);
         // ---- the new proposal on all earlier samples
         for (int m = tid; m < i * S; m += T) {
-            float q[7];
+            if constexpr (DOF == 6) {
+                float q[7];
 #pragma unroll
-            for (int k = 0; k < 7; ++k) q[k] = smp[m * 7 + k];
-            logp[m] = log_add_exp(logp[m], proposal_logpdf6(sh.prop[i], q));
+                for (int k = 0; k < 7; ++k) q[k] = smp[m * 7 + k];
+                logp[m] = log_add_exp(logp[m], proposal_logpdf6(sh.prop[i], q));
+            } else {
+                logp[m] = log_add_exp(logp[m], proposal_logpdf4(sh.prop[i], smp + m * 4));
+            }
         }
         __syncthreads();
         PH_MARK(a, PH_LOGP_OLD);
@@ -227,65 +248,95 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
         float mx = -CUDART_INF_F;
         for (int m = tid; m < n; m += T) mx = fmaxf(mx, logweight(m));
         PH_MARK(a, PH_WEIGHTS);
-        // ---- refit proposal i+1 to the weighted samples (estimate_params, epropnp.py:317-342).
-        // Four block reductions, one barrier each:
+        // ---- refit proposal i+1 to the weighted samples (estimate_params; 6DoF epropnp.py:317-342, 4DoF :232-260).
+        // One block reduction, one barrier each:
         //   A  max of the log-weights
-        //   B  e = exp(lw - max): sum e, sum e t, and ACG fixed-point iteration 1 (Lambda_0 = I, so
-        //      M = q.q) -- the normalisation of the weights cancels in Lambda
-        //   C  translation covariance about the mean (+ ACG iteration 2)
-        //   D+ remaining ACG iterations
+        //   B  e = exp(lw - max): sum e, sum e t; 6DoF: and ACG fixed-point iteration 1 (Lambda_0 = I, so
+        //      M = q.q) -- the normalisation of the weights cancels in Lambda; 4DoF: and sum e sin, sum e cos
+        //   C  translation covariance about the mean (6DoF: + ACG iteration 2)
+        //   D+ 6DoF: remaining ACG iterations
         mx = block_max<T>(mx, sh.red, 0);
-        float lam10[10];
+        // the refit's results live to the end of the iteration: scoped to the 6DoF branch, they change that family's
+        // 512-thread code
+        float lam10[10];                    // 6DoF: the ACG scatter
         float mean[3], inv_sum;
-        {
-            float acc[15];
-#pragma unroll
-            for (int r = 0; r < 15; ++r) acc[r] = 0.f;
-            for (int m = tid; m < n; m += T) {
-                const float e = fast_exp(logweight(m) - mx);
-                const float* s7 = smp + m * 7;
-                acc[0] += e;
-                acc[1] = fmaf(e, s7[0], acc[1]); acc[2] = fmaf(e, s7[1], acc[2]); acc[3] = fmaf(e, s7[2], acc[3]);
-                const float* q = s7 + 3;
-                const float mq = fmaxf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3], p.amis_eps);
-                const float wm = e / mq;
-                acc[4] += wm;
-                int idx = 5;
-#pragma unroll
-                for (int r = 0; r < 4; ++r)
-#pragma unroll
-                    for (int c = r; c < 4; ++c) { acc[idx] = fmaf(wm * q[r], q[c], acc[idx]); ++idx; }
-            }
-            amis_block_sum<15, T>(acc, sh.red, 1);
-            inv_sum = 1.0f / acc[0];
-            mean[0] = acc[1] * inv_sum; mean[1] = acc[2] * inv_sum; mean[2] = acc[3] * inv_sum;
-            const float inv0 = 1.0f / acc[4];
-#pragma unroll
-            for (int r = 0; r < 10; ++r) lam10[r] = acc[5 + r] * inv0;
-            lam10[0] += p.amis_eps; lam10[4] += p.amis_eps; lam10[7] += p.amis_eps; lam10[9] += p.amis_eps;
-        }
-        if (p.acg_mle_iter == 0) {          // degenerate configuration: Lambda stays the identity
-#pragma unroll
-            for (int r = 0; r < 10; ++r) lam10[r] = 0.f;
-            lam10[0] = lam10[4] = lam10[7] = lam10[9] = 1.f;
-        }
         float tc[6];
-        {
-            const bool more = p.acg_mle_iter >= 2;
-            float lam_inv[16];
-            if (more) acg_scatter_inverse(lam10, lam_inv);
-            float acc[17];
+        if constexpr (DOF == 6) {
+            {
+                float acc[15];
 #pragma unroll
-            for (int r = 0; r < 17; ++r) acc[r] = 0.f;
-            for (int m = tid; m < n; m += T) {
-                const float w = fast_exp(logweight(m) - mx) * inv_sum;       // normalised softmax weight
-                const float* s7 = smp + m * 7;
-                const float d0 = s7[0] - mean[0], d1 = s7[1] - mean[1], d2 = s7[2] - mean[2];
-                acc[11] = fmaf(w * d0, d0, acc[11]); acc[12] = fmaf(w * d0, d1, acc[12]); acc[13] = fmaf(w * d0, d2, acc[13]);
-                acc[14] = fmaf(w * d1, d1, acc[14]); acc[15] = fmaf(w * d1, d2, acc[15]); acc[16] = fmaf(w * d2, d2, acc[16]);
-                if (more) {
+                for (int r = 0; r < 15; ++r) acc[r] = 0.f;
+                for (int m = tid; m < n; m += T) {
+                    const float e = fast_exp(logweight(m) - mx);
+                    const float* s7 = smp + m * 7;
+                    acc[0] += e;
+                    acc[1] = fmaf(e, s7[0], acc[1]); acc[2] = fmaf(e, s7[1], acc[2]); acc[3] = fmaf(e, s7[2], acc[3]);
                     const float* q = s7 + 3;
-                    const float wm = w / fmaxf(quad4(lam_inv, q), p.amis_eps);
+                    const float mq = fmaxf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3], p.amis_eps);
+                    const float wm = e / mq;
+                    acc[4] += wm;
+                    int idx = 5;
+#pragma unroll
+                    for (int r = 0; r < 4; ++r)
+#pragma unroll
+                        for (int c = r; c < 4; ++c) { acc[idx] = fmaf(wm * q[r], q[c], acc[idx]); ++idx; }
+                }
+                amis_block_sum<15, T>(acc, sh.red, 1);
+                inv_sum = 1.0f / acc[0];
+                mean[0] = acc[1] * inv_sum; mean[1] = acc[2] * inv_sum; mean[2] = acc[3] * inv_sum;
+                const float inv0 = 1.0f / acc[4];
+#pragma unroll
+                for (int r = 0; r < 10; ++r) lam10[r] = acc[5 + r] * inv0;
+                lam10[0] += p.amis_eps; lam10[4] += p.amis_eps; lam10[7] += p.amis_eps; lam10[9] += p.amis_eps;
+            }
+            if (p.acg_mle_iter == 0) {          // degenerate configuration: Lambda stays the identity
+#pragma unroll
+                for (int r = 0; r < 10; ++r) lam10[r] = 0.f;
+                lam10[0] = lam10[4] = lam10[7] = lam10[9] = 1.f;
+            }
+            {
+                const bool more = p.acg_mle_iter >= 2;
+                float lam_inv[16];
+                if (more) acg_scatter_inverse(lam10, lam_inv);
+                float acc[17];
+#pragma unroll
+                for (int r = 0; r < 17; ++r) acc[r] = 0.f;
+                for (int m = tid; m < n; m += T) {
+                    const float w = fast_exp(logweight(m) - mx) * inv_sum;       // normalised softmax weight
+                    const float* s7 = smp + m * 7;
+                    const float d0 = s7[0] - mean[0], d1 = s7[1] - mean[1], d2 = s7[2] - mean[2];
+                    acc[11] = fmaf(w * d0, d0, acc[11]); acc[12] = fmaf(w * d0, d1, acc[12]); acc[13] = fmaf(w * d0, d2, acc[13]);
+                    acc[14] = fmaf(w * d1, d1, acc[14]); acc[15] = fmaf(w * d1, d2, acc[15]); acc[16] = fmaf(w * d2, d2, acc[16]);
+                    if (more) {
+                        const float* q = s7 + 3;
+                        const float wm = w / fmaxf(quad4(lam_inv, q), p.amis_eps);
+                        acc[0] += wm;
+                        int idx = 1;
+#pragma unroll
+                        for (int r = 0; r < 4; ++r)
+#pragma unroll
+                            for (int c = r; c < 4; ++c) { acc[idx] = fmaf(wm * q[r], q[c], acc[idx]); ++idx; }
+                    }
+                }
+                amis_block_sum<17, T>(acc, sh.red, 0);
+#pragma unroll
+                for (int r = 0; r < 6; ++r) tc[r] = acc[11 + r];
+                if (more) {
+                    const float inv0 = 1.0f / acc[0];
+#pragma unroll
+                    for (int r = 0; r < 10; ++r) lam10[r] = acc[1 + r] * inv0;
+                    lam10[0] += p.amis_eps; lam10[4] += p.amis_eps; lam10[7] += p.amis_eps; lam10[9] += p.amis_eps;
+                }
+            }
+            for (int itr = 2; itr < p.acg_mle_iter; ++itr) {
+                float lam_inv[16];
+                acg_scatter_inverse(lam10, lam_inv);
+                float acc[11];
+#pragma unroll
+                for (int r = 0; r < 11; ++r) acc[r] = 0.f;
+                for (int m = tid; m < n; m += T) {
+                    const float* q = smp + m * 7 + 3;
+                    const float wm = fast_exp(logweight(m) - mx) * inv_sum / fmaxf(quad4(lam_inv, q), p.amis_eps);
                     acc[0] += wm;
                     int idx = 1;
 #pragma unroll
@@ -293,182 +344,59 @@ __device__ void amis_phase6(const KArgs& a, AmisHead<6, T>& sh, const float* pts
 #pragma unroll
                         for (int c = r; c < 4; ++c) { acc[idx] = fmaf(wm * q[r], q[c], acc[idx]); ++idx; }
                 }
-            }
-            amis_block_sum<17, T>(acc, sh.red, 0);
-#pragma unroll
-            for (int r = 0; r < 6; ++r) tc[r] = acc[11 + r];
-            if (more) {
+                amis_block_sum<11, T>(acc, sh.red, (itr + 1) & 1);
                 const float inv0 = 1.0f / acc[0];
 #pragma unroll
                 for (int r = 0; r < 10; ++r) lam10[r] = acc[1 + r] * inv0;
                 lam10[0] += p.amis_eps; lam10[4] += p.amis_eps; lam10[7] += p.amis_eps; lam10[9] += p.amis_eps;
             }
-        }
-        for (int itr = 2; itr < p.acg_mle_iter; ++itr) {
-            float lam_inv[16];
-            acg_scatter_inverse(lam10, lam_inv);
-            float acc[11];
-#pragma unroll
-            for (int r = 0; r < 11; ++r) acc[r] = 0.f;
+            PH_MARK(a, PH_REFIT_SUMS);
+            if (tid == st) refit_finish6(mean, tc, lam10, p.acg_dispersion, sh.prop[i + 1]);
+        } else {
+            float accB[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
             for (int m = tid; m < n; m += T) {
-                const float* q = smp + m * 7 + 3;
-                const float wm = fast_exp(logweight(m) - mx) * inv_sum / fmaxf(quad4(lam_inv, q), p.amis_eps);
-                acc[0] += wm;
-                int idx = 1;
-#pragma unroll
-                for (int r = 0; r < 4; ++r)
-#pragma unroll
-                    for (int c = r; c < 4; ++c) { acc[idx] = fmaf(wm * q[r], q[c], acc[idx]); ++idx; }
+                const float e = fast_exp(logweight(m) - mx);
+                const float* s4 = smp + m * 4;
+                float sn, cs;
+                sincosf(s4[3], &sn, &cs);
+                accB[0] += e;
+                accB[1] = fmaf(e, s4[0], accB[1]); accB[2] = fmaf(e, s4[1], accB[2]); accB[3] = fmaf(e, s4[2], accB[3]);
+                accB[4] = fmaf(e, sn, accB[4]); accB[5] = fmaf(e, cs, accB[5]);
             }
-            amis_block_sum<11, T>(acc, sh.red, (itr + 1) & 1);
-            const float inv0 = 1.0f / acc[0];
+            block_sum<6, T>(accB, sh.red, 1);
+            inv_sum = 1.0f / accB[0];
+            mean[0] = accB[1] * inv_sum; mean[1] = accB[2] * inv_sum; mean[2] = accB[3] * inv_sum;
 #pragma unroll
-            for (int r = 0; r < 10; ++r) lam10[r] = acc[1 + r] * inv0;
-            lam10[0] += p.amis_eps; lam10[4] += p.amis_eps; lam10[7] += p.amis_eps; lam10[9] += p.amis_eps;
+            for (int r = 0; r < 6; ++r) tc[r] = 0.f;
+            for (int m = tid; m < n; m += T) {
+                const float w = fast_exp(logweight(m) - mx) * inv_sum;
+                const float* s4 = smp + m * 4;
+                const float d0 = s4[0] - mean[0], d1 = s4[1] - mean[1], d2 = s4[2] - mean[2];
+                tc[0] = fmaf(w * d0, d0, tc[0]); tc[1] = fmaf(w * d0, d1, tc[1]); tc[2] = fmaf(w * d0, d2, tc[2]);
+                tc[3] = fmaf(w * d1, d1, tc[3]); tc[4] = fmaf(w * d1, d2, tc[4]); tc[5] = fmaf(w * d2, d2, tc[5]);
+            }
+            block_sum<6, T>(tc, sh.red, 0);
+            PH_MARK(a, PH_REFIT_SUMS);
+            if (tid == st) refit_finish4(mean, tc, accB[4] * inv_sum, accB[5] * inv_sum, p.amis_eps, sh.prop[i + 1]);
         }
-        PH_MARK(a, PH_REFIT_SUMS);
-        if (tid == st) refit_finish6(mean, tc, lam10, p.acg_dispersion, sh.prop[i + 1]);
         PH_MARK(a, PH_REFIT_FINISH);
         __syncthreads();
     }
-    if (a.proposals && tid < I && (!SPLIT || sc.rank == 0)) {
+    if (a.proposals && tid < I && (!SPLIT || sc.rank == 0)) {   // (B, I, 19): mu3, Lt6, then Lr10 or mode, kappa, 0...
         float* o = a.proposals + ((size_t)obj * I + tid) * PROP_FLOATS;
         SPLIT_AUDIT_STORES(PROP_FLOATS);
-        const Proposal6& pr = sh.prop[tid];
+        const typename ProposalOf<DOF>::type& pr = sh.prop[tid];
         o[0] = pr.mu[0]; o[1] = pr.mu[1]; o[2] = pr.mu[2];
 #pragma unroll
         for (int r = 0; r < 6; ++r) o[3 + r] = pr.lt[r];
+        if constexpr (DOF == 6) {
 #pragma unroll
-        for (int r = 0; r < 10; ++r) o[9 + r] = pr.lr[r];
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// AMIS loop for the resident object, 4DoF (EProPnP4DoF, epropnp.py:199-260): same skeleton as amis_phase6
-// with the yaw proposal 0.75 von Mises + 0.25 uniform.  Injected noise: noise_rot (B, M) holds the yaw
-// draws themselves (the reference samples them with numpy on the host, distributions.py:61-72, so there
-// is no base noise to replay).
-// SPLIT: the cluster form (sc describes the CTA's share); every rank draws the same samples and, after the exchange of
-// the partial costs, holds the same costs, so each runs the same refits; rank 0 alone writes the outputs.
-template <int T, bool SPLIT = false>
-__device__ void amis_phase4(const KArgs& a, AmisHead<4, T>& sh, const float* pts4, float* smp, float* cst, float* logp,
-                            float* cpart, const Cam& cam, float delta, int obj, const SplitCtx sc = SplitCtx{}) {
-    constexpr int PARTS = T / NT;
-    const Params& p = a.p;
-    const int tid = threadIdx.x;
-    const int M = p.mc_samples, I = p.mc_iter, S = M / I;
-    const bool injected = a.noise_n3 != nullptr;
-    const int st = serial_thread<T>(a);
-    float* const logw_out = a.logw + (size_t)obj * M;
-    PH_DECL;
-
-    for (int i = 0; i < I; ++i) {
-        for (int s = tid; s < S; s += NT) {
-            if (PARTS > 1 && tid >= NT) break;
-            const int m = i * S + s;
-            float n3[3], chi2, q[4];
-            if (injected) {
-                const size_t g = (size_t)obj * M + m;
-                n3[0] = __ldg(a.noise_n3 + g * 3); n3[1] = __ldg(a.noise_n3 + g * 3 + 1); n3[2] = __ldg(a.noise_n3 + g * 3 + 2);
-                chi2 = __ldg(a.noise_chi2 + g);
-                q[3] = __ldg(a.noise_rot + g);
-            } else {
-                draw_base_noise_t(a.seed, a.obj_offset + (uint32_t)obj, (uint32_t)m, n3, chi2);
-                q[3] = draw_yaw(a.seed, a.obj_offset + (uint32_t)obj, (uint32_t)m, s, S, sh.prop[i].mode, sh.prop[i].kappa);
-            }
-            draw_translation(sh.prop[i].mu, sh.prop[i].lt, n3, chi2, q);
+            for (int r = 0; r < 10; ++r) o[9 + r] = pr.lr[r];
+        } else {
+            o[9] = pr.mode; o[10] = pr.kappa;
 #pragma unroll
-            for (int k = 0; k < 4; ++k) smp[m * 4 + k] = q[k];
-            if constexpr (PARTS == 1) cst[m] = pose_cost_pairs<4>(pts4, 0, (a.N + 1) >> 1, q, cam, delta, sh.box);
-            RunningLse l;
-            l.start(proposal_logpdf4(sh.prop[0], q));
-            for (int j = 1; j <= i; ++j) l.add(proposal_logpdf4(sh.prop[j], q));
-            logp[m] = l.value();
+            for (int r = 11; r < PROP_FLOATS; ++r) o[r] = 0.f;
         }
-        if constexpr (PARTS > 1) {
-            __syncthreads();
-            const int part = tid / NT, npair = SPLIT ? sc.npair : (a.N + 1) >> 1;
-            const int j0 = (int)((long long)npair * part / PARTS) & ~3, j1 = part + 1 == PARTS ? npair : ((int)((long long)npair * (part + 1) / PARTS) & ~3);
-            for (int s = tid % NT; s < S; s += NT) {
-                const int m = i * S + s;
-                cpart[part * M + m] = pose_cost_pairs<4>(pts4, j0, j1, smp + m * 4, cam, delta, sh.box);
-            }
-            __syncthreads();
-            for (int s = tid; s < S; s += T) {
-                const int m = i * S + s;
-                float c = cpart[m];
-#pragma unroll
-                for (int r = 1; r < PARTS; ++r) c += cpart[r * M + m];
-                if constexpr (SPLIT) sc.xbuf[(i & 1) * S + s] = c;
-                else cst[m] = c;
-            }
-            if constexpr (SPLIT) {
-                // One cluster barrier per iteration: the half (i & 1) of xbuf is written again at iteration i + 2, after
-                // the barrier of iteration i + 1, which every rank reaches only once its reads below are done.
-                cluster_sync();
-                for (int s = tid; s < S; s += T) {
-                    const float* x = sc.xbuf + (i & 1) * S + s;
-                    float c = dsmem_ld(x, 0);
-                    for (int r = 1; r < sc.ctas; ++r) c += dsmem_ld(x, r);
-                    cst[i * S + s] = c;
-                }
-            }
-        }
-        PH_MARK(a, PH_DRAW_SWEEP);
-        for (int m = tid; m < i * S; m += T) logp[m] = log_add_exp(logp[m], proposal_logpdf4(sh.prop[i], smp + m * 4));
-        __syncthreads();
-        PH_MARK(a, PH_LOGP_OLD);
-        const int n = (i + 1) * S;
-        const float log_cnt = logf((float)(i + 1));
-        auto logweight = [&](int m) { return -cst[m] - (logp[m] - log_cnt); };
-        if (i == I - 1) {
-            if (!SPLIT || sc.rank == 0)
-                for (int m = tid; m < M; m += T) { logw_out[m] = logweight(m); SPLIT_AUDIT_STORES(1); }
-            PH_MARK(a, PH_OUTPUT);
-            break;
-        }
-        float mx = -CUDART_INF_F;
-        for (int m = tid; m < n; m += T) mx = fmaxf(mx, logweight(m));
-        PH_MARK(a, PH_WEIGHTS);
-        // ---- refit (estimate_params, epropnp.py:232-260): A max, B sums of e, e t, e sin, e cos, C covariance
-        mx = block_max<T>(mx, sh.red, 0);
-        float accB[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        for (int m = tid; m < n; m += T) {
-            const float e = fast_exp(logweight(m) - mx);
-            const float* s4 = smp + m * 4;
-            float sn, cs;
-            sincosf(s4[3], &sn, &cs);
-            accB[0] += e;
-            accB[1] = fmaf(e, s4[0], accB[1]); accB[2] = fmaf(e, s4[1], accB[2]); accB[3] = fmaf(e, s4[2], accB[3]);
-            accB[4] = fmaf(e, sn, accB[4]); accB[5] = fmaf(e, cs, accB[5]);
-        }
-        block_sum<6, T>(accB, sh.red, 1);
-        const float inv_sum = 1.0f / accB[0];
-        const float mean[3] = {accB[1] * inv_sum, accB[2] * inv_sum, accB[3] * inv_sum};
-        float tc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        for (int m = tid; m < n; m += T) {
-            const float w = fast_exp(logweight(m) - mx) * inv_sum;
-            const float* s4 = smp + m * 4;
-            const float d0 = s4[0] - mean[0], d1 = s4[1] - mean[1], d2 = s4[2] - mean[2];
-            tc[0] = fmaf(w * d0, d0, tc[0]); tc[1] = fmaf(w * d0, d1, tc[1]); tc[2] = fmaf(w * d0, d2, tc[2]);
-            tc[3] = fmaf(w * d1, d1, tc[3]); tc[4] = fmaf(w * d1, d2, tc[4]); tc[5] = fmaf(w * d2, d2, tc[5]);
-        }
-        block_sum<6, T>(tc, sh.red, 0);
-        PH_MARK(a, PH_REFIT_SUMS);
-        if (tid == st) refit_finish4(mean, tc, accB[4] * inv_sum, accB[5] * inv_sum, p.amis_eps, sh.prop[i + 1]);
-        PH_MARK(a, PH_REFIT_FINISH);
-        __syncthreads();
-    }
-    if (a.proposals && tid < I && (!SPLIT || sc.rank == 0)) {       // (B, I, 19): mu3, Lt6, mode, kappa, 0...
-        float* o = a.proposals + ((size_t)obj * I + tid) * PROP_FLOATS;
-        SPLIT_AUDIT_STORES(PROP_FLOATS);
-        const Proposal4& pr = sh.prop[tid];
-        o[0] = pr.mu[0]; o[1] = pr.mu[1]; o[2] = pr.mu[2];
-#pragma unroll
-        for (int r = 0; r < 6; ++r) o[3 + r] = pr.lt[r];
-        o[9] = pr.mode; o[10] = pr.kappa;
-#pragma unroll
-        for (int r = 11; r < PROP_FLOATS; ++r) o[r] = 0.f;
     }
 }
 
@@ -510,6 +438,21 @@ __device__ __noinline__ void push_rows(const float* src, const float* pose, size
     }
 }
 
+// The serial thread's part of the set-up: the LM solution and its covariance from global memory, and the first proposal
+// fitted to them (EProPnP*.initial_fit: fp64 factorizations, ~12 k cycles on one lane).  The covariance is read BEFORE
+// this object's sample rows are written: the fused entry point may have parked it there (cov_stride = M * D); plain
+// loads, that memory is written later in this launch.
+template <int DOF, int T>
+__device__ __forceinline__ void amis_initial_fit(const KArgs& a, AmisHead<DOF, T>& sh, int obj) {
+    constexpr int PD = Dim<DOF>::POSE;
+#pragma unroll
+    for (int i = 0; i < PD; ++i) sh.pose[i] = a.pose_opt_in[(size_t)obj * PD + i];
+#pragma unroll
+    for (int i = 0; i < DOF * DOF; ++i) sh.cov[i] = a.pose_cov_in[(size_t)obj * a.cov_stride + i];
+    if constexpr (DOF == 6) initial_fit6(sh.pose, sh.cov, a.p.acg_dispersion, sh.prop[0]);
+    else initial_fit4(sh.pose, sh.cov, a.p.amis_eps, sh.prop[0]);
+}
+
 // One object per CTA of T threads (blockIdx.x = object).  The body of amis_kernel and amis_seedptr_kernel.
 template <int DOF, int T>
 __device__ __forceinline__ void amis_body(const KArgs& a, const PushArgs& push) {
@@ -524,21 +467,11 @@ __device__ __forceinline__ void amis_body(const KArgs& a, const PushArgs& push) 
     float* pts4 = dyn + pl.pts;
     const int obj = blockIdx.x, tid = threadIdx.x;
     PH_DECL;
-    // Set-up, two things at once.  The serial warp's lane 0 fetches the LM solution and fits the first proposal to it
-    // (EProPnP*.initial_fit: fp64 factorizations, ~12 k cycles on one lane); the other warps meanwhile pull the object's
-    // correspondences through the TMA ring and pack them (named barrier 1 among themselves).  The covariance is read
-    // BEFORE this object's sample rows are written: the fused entry point may have parked it there (cov_stride = M * D);
-    // plain loads, that memory is written later in this launch.
+    // Set-up, two things at once: the serial warp's lane 0 fits the first proposal, the other warps meanwhile pull the
+    // object's correspondences through the TMA ring and pack them (named barrier 1 among themselves).
     const int serial_warp = st >> 5;
     if ((tid >> 5) == serial_warp) {
-        if (tid == st) {
-#pragma unroll
-            for (int i = 0; i < PD; ++i) sh.pose[i] = a.pose_opt_in[(size_t)obj * PD + i];
-#pragma unroll
-            for (int i = 0; i < DOF * DOF; ++i) sh.cov[i] = a.pose_cov_in[(size_t)obj * a.cov_stride + i];
-            if constexpr (DOF == 6) initial_fit6(sh.pose, sh.cov, a.p.acg_dispersion, sh.prop[0]);
-            else initial_fit4(sh.pose, sh.cov, a.p.amis_eps, sh.prop[0]);
-        }
+        if (tid == st) amis_initial_fit(a, sh, obj);
     } else {
         LoaderT<(T > NT ? AMIS_CHUNK_DENSE : CH)> ld(a, sh.bar, dyn + pl.stage);
         ld.template load_object<T>(obj, pts4, serial_warp);
@@ -548,8 +481,7 @@ __device__ __forceinline__ void amis_body(const KArgs& a, const PushArgs& push) 
     const Cam cam = load_cam(a, obj);
     const float delta = __ldg(a.delta + obj);
     PH_MARK(a, PH_LOAD);
-    if constexpr (DOF == 6) amis_phase6<T>(a, sh, pts4, dyn + pl.smp, dyn + pl.cost, dyn + pl.logp, dyn + pl.cpart, cam, delta, obj);
-    else amis_phase4<T>(a, sh, pts4, dyn + pl.smp, dyn + pl.cost, dyn + pl.logp, dyn + pl.cpart, cam, delta, obj);
+    amis_loop<DOF, T, false>(a, sh, pts4, dyn + pl.smp, dyn + pl.cost, dyn + pl.logp, dyn + pl.cpart, cam, delta, obj);
     // The samples leave as one contiguous run per object: `smp` holds them in the output's (M, PD) layout, complete since
     // the AMIS loop's last barrier.  (The covariance the fused call may have parked in these rows was read at set-up.)
     block_copy<T>(a.pose_samples + (size_t)obj * M * PD, dyn + pl.smp, M * PD);
@@ -583,9 +515,9 @@ __global__ void __launch_bounds__(T, T == NT ? AMIS_CTAS_PER_SM : 1)
 // holding the contiguous point range [r share, (r + 1) share) (split_share).  Every rank runs the whole AMIS control
 // flow of amis_kernel<DOF, 512> on the same samples -- Philox keyed by (seed, obj_offset + object, m), or the same
 // injected noise -- and sweeps only its own range, in the dense kernel's four point ranges.  Per iteration the ranks
-// exchange their per-sample partial costs through distributed shared memory and add them in rank order 0 .. ctas - 1, so
-// all ranks hold bit-identical costs and log-densities and compute the refits redundantly (no proposal broadcast).  The
-// result depends on ctas (the order of that sum), never on B, the shard or obj_offset.
+// exchange their per-sample partial costs through distributed shared memory and add them (sum_ranks), so all ranks
+// hold bit-identical costs and log-densities and compute the refits redundantly (no proposal broadcast).  The result
+// depends on ctas, never on B, the shard or obj_offset.
 constexpr int SPLIT_MAX_CTAS = 8;                   // the portable cluster size
 
 // Points per rank: ceil(N / C) rounded up to a multiple of 8, so every range starts where a bulk copy may start; the
@@ -638,14 +570,7 @@ __device__ __forceinline__ void amis_split_body(const KArgs& a, const int ctas) 
     // writes the sample rows only after the AMIS loop: no rank can read a row that rank 0 has overwritten.
     const int serial_warp = st >> 5;
     if ((tid >> 5) == serial_warp) {
-        if (tid == st) {
-#pragma unroll
-            for (int i = 0; i < PD; ++i) sh.pose[i] = a.pose_opt_in[(size_t)obj * PD + i];
-#pragma unroll
-            for (int i = 0; i < DOF * DOF; ++i) sh.cov[i] = a.pose_cov_in[(size_t)obj * a.cov_stride + i];
-            if constexpr (DOF == 6) initial_fit6(sh.pose, sh.cov, a.p.acg_dispersion, sh.prop[0]);
-            else initial_fit4(sh.pose, sh.cov, a.p.amis_eps, sh.prop[0]);
-        }
+        if (tid == st) amis_initial_fit(a, sh, obj);
     } else {
         LoaderT<CH> ld(a, sh.bar, dyn + pl.a.stage);
         ld.template load_range<T>(obj, pts4, p0, p1, serial_warp);
@@ -658,10 +583,7 @@ __device__ __forceinline__ void amis_split_body(const KArgs& a, const int ctas) 
     const float delta = __ldg(a.delta + obj);
     PH_MARK(a, PH_LOAD);
     const SplitCtx sc{dyn + pl.xbuf, rank, ctas, (p1 - p0 + 1) >> 1};
-    if constexpr (DOF == 6)
-        amis_phase6<T, true>(a, sh, pts4, dyn + pl.a.smp, dyn + pl.a.cost, dyn + pl.a.logp, dyn + pl.a.cpart, cam, delta, obj, sc);
-    else
-        amis_phase4<T, true>(a, sh, pts4, dyn + pl.a.smp, dyn + pl.a.cost, dyn + pl.a.logp, dyn + pl.a.cpart, cam, delta, obj, sc);
+    amis_loop<DOF, T, true>(a, sh, pts4, dyn + pl.a.smp, dyn + pl.a.cost, dyn + pl.a.logp, dyn + pl.a.cpart, cam, delta, obj, sc);
 #ifdef EPNP_SPLIT_AUDIT
     cluster_sync();                         // every rank's state is final
     for (int m = tid; m < M; m += T) {

@@ -1,7 +1,7 @@
 // pnp_device.cuh -- device-side plumbing shared by the sm_90a kernels of the EPro-PnP hot path: launch / shared-memory
 // macros (which also let the file build under the test-only CPU SIMT emulator), mbarrier + 1-D TMA bulk-copy wrappers,
-// special-function functors, the kernel argument block, warp / block reductions, the packed point store with its TMA
-// loader, and the Huber cost sweep over the resident points.  Included by pnp_kernels.cu only.
+// special-function functors, the rank-ordered cluster sums, the kernel argument block, warp / block reductions, the packed
+// point store with its TMA loader, and the Huber cost sweep over the resident points.  Included by pnp_kernels.cu only.
 #pragma once
 #include <cuda_runtime.h>
 #include <math_constants.h>
@@ -154,6 +154,26 @@ struct FastRsqrt {
     __device__ __forceinline__ float operator()(float x) const { float r; asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 };
 #endif
+
+__device__ __forceinline__ double dsmem_ld_f64(const double* p, int rank) {
+    const float* f = reinterpret_cast<const float*>(p);
+    uint32_t h[2] = {__float_as_uint(dsmem_ld(f, rank)), __float_as_uint(dsmem_ld(f + 1, rank))};
+    double v;
+    memcpy(&v, h, 8);
+    return v;
+}
+// The sum over the cluster of the value at `p`'s offset, added in rank order 0 .. ctas - 1.  Every cross-rank sum of the
+// split kernels goes through here: with the order fixed, a result depends on the cluster size, never on the batch.
+__device__ __forceinline__ float sum_ranks(const float* p, int ctas) {
+    float v = dsmem_ld(p, 0);
+    for (int r = 1; r < ctas; ++r) v += dsmem_ld(p, r);
+    return v;
+}
+__device__ __forceinline__ double sum_ranks(const double* p, int ctas) {
+    double v = dsmem_ld_f64(p, 0);
+    for (int r = 1; r < ctas; ++r) v += dsmem_ld_f64(p, r);
+    return v;
+}
 
 // ------------------------------------------------------------------------------------------------
 struct KArgs {

@@ -16,7 +16,8 @@
 //   amis_split_kernel (pnp_amis.cuh), cost_split_kernel, gn_plus_backward_split_kernel, epnp_init_split_kernel   the AMIS
 //                                    loop, the stacked-pose cost, the pose_opt_plus backward and the EPnP initialiser for
 //                                    objects whose points do not fit one SM: one thread-block CLUSTER of 2..8 CTAs per
-//                                    object, each holding a point range, partial sums added over distributed shared memory.
+//                                    object, each holding a point range, partial sums added in rank order over distributed
+//                                    shared memory (sum_ranks, pnp_device.cuh).
 //   push_split_kernel                the multi-GPU gather of the split solve: this rank's rows copied into its peers' buffers.
 // No tensor cores: the only contraction is 6-deep, the work is FP32-pipe + MUFU bound (DESIGN.md).
 // Build options: EPNP_PHASE_TIMERS (profiling), EPNP_SIMT_EMUL (g++ build for the test-only CPU emulator).
@@ -76,8 +77,7 @@ __global__ void __launch_bounds__(NT, 4) cost_kernel(const KArgs a) {
 
 // cost_kernel for objects too large for one SM: one cluster of `ctas` CTAs per object (grid = B * ctas), rank r holding
 // the points [r share, (r + 1) share) (split_share).  Every rank evaluates every pose on its own range, COST_SPLIT_TILE
-// poses at a time (one per thread); rank 0 adds the ranks' partial costs in rank order through distributed shared memory
-// and writes the result.  The result depends on ctas (the order of that sum), never on B.
+// poses at a time (one per thread); rank 0 adds the ranks' partial costs (sum_ranks) and writes the result.
 constexpr int COST_SPLIT_TILE = 512;
 struct CostSplitPlan { int stage, pts, xbuf, total_bytes; };
 __host__ __device__ inline CostSplitPlan plan_cost_split(int share) {
@@ -120,9 +120,7 @@ __global__ void __launch_bounds__(COST_SPLIT_TILE, 1) cost_split_kernel(const KA
         *x = part;
         cluster_sync();
         if (rank == 0 && s < a.S_eval) {
-            float c = dsmem_ld(x, 0);
-            for (int r = 1; r < ctas; ++r) c += dsmem_ld(x, r);
-            a.cost_out[(size_t)s * a.B + obj] = c;
+            a.cost_out[(size_t)s * a.B + obj] = sum_ranks(x, ctas);
             SPLIT_AUDIT_STORES(1);
         }
     }
@@ -621,9 +619,9 @@ __global__ void __launch_bounds__(NT, 2) gn_plus_backward_kernel(const GnBwArgs 
 // object (grid = B * ctas), rank r holding the points [r share, (r + 1) share) (split_share) in plan_cost_split(share),
 // with the head below in the 2 x COST_SPLIT_TILE floats the cost kernel uses for its partial costs -- so C and the point
 // limit are the cost kernel's.  Every rank evaluates the normal equations on its own range, reads every rank's partial
-// through distributed shared memory and adds them in rank order 0 .. ctas - 1: all ranks hold the same bits of H, g and
-// cost, and their serial threads form the same step and v (no broadcast).  Each rank then writes the gradient rows of
-// its own points; rank 0 adds the ranks' grad_delta partials in rank order.  The result depends on ctas, never on B.
+// through distributed shared memory and adds them (sum_ranks): all ranks hold the same bits of H, g and cost, and their
+// serial threads form the same step and v (no broadcast).  Each rank then writes the gradient rows of its own points;
+// rank 0 adds the ranks' grad_delta partials.
 constexpr int GNBW_SPLIT_T = 512;
 template <int DOF> struct GnBwSplitHead {
     float red[GNBW_SPLIT_T];            // eval_normal_eq / block_sum scratch
@@ -658,11 +656,7 @@ __global__ void __launch_bounds__(GNBW_SPLIT_T, 1) gn_plus_backward_split_kernel
     // read it, and never again -- the two slots are distinct, so no rank can overwrite what another is still reading.
     eval_normal_eq<DOF, true, T>(pts, cnt, sh.pose, cam, delta, a.p.huber_eps, sh.red, sh.part);
     cluster_sync();
-    if (tid < NV) {
-        float v = dsmem_ld(sh.part + tid, 0);
-        for (int r = 1; r < ctas; ++r) v += dsmem_ld(sh.part + tid, r);
-        sh.ev[tid] = v;
-    }
+    if (tid < NV) sh.ev[tid] = sum_ranks(sh.part + tid, ctas);
     __syncthreads();
     float* step = sh.step;              // [DOF]
     float* vvec = sh.step + DOF;        // [DOF]
@@ -711,9 +705,7 @@ __global__ void __launch_bounds__(GNBW_SPLIT_T, 1) gn_plus_backward_split_kernel
     }
 #endif
     if (rank == 0 && tid == 0 && g.gdelta) {
-        float c = dsmem_ld(sh.gdpart, 0);
-        for (int r = 1; r < ctas; ++r) c += dsmem_ld(sh.gdpart, r);
-        g.gdelta[obj] = c;
+        g.gdelta[obj] = sum_ranks(sh.gdpart, ctas);
         SPLIT_AUDIT_STORES(1);
     }
     // Ordering rule 2: a CTA's shared memory disappears when it exits; this barrier keeps every CTA of the cluster alive
@@ -1046,8 +1038,7 @@ __global__ void __launch_bounds__(NT, 4) cost_pose_backward_kernel(const PoseBwA
 // holds the points [r share, (r + 1) share) and sweeps them for a tile of COST_SPLIT_TILE poses (one per thread).  The
 // 12 sums of a pose cross ranks through the staging ring, which is free once the points are loaded and holds them for
 // POSE_BW_PASS poses: the tile is exchanged pass by pass -- the pass's threads write their sums, a cluster barrier,
-// rank 0 adds the ranks' sums in rank order 0 .. ctas - 1 through distributed shared memory, contracts and stores, a
-// second barrier frees the slot.  The gradient depends on ctas (the order of that sum), never on B.
+// rank 0 adds the ranks' sums (sum_ranks), contracts and stores, a second barrier frees the slot.
 constexpr int POSE_BW_PASS = 128;
 static_assert(12 * POSE_BW_PASS <= 2 * STAGE_FLOATS, "a pass's sums must fit the staging ring");
 static_assert(COST_SPLIT_TILE % POSE_BW_PASS == 0, "whole passes per tile");
@@ -1088,11 +1079,7 @@ __global__ void __launch_bounds__(COST_SPLIT_TILE, 1) cost_pose_backward_split_k
             if (rank == 0 && mine) {
                 float sum[12], out[PD];
 #pragma unroll
-                for (int k = 0; k < 12; ++k) {
-                    float v = dsmem_ld(x + k * POSE_BW_PASS, 0);
-                    for (int r = 1; r < ctas; ++r) v += dsmem_ld(x + k * POSE_BW_PASS, r);
-                    sum[k] = v;
-                }
+                for (int k = 0; k < 12; ++k) sum[k] = sum_ranks(x + k * POSE_BW_PASS, ctas);
                 pose_grad_contract<DOF>(sum, pose, cam, __ldg(g.grad + row), out);
 #pragma unroll
                 for (int k = 0; k < PD; ++k) g.gpose[row * PD + k] = out[k];
@@ -1363,7 +1350,7 @@ __global__ void __launch_bounds__(NT) epnp_init_kernel(const EpnpInitArgs a) {
 // epnp_init_kernel for objects too large for one SM (epnp_epnp_init_split_f32): one cluster of `ctas` CTAs per object
 // (grid = B * ctas), rank r holding the points [r share, (r + 1) share) (split_share).  Each rank runs the resident
 // kernel's steps over its own range.  What crosses ranks goes through an exchange slot in the rank's shared memory and
-// one cluster barrier, after which every rank adds the ranks' values in rank order 0 .. ctas - 1:
+// one cluster barrier, after which every rank adds the ranks' values (sum_ranks):
 //   1. the NaN counts: an object with a NaN confidence anywhere takes the NaN path on every rank;
 //   2. per radix-select pass, the two counts over the global N (integers, exact in fp32: the threshold and the kept set
 //      are np.quantile's over all N points whatever ctas is);
@@ -1371,7 +1358,7 @@ __global__ void __launch_bounds__(NT) epnp_init_kernel(const EpnpInitArgs a) {
 //      in index order, which fixes the sign of the camera-frame control points; every rank reads it from there;
 //   4. the fp64 partials of the centroid, the scatter, the 56 EPnP sums and the three reprojection errors.
 // So every rank holds the same bits and runs control_points / solve_candidates itself (no broadcast); rank 0 alone
-// writes pose and n_sel.  The result depends on ctas (the order of the fp64 sums over ranks), never on B.
+// writes pose and n_sel.
 // Ordering: each exchange slot is written once, before the cluster barrier after which its peers read it -- except the
 // radix counts, whose two halves alternate by pass: a half is written again two passes later, past the next barrier,
 // which no rank reaches before its reads of that half are done.  Every rank passes the same barriers whatever its range
@@ -1402,21 +1389,8 @@ static_assert(EPNP_SPLIT_HEAD_BYTES <= 128 + (2 * STAGE_FLOATS + 2 * COST_SPLIT_
               "the EPnP split image must not exceed the cost split image at any share");
 __host__ __device__ inline int epnp_split_smem_bytes(int share) { return EPNP_SPLIT_HEAD_BYTES + share * 6 * 4; }
 
-__device__ __forceinline__ double dsmem_ld_f64(const double* p, int rank) {
-    const float* f = reinterpret_cast<const float*>(p);
-    uint32_t h[2] = {__float_as_uint(dsmem_ld(f, rank)), __float_as_uint(dsmem_ld(f + 1, rank))};
-    double v;
-    memcpy(&v, h, 8);
-    return v;
-}
-__device__ __forceinline__ float sum_ranks(const float* p, int ctas) {
-    float v = dsmem_ld(p, 0);
-    for (int r = 1; r < ctas; ++r) v += dsmem_ld(p, r);
-    return v;
-}
-
-// this rank's block sums of K fp64 values -> `slot`; one cluster barrier; thread k < K adds slot k of ranks 0 .. ctas - 1
-// in rank order into tot[k]; every thread gets the totals in v.  (The totals go on in a thread-local array, as in
+// this rank's block sums of K fp64 values -> `slot`; one cluster barrier; thread k < K adds slot k of every rank into
+// tot[k]; every thread gets the totals in v.  (The totals go on in a thread-local array, as in
 // epnp_init_kernel: pnp_epnp.cuh's out-of-line functions then see the address spaces they see there, and
 // epnp_init_kernel's code does not change.)
 template <int K>
@@ -1427,11 +1401,7 @@ __device__ __forceinline__ void cluster_sum_f64(double (&v)[K], double* red, dou
         for (int k = 0; k < K; ++k) slot[k] = v[k];
     }
     cluster_sync();
-    if (threadIdx.x < K) {
-        double s = dsmem_ld_f64(slot + threadIdx.x, 0);
-        for (int r = 1; r < ctas; ++r) s += dsmem_ld_f64(slot + threadIdx.x, r);
-        tot[threadIdx.x] = s;
-    }
+    if (threadIdx.x < K) tot[threadIdx.x] = sum_ranks(slot + threadIdx.x, ctas);
     __syncthreads();
 #pragma unroll
     for (int k = 0; k < K; ++k) v[k] = tot[k];
