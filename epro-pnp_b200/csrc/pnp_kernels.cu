@@ -1090,6 +1090,338 @@ __global__ void __launch_bounds__(COST_SPLIT_TILE, 1) cost_pose_backward_split_k
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Backward of the cost with respect to the CAMERA: sum_p g[b, p] * d cost(pose[b, p]) / d (K_b, lb_b, ub_b) over the
+// two pose sets of BwArgs (A: (B, PA, D) with (B, PA) upstream; B [opt]: (B, PB, D) with (B, PB)), so the Monte-Carlo
+// backward (the samples with -dL/dlogw and the cost_init pose) is one launch.  cost_pose_backward_kernel's shape: one
+// CTA per object, thread <-> pose.  Per point pair_camera_grad takes pair_pose_grad's chain to the same 12 sums of
+// h = d cost / d (xh, yh, zh) and adds four: the gradient with respect to a clamped coordinate, which the pose path
+// drops, goes to the bound that clamped it (torch.maximum / torch.minimum in the reference).  Since x_h = K (R X + t),
+// d cost / d K = (sum h X^T) R^T + (sum h) t^T is linear in the sums: after each pose's sweep they contract to 13 values
+// (K row-major, then lbx lby ubx uby) times the pose's upstream, and each thread adds them over its own poses.  One
+// fixed-order block reduction per object, no atomics: the result depends on neither B nor the loader.
+constexpr int CAM_GRADS = 13;
+struct CamBwArgs {
+    KArgs k;                            // correspondences, camera, bounds, delta, p.z_min
+    const float *poses_a, *grad_a;      // (B, PA, D), (B, PA)
+    const float *poses_b, *grad_b;      // [opt] (B, PB, D), (B, PB)
+    float *gcam, *glb, *gub;            // [opt] (B, 3, 3), (B, 2), (B, 2)
+    int PA, PB;
+};
+
+template <bool BOUNDED>
+__device__ __forceinline__ void pair_camera_grad(const float (&P)[12], const Cam& cam, float delta, const float4 q0,
+                                                 const float4 q1, const float4 q2, const float4 q3, float2 (&h)[16]) {
+    const float2 X = make_float2(q0.x, q0.y), Y = make_float2(q0.z, q0.w), Z = make_float2(q1.x, q1.y);
+    const float2 nu = make_float2(q1.z, q1.w), nv = make_float2(q2.x, q2.y);
+    const float2 wu = make_float2(q2.z, q2.w), wv = make_float2(q3.x, q3.y);
+    const float2 xh = v2fma(splat(P[0]), X, v2fma(splat(P[1]), Y, v2fma(splat(P[2]), Z, splat(P[3]))));
+    const float2 yh = v2fma(splat(P[4]), X, v2fma(splat(P[5]), Y, v2fma(splat(P[6]), Z, splat(P[7]))));
+    const float2 zh = v2fma(splat(P[8]), X, v2fma(splat(P[9]), Y, v2fma(splat(P[10]), Z, splat(P[11]))));
+    const float2 iz = make_float2(FastRcp()(fmaxf(zh.x, cam.z_min)), FastRcp()(fmaxf(zh.y, cam.z_min)));
+    const float2 px = v2mul(xh, iz), py = v2mul(yh, iz);
+    float2 pxc = px, pyc = py;
+    if (BOUNDED) {
+        pxc.x = fminf(fmaxf(px.x, cam.lbx), cam.ubx); pxc.y = fminf(fmaxf(px.y, cam.lbx), cam.ubx);
+        pyc.x = fminf(fmaxf(py.x, cam.lby), cam.uby); pyc.y = fminf(fmaxf(py.y, cam.lby), cam.uby);
+    }
+    const float2 rx = v2mul(v2add(pxc, nu), wu), ry = v2mul(v2add(pyc, nv), wv);
+    const float2 s2 = v2fma(rx, rx, v2mul(ry, ry));
+    const float2 rs = make_float2(FastRsqrt()(fmaxf(s2.x, 1e-30f)), FastRsqrt()(fmaxf(s2.y, 1e-30f)));
+    const float2 s = v2mul(s2, rs);
+    const float2 k = make_float2(s.x <= delta ? 1.f : delta * rs.x, s.y <= delta ? 1.f : delta * rs.y);    // rho'
+    float2 gpx = v2mul(v2mul(k, rx), wu), gpy = v2mul(v2mul(k, ry), wv);
+    if (BOUNDED) {
+        // a clamped coordinate equals the bound it sits on: ub when it is ub (the outer min), else lb
+        const bool cx0 = pxc.x != px.x, cx1 = pxc.y != px.y, cy0 = pyc.x != py.x, cy1 = pyc.y != py.y;
+        const bool ux0 = pxc.x == cam.ubx, ux1 = pxc.y == cam.ubx, uy0 = pyc.x == cam.uby, uy1 = pyc.y == cam.uby;
+        h[12] = v2add(h[12], make_float2(cx0 && !ux0 ? gpx.x : 0.f, cx1 && !ux1 ? gpx.y : 0.f));
+        h[13] = v2add(h[13], make_float2(cy0 && !uy0 ? gpy.x : 0.f, cy1 && !uy1 ? gpy.y : 0.f));
+        h[14] = v2add(h[14], make_float2(cx0 && ux0 ? gpx.x : 0.f, cx1 && ux1 ? gpx.y : 0.f));
+        h[15] = v2add(h[15], make_float2(cy0 && uy0 ? gpy.x : 0.f, cy1 && uy1 ? gpy.y : 0.f));
+        gpx.x = cx0 ? 0.f : gpx.x; gpx.y = cx1 ? 0.f : gpx.y;
+        gpy.x = cy0 ? 0.f : gpy.x; gpy.y = cy1 ? 0.f : gpy.y;
+    }
+    const float2 gxh = v2mul(gpx, iz), gyh = v2mul(gpy, iz);
+    const float2 tz = v2fma(gxh, px, v2mul(gyh, py));
+    const float2 gzh = make_float2(zh.x >= cam.z_min ? -tz.x : 0.f, zh.y >= cam.z_min ? -tz.y : 0.f);
+    h[0] = v2add(h[0], gxh); h[1] = v2add(h[1], gyh); h[2] = v2add(h[2], gzh);
+    h[3] = v2fma(gxh, X, h[3]); h[4] = v2fma(gxh, Y, h[4]); h[5] = v2fma(gxh, Z, h[5]);
+    h[6] = v2fma(gyh, X, h[6]); h[7] = v2fma(gyh, Y, h[7]); h[8] = v2fma(gyh, Z, h[8]);
+    h[9] = v2fma(gzh, X, h[9]); h[10] = v2fma(gzh, Y, h[10]); h[11] = v2fma(gzh, Z, h[11]);
+}
+
+// acc += up * d cost(pose) / d (K, lb, ub) over the pair records [0, npair): the 16 sums, then their contraction
+template <int DOF>
+__device__ __forceinline__ void camera_grad_pose(const float* pts, int npair, const float* pose, const Cam& cam,
+                                                 float delta, float up, float (&acc)[CAM_GRADS]) {
+    float R[9], P[12];
+    pose_to_rot<DOF>(pose, R);
+    make_proj(cam.k, R, pose, P);
+    float2 h[16];
+#pragma unroll
+    for (int k = 0; k < 16; ++k) h[k] = splat(0.f);
+    const float4* q = reinterpret_cast<const float4*>(pts);
+    if (cam.bounded) {
+        for (int j = 0; j < npair; ++j) pair_camera_grad<true>(P, cam, delta, q[4 * j], q[4 * j + 1], q[4 * j + 2], q[4 * j + 3], h);
+    } else {
+        for (int j = 0; j < npair; ++j) pair_camera_grad<false>(P, cam, delta, q[4 * j], q[4 * j + 1], q[4 * j + 2], q[4 * j + 3], h);
+    }
+    float hs[16];
+#pragma unroll
+    for (int k = 0; k < 16; ++k) hs[k] = h[k].x + h[k].y;
+    // d cost / d K[i][j] = sum_c (sum h_i X_c) R[j][c] + (sum h_i) t_j
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+            acc[i * 3 + j] += up * (hs[3 + 3 * i] * R[3 * j] + hs[4 + 3 * i] * R[3 * j + 1] + hs[5 + 3 * i] * R[3 * j + 2]
+                                    + hs[i] * pose[j]);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) acc[9 + k] += up * hs[12 + k];
+}
+
+// The poses of both sets that thread threadIdx.x takes (stride T), each swept over the pair records [0, npair).
+template <int DOF, int T>
+__device__ __forceinline__ void camera_grad_poses(const CamBwArgs& g, int obj, const float* pts, int npair,
+                                                  const Cam& cam, float delta, float (&acc)[CAM_GRADS]) {
+    constexpr int PD = Dim<DOF>::POSE;
+    for (int p = threadIdx.x; p < g.PA + g.PB; p += T) {
+        const bool in_a = p < g.PA;
+        const size_t row = in_a ? (size_t)obj * g.PA + p : (size_t)obj * g.PB + (p - g.PA);
+        const float* src = (in_a ? g.poses_a : g.poses_b) + row * PD;
+        float pose[PD];
+#pragma unroll
+        for (int k = 0; k < PD; ++k) pose[k] = __ldg(src + k);
+        camera_grad_pose<DOF>(pts, npair, pose, cam, delta, __ldg((in_a ? g.grad_a : g.grad_b) + row), acc);
+    }
+}
+
+// The requested outputs of one object from its 13 totals.  Returns the number of floats stored.
+__device__ __forceinline__ int store_camera_grad(float* gcam, float* glb, float* gub, int obj,
+                                                 const float (&v)[CAM_GRADS]) {
+    int n = 0;
+    if (gcam) {
+#pragma unroll
+        for (int k = 0; k < 9; ++k) gcam[(size_t)obj * 9 + k] = v[k];
+        n += 9;
+    }
+    if (glb) { glb[(size_t)obj * 2] = v[9]; glb[(size_t)obj * 2 + 1] = v[10]; n += 2; }
+    if (gub) { gub[(size_t)obj * 2] = v[11]; gub[(size_t)obj * 2 + 1] = v[12]; n += 2; }
+    return n;
+}
+
+template <int DOF>
+__global__ void __launch_bounds__(NT, 4) cost_camera_backward_kernel(const CamBwArgs g) {
+    EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
+    ObjHead<DOF>& sh = *reinterpret_cast<ObjHead<DOF>*>(smem_raw);
+    float* dyn = reinterpret_cast<float*>(smem_raw);
+    const KArgs& a = g.k;
+    const ObjPlan pl = plan_obj<DOF>(a.N);
+    float* pts = dyn + pl.pts;
+    const int obj = blockIdx.x;
+    Loader ld(a, sh.bar, dyn + pl.stage);
+    ld.load_object(obj, pts);
+    const Cam cam = load_cam(a, obj);
+    const float delta = __ldg(a.delta + obj);
+    float acc[CAM_GRADS];
+#pragma unroll
+    for (int k = 0; k < CAM_GRADS; ++k) acc[k] = 0.f;
+    camera_grad_poses<DOF, NT>(g, obj, pts, (a.N + 1) >> 1, cam, delta, acc);
+    block_sum<CAM_GRADS>(acc, sh.red, 0);
+    if (threadIdx.x == 0) store_camera_grad(g.gcam, g.glb, g.gub, obj, acc);
+}
+
+// cost_camera_backward_kernel for objects too large for one SM, on cost_split_kernel's plan and cluster size: rank r
+// sweeps its points [r share, (r + 1) share) for every pose, contracts and reduces to 13 floats in the partial-cost
+// region; after a cluster barrier rank 0 adds the ranks' 13 in rank order (sum_ranks) and stores; a second barrier keeps
+// every CTA resident until then.  A rank with an empty range contributes zeros and passes both barriers.  The result
+// depends on ctas (the order of that sum), never on B.
+template <int DOF>
+__global__ void __launch_bounds__(COST_SPLIT_TILE, 1) cost_camera_backward_split_kernel(const CamBwArgs g, const int ctas) {
+    EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
+    float* dyn = reinterpret_cast<float*>(smem_raw);
+    constexpr int T = COST_SPLIT_TILE;
+    const KArgs& a = g.k;
+    const int share = split_share(a.N, ctas);
+    const CostSplitPlan pl = plan_cost_split(share);
+    const int rank = cluster_rank(), obj = blockIdx.x / ctas;
+    const int p0 = min(a.N, rank * share), p1 = min(a.N, p0 + share);
+    float* pts = dyn + pl.pts;
+    float* red = dyn + pl.xbuf;                         // block_sum scratch, one half: T floats
+    float* part = red + T;                              // exchange slot: this rank's 13 totals
+    Loader ld(a, reinterpret_cast<uint64_t*>(smem_raw), dyn + pl.stage);
+    ld.load_range<T>(obj, pts, p0, p1);
+    const Cam cam = load_cam(a, obj);
+    const float delta = __ldg(a.delta + obj);
+    float acc[CAM_GRADS];
+#pragma unroll
+    for (int k = 0; k < CAM_GRADS; ++k) acc[k] = 0.f;
+    camera_grad_poses<DOF, T>(g, obj, pts, (p1 - p0 + 1) >> 1, cam, delta, acc);
+    block_sum<CAM_GRADS, T>(acc, red, 0);
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < CAM_GRADS; ++k) part[k] = acc[k];
+    }
+    cluster_sync();
+    if (rank == 0 && threadIdx.x == 0) {
+        float v[CAM_GRADS];
+#pragma unroll
+        for (int k = 0; k < CAM_GRADS; ++k) v[k] = sum_ranks(part + k, ctas);
+        const int stored = store_camera_grad(g.gcam, g.glb, g.gub, obj, v);
+        SPLIT_AUDIT_STORES(stored);
+        (void)stored;
+    }
+    cluster_sync();                                     // no CTA leaves while rank 0 may still read its slot
+}
+
+// ------------------------------------------------------------------------------------------------
+// The camera gradient of pose_opt_plus = pose (+) gn_step(pose): gn_plus_backward_kernel's structure (normal equations at
+// the pose; the serial lane forms step and v), then thread <-> correspondence with gn_step_point_camera_backward (Dual<13>
+// seeded at K and the bounds), and one block reduction of 13 floats per object.  A launch of its own, made only when the
+// camera needs a gradient; gn_plus_backward's launch and outputs do not change.
+struct GnCamBwArgs {
+    KArgs k;                    // correspondences, camera, bounds, delta, poses = pose (B, D), p.eps / huber_eps / z_min
+    const float* gplus;         // (B, D)  dL/d pose_opt_plus
+    float *gcam, *glb, *gub;    // [opt] (B, 3, 3), (B, 2), (B, 2)
+};
+
+// The serial lane of both GN-plus camera kernels: step = the damped step at the pose, v = -(H + eps I)^-1 dL/dstep.
+template <int DOF>
+__device__ __forceinline__ void gn_plus_step_and_v(const float* ev, const float* pose_sh, const float* gplus, float eps,
+                                                   float* step, float* vvec) {
+    constexpr int PD = Dim<DOF>::POSE, NA = Dim<DOF>::NA;
+    float add[DOF], st[DOF], sbar[DOF], vv[DOF], gout[PD], pose[PD];
+#pragma unroll
+    for (int i = 0; i < DOF; ++i) add[i] = eps;
+#pragma unroll
+    for (int i = 0; i < PD; ++i) { pose[i] = pose_sh[i]; gout[i] = __ldg(gplus + i); }
+    damped_step_refined<DOF>(ev, ev + NA, add, st);
+    pose_add_backward<DOF>(pose, st, gout, sbar);
+    damped_step_refined<DOF>(ev, sbar, add, vv);
+#pragma unroll
+    for (int i = 0; i < DOF; ++i) { step[i] = st[i]; vvec[i] = vv[i]; }
+}
+
+// acc += the camera gradient of the points [0, cnt) of the pair records, thread tid of T.
+template <int DOF, int T>
+__device__ __forceinline__ void gn_plus_camera_points(const float* pts, int cnt, const float* pose_sh, const float* step,
+                                                      const Cam& cam, float delta, float huber_eps,
+                                                      float (&acc)[CAM_GRADS]) {
+    constexpr int PD = Dim<DOF>::POSE;
+    float R[9], t[3], sv[DOF], vv[DOF];
+    {
+        float ps[PD];
+#pragma unroll
+        for (int i = 0; i < PD; ++i) ps[i] = pose_sh[i];
+        pose_to_rot<DOF>(ps, R);
+        t[0] = ps[0]; t[1] = ps[1]; t[2] = ps[2];
+#pragma unroll
+        for (int i = 0; i < DOF; ++i) { sv[i] = step[i]; vv[i] = step[DOF + i]; }
+    }
+    for (int n = threadIdx.x; n < cnt; n += T) {
+        const float* q = pts + (n >> 1) * 16 + (n & 1);
+        gn_step_point_camera_backward<DOF>(R, t, cam, delta, huber_eps, q[0], q[2], q[4], -q[6], -q[8], q[10], q[12], vv,
+                                           sv, acc);
+    }
+}
+
+template <int DOF>
+__global__ void __launch_bounds__(NT, 2) gn_plus_camera_backward_kernel(const GnCamBwArgs g) {
+    const KArgs& a = g.k;
+    EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
+    ObjHead<DOF>& sh = *reinterpret_cast<ObjHead<DOF>*>(smem_raw);
+    float* dyn = reinterpret_cast<float*>(smem_raw);
+    const ObjPlan pl = plan_obj<DOF>(a.N);
+    float* pts = dyn + pl.pts;
+    constexpr int PD = Dim<DOF>::POSE;
+    const int tid = threadIdx.x, obj = blockIdx.x;
+    Loader ld(a, sh.bar, dyn + pl.stage);
+    ld.load_object(obj, pts);
+    const Cam cam = load_cam(a, obj);
+    const float delta = __ldg(a.delta + obj);
+    if (tid < PD) sh.pose[tid] = __ldg(a.poses + (size_t)obj * PD + tid);
+    __syncthreads();
+    eval_normal_eq<DOF, true>(pts, a.N, sh.pose, cam, delta, a.p.huber_eps, sh.red, sh.ev);
+    if (tid == 0) gn_plus_step_and_v<DOF>(sh.ev, sh.pose, g.gplus + (size_t)obj * PD, a.p.eps, sh.step, sh.step + DOF);
+    __syncthreads();
+    float acc[CAM_GRADS];
+#pragma unroll
+    for (int k = 0; k < CAM_GRADS; ++k) acc[k] = 0.f;
+    gn_plus_camera_points<DOF, NT>(pts, a.N, sh.pose, sh.step, cam, delta, a.p.huber_eps, acc);
+    block_sum<CAM_GRADS>(acc, sh.red, 0);
+    if (tid == 0) store_camera_grad(g.gcam, g.glb, g.gub, obj, acc);
+}
+
+// gn_plus_camera_backward_kernel for objects too large for one SM, on gn_plus_backward_split_kernel's clusters and head
+// layout: every rank reduces the normal equations of its own range, the ranks' partials are added in rank order on every
+// rank (all form the same step and v), each rank reduces the 13 camera partials of its own points, and after one more
+// cluster barrier rank 0 adds them in rank order and stores; a final barrier keeps every CTA resident until then.
+template <int DOF> struct GnCamSplitHead {
+    float red[GNBW_SPLIT_T];            // eval_normal_eq / block_sum scratch
+    float part[32];                     // exchange slot 1: this rank's normal equations (NV floats)
+    float cpart[16];                    // exchange slot 2: this rank's 13 camera partials
+    float ev[32];                       // the normal equations of the whole object
+    float pose[8];
+    float step[2 * DOF];                // step, v
+};
+static_assert(sizeof(GnCamSplitHead<6>) <= 2 * COST_SPLIT_TILE * sizeof(float), "the head must fit the partial-cost region");
+
+template <int DOF>
+__global__ void __launch_bounds__(GNBW_SPLIT_T, 1) gn_plus_camera_backward_split_kernel(const GnCamBwArgs g,
+                                                                                       const int ctas) {
+    constexpr int T = GNBW_SPLIT_T;
+    const KArgs& a = g.k;
+    EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
+    float* dyn = reinterpret_cast<float*>(smem_raw);
+    constexpr int PD = Dim<DOF>::POSE, NV = Dim<DOF>::NV;
+    const int share = split_share(a.N, ctas);
+    const CostSplitPlan pl = plan_cost_split(share);
+    GnCamSplitHead<DOF>& sh = *reinterpret_cast<GnCamSplitHead<DOF>*>(dyn + pl.xbuf);
+    const int rank = cluster_rank(), obj = blockIdx.x / ctas, tid = threadIdx.x;
+    const int p0 = min(a.N, rank * share), p1 = min(a.N, p0 + share), cnt = p1 - p0;
+    float* pts = dyn + pl.pts;
+    Loader ld(a, reinterpret_cast<uint64_t*>(smem_raw), dyn + pl.stage);
+    ld.load_range<T>(obj, pts, p0, p1);
+    const Cam cam = load_cam(a, obj);
+    const float delta = __ldg(a.delta + obj);
+    if (tid < PD) sh.pose[tid] = __ldg(a.poses + (size_t)obj * PD + tid);
+    __syncthreads();
+    // each exchange slot is written once, before the cluster barrier after which its peers read it
+    eval_normal_eq<DOF, true, T>(pts, cnt, sh.pose, cam, delta, a.p.huber_eps, sh.red, sh.part);
+    cluster_sync();
+    if (tid < NV) sh.ev[tid] = sum_ranks(sh.part + tid, ctas);
+    __syncthreads();
+    if (tid == 0) gn_plus_step_and_v<DOF>(sh.ev, sh.pose, g.gplus + (size_t)obj * PD, a.p.eps, sh.step, sh.step + DOF);
+    __syncthreads();
+    float acc[CAM_GRADS];
+#pragma unroll
+    for (int k = 0; k < CAM_GRADS; ++k) acc[k] = 0.f;
+    gn_plus_camera_points<DOF, T>(pts, cnt, sh.pose, sh.step, cam, delta, a.p.huber_eps, acc);
+    block_sum<CAM_GRADS, T>(acc, sh.red, 0);
+    if (tid == 0) {
+#pragma unroll
+        for (int k = 0; k < CAM_GRADS; ++k) sh.cpart[k] = acc[k];
+    }
+    cluster_sync();
+#ifdef EPNP_SPLIT_AUDIT
+    for (int k = tid; k < NV + 2 * DOF; k += T) {        // H, g, cost, step and v: rank 0's bits on every rank
+        const float* x = k < NV ? sh.ev + k : sh.step + (k - NV);
+        if (__float_as_uint(dsmem_ld(x, 0)) != __float_as_uint(*x)) SPLIT_AUDIT_MISMATCH();
+    }
+#endif
+    if (rank == 0 && tid == 0) {
+        float v[CAM_GRADS];
+#pragma unroll
+        for (int k = 0; k < CAM_GRADS; ++k) v[k] = sum_ranks(sh.cpart + k, ctas);
+        const int stored = store_camera_grad(g.gcam, g.glb, g.gub, obj, v);
+        SPLIT_AUDIT_STORES(stored);
+        (void)stored;
+    }
+    cluster_sync();                                     // no CTA leaves while rank 0 may still read its slot
+}
+
 // AdaptiveHuberPnPCost.set_param: delta = mean(w2d) * sqrt(var_x + var_y) * relative_delta
 __global__ void __launch_bounds__(NT) adaptive_delta_kernel(const float* x2d, const float* w2d, float rel,
                                                           float* delta, int N) {
@@ -1727,6 +2059,8 @@ inline KArgs& kargs_of(KArgs& a) { return a; }
 inline KArgs& kargs_of(SeededKArgs& s) { return s.k; }
 inline int prepare_launch(GnBwArgs& g) { return prepare_launch(g.k); }
 inline int prepare_launch(PoseBwArgs& g) { return prepare_launch(g.k); }
+inline int prepare_launch(CamBwArgs& g) { return prepare_launch(g.k); }
+inline int prepare_launch(GnCamBwArgs& g) { return prepare_launch(g.k); }
 inline int prepare_launch(SeededKArgs& s) { return prepare_launch(s.k); }
 inline int prepare_launch(EpnpInitArgs&) { return EPNP_OK; }
 #if defined(EPNP_SIMT_EMUL) && !defined(SIMT_EMUL_HAS_CLUSTERS)
@@ -2111,6 +2445,64 @@ int epnp_gn_plus_backward_split_f32(const float* x3d, const float* x2d, const fl
     });
 }
 
+// The outputs of the camera backward entry points: at least one, and a bound's gradient only with bounds.
+static int camera_outputs_ok(const float* lb, const float* grad_cam, const float* grad_lb, const float* grad_ub) {
+    if (!grad_cam && !grad_lb && !grad_ub) return EPNP_ERR_BAD_ARG;
+    return ((grad_lb || grad_ub) && !lb) ? EPNP_ERR_BAD_ARG : EPNP_OK;
+}
+
+// The checked arguments of epnp_gn_plus_camera_backward_f32 and its split form, or the refusal.
+static int gn_cam_bw_args(GnCamBwArgs& g, const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                          const float* lb, const float* ub, const float* delta, const float* pose,
+                          const float* grad_pose_plus, float* grad_cam, float* grad_lb, float* grad_ub, int B, int N,
+                          int dof, float z_min, float eps, float huber_eps) {
+    KArgs& a = g.k;
+    a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
+    a.poses = pose;
+    epnp_default_params(&a.p, dof);
+    a.p.z_min = z_min; a.p.eps = eps; a.p.huber_eps = huber_eps;
+    g.gplus = grad_pose_plus; g.gcam = grad_cam; g.glb = grad_lb; g.gub = grad_ub;
+    const int rc = check_common(a);
+    if (rc != EPNP_OK) return rc;
+    if (!pose || !grad_pose_plus) return EPNP_ERR_BAD_ARG;
+    return camera_outputs_ok(lb, grad_cam, grad_lb, grad_ub);
+}
+
+int epnp_gn_plus_camera_backward_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                     const float* lb, const float* ub, const float* delta, const float* pose,
+                                     const float* grad_pose_plus, float* grad_cam, float* grad_lb, float* grad_ub,
+                                     int B, int N, int dof, float z_min, float eps, float huber_eps, void* stream) {
+    GnCamBwArgs g{};
+    const int rc = gn_cam_bw_args(g, x3d, x2d, w2d, cam_mats, lb, ub, delta, pose, grad_pose_plus, grad_cam, grad_lb,
+                                  grad_ub, B, N, dof, z_min, eps, huber_eps);
+    if (rc != EPNP_OK || B == 0) return rc;
+    return by_dof(dof, [&](auto D) {
+        const int smem_bytes = plan_obj<D>(N).total_bytes;
+        const int rc = prepare_resident(g.k, smem_bytes);
+        if (rc != EPNP_OK) return rc;
+        return launch_plain(gn_plus_camera_backward_kernel<D>, B, NT, smem_bytes, SmemAttr::size, (cudaStream_t)stream,
+                            g);
+    });
+}
+
+int epnp_gn_plus_camera_backward_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                           const float* lb, const float* ub, const float* delta, const float* pose,
+                                           const float* grad_pose_plus, float* grad_cam, float* grad_lb,
+                                           float* grad_ub, int B, int N, int dof, float z_min, float eps,
+                                           float huber_eps, int cluster_ctas, void* stream) {
+    GnCamBwArgs g{};
+    const int rc = gn_cam_bw_args(g, x3d, x2d, w2d, cam_mats, lb, ub, delta, pose, grad_pose_plus, grad_cam, grad_lb,
+                                  grad_ub, B, N, dof, z_min, eps, huber_eps);
+    if (rc != EPNP_OK) return rc;
+    const int ctas = split_ctas_for(dof, N, 0, 0, cluster_ctas);
+    if (ctas < 0) return ctas;
+    const int smem_bytes = split_smem_bytes(dof, N, ctas, 0, 0);
+    return by_dof(dof, [&](auto D) {
+        return launch_cluster<GNBW_SPLIT_T>(gn_plus_camera_backward_split_kernel<D>, g, B, smem_bytes, ctas,
+                                            (cudaStream_t)stream);
+    });
+}
+
 int epnp_rslm_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
                   const float* lb, const float* ub, const float* delta, const int* inds, const float* start,
                   float* pose_best, float* cost_best, float* pose_all, float* cost_all,
@@ -2441,6 +2833,62 @@ int epnp_cost_pose_backward_split_f32(const float* x3d, const float* x2d, const 
     const int smem_bytes = split_smem_bytes(dof, N, ctas, 0, 0);
     return by_dof(dof, [&](auto D) {
         return launch_cluster<COST_SPLIT_TILE>(cost_pose_backward_split_kernel<D>, g, B, smem_bytes, ctas,
+                                               (cudaStream_t)stream);
+    });
+}
+
+// The checked arguments of epnp_cost_camera_backward_f32 and its split form, or the refusal.
+static int cam_bw_args(CamBwArgs& g, const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                       const float* lb, const float* ub, const float* delta, const float* poses_a, const float* grad_a,
+                       int PA, const float* poses_b, const float* grad_b, int PB, float* grad_cam, float* grad_lb,
+                       float* grad_ub, int B, int N, int dof, float z_min) {
+    KArgs& a = g.k;
+    a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
+    epnp_default_params(&a.p, dof);
+    a.p.z_min = z_min;
+    g.poses_a = poses_a; g.grad_a = grad_a; g.poses_b = poses_b; g.grad_b = grad_b; g.PA = PA; g.PB = PB;
+    g.gcam = grad_cam; g.glb = grad_lb; g.gub = grad_ub;
+    const int rc = check_common(a);
+    if (rc != EPNP_OK) return rc;
+    if (PA < 0 || PB < 0 || (PA > 0 && (!poses_a || !grad_a)) || (PB > 0 && (!poses_b || !grad_b)))
+        return EPNP_ERR_BAD_ARG;
+    return camera_outputs_ok(lb, grad_cam, grad_lb, grad_ub);
+}
+
+int epnp_cost_camera_backward_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                  const float* lb, const float* ub, const float* delta,
+                                  const float* poses_a, const float* grad_a, int PA,
+                                  const float* poses_b, const float* grad_b, int PB,
+                                  float* grad_cam, float* grad_lb, float* grad_ub,
+                                  int B, int N, int dof, float z_min, void* stream) {
+    CamBwArgs g{};
+    const int rc = cam_bw_args(g, x3d, x2d, w2d, cam_mats, lb, ub, delta, poses_a, grad_a, PA, poses_b, grad_b, PB,
+                               grad_cam, grad_lb, grad_ub, B, N, dof, z_min);
+    if (rc != EPNP_OK || B == 0) return rc;
+    return by_dof(dof, [&](auto D) {
+        const int smem_bytes = plan_obj<D>(N).total_bytes;
+        const int rc = prepare_resident(g.k, smem_bytes);
+        if (rc != EPNP_OK) return rc;
+        return launch_plain(cost_camera_backward_kernel<D>, B, NT, smem_bytes, SmemAttr::size_and_carveout,
+                            (cudaStream_t)stream, g);
+    });
+}
+
+int epnp_cost_camera_backward_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                        const float* lb, const float* ub, const float* delta,
+                                        const float* poses_a, const float* grad_a, int PA,
+                                        const float* poses_b, const float* grad_b, int PB,
+                                        float* grad_cam, float* grad_lb, float* grad_ub,
+                                        int B, int N, int dof, float z_min, int cluster_ctas, void* stream) {
+    CamBwArgs g{};
+    const int rc = cam_bw_args(g, x3d, x2d, w2d, cam_mats, lb, ub, delta, poses_a, grad_a, PA, poses_b, grad_b, PB,
+                               grad_cam, grad_lb, grad_ub, B, N, dof, z_min);
+    if (rc != EPNP_OK) return rc;
+    const int ctas = split_ctas_for(dof, N, 0, 0, cluster_ctas);
+    if (ctas < 0) return ctas;
+    const int smem_bytes = split_smem_bytes(dof, N, ctas, 0, 0);
+    return by_dof(dof, [&](auto D) {
+        return launch_cluster<COST_SPLIT_TILE>(cost_camera_backward_split_kernel<D>, g, B, smem_bytes, ctas,
                                                (cudaStream_t)stream);
     });
 }

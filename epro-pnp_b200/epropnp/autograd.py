@@ -6,16 +6,19 @@
                                     (samples and proposals are built under no_grad, epropnp.py:139-140,172-179)
                                     -> same native kernel, upstream gradient -dL/dlogw
     evaluate_pnp(out_cost=True)     the same two kernels (correspondences / delta, poses)
+    cost_init, logweights, evaluate_pnp   d/d(cam_mats, lb, ub)   native kernel (epnp_cost_camera_backward_f32)
     pose_opt_plus                   one un-damped Gauss-Newton step at the (detached) solution; differentiated
                                     by torch autograd through `PerspectiveCamera.project` + `HuberPnPCost.compute`
                                     (a single evaluation, levenberg_marquardt.py:243-253 -- not the iterated path),
-                                    or, with EPNP_NATIVE_GN_STEP=1, by the native kernel epnp_gn_plus_backward_f32
+                                    or, with EPNP_NATIVE_GN_STEP=1, by the native kernels epnp_gn_plus_backward_f32
+                                    and, for cam_mats / lb / ub, epnp_gn_plus_camera_backward_f32
 
 Objects with more points than one SM holds (N above epnp_max_points: about 5,400 for the AMIS loop at M = 512, 7,000
 for the cost, the pose_opt_plus backward and the EPnP initialiser) take the cluster-split kernels (fused_forward,
 stacked_cost, gn_plus_backward, epnp_init), up to epnp_max_points_split; at or below those limits nothing changes.  The
 Monte-Carlo cost backward kernel streams the points, so it serves both; the pose_opt_plus forward (the LM kernel) streams
-them too; the pose backward has a split form of its own (native.cost_pose_backward chooses).  RSLM init takes its split
+them too; the pose and camera backwards have split forms of their own (native.cost_pose_backward,
+native.cost_camera_backward and native.gn_plus_camera_backward choose).  RSLM init takes its split
 form (rslm_solve) only when the solver was built with RSLMSolver(cluster_split=True), up to min(epnp_max_points_split,
 the native draw's own limit: 53,504 points at n = 16); by default it refuses objects above the resident limit.
 
@@ -105,6 +108,7 @@ class _MonteCarloForward(torch.autograd.Function):
         ctx.needs = (x3d.requires_grad, x2d.requires_grad, w2d.requires_grad,
                      torch.is_tensor(delta) and delta.requires_grad)
         ctx.pose_like = cost_init_pose if cost_init_pose is not None and cost_init_pose.requires_grad else None
+        ctx.cam_like = _camera_like(prob, cam_mats, lb, ub)
         cost = out["cost"] if want_cost else x3d.new_zeros(0)
         ci = cost_init if cost_init is not None else x3d.new_zeros(0)
         dt = x3d.dtype
@@ -131,7 +135,9 @@ class _MonteCarloForward(torch.autograd.Function):
         gpose = None
         if ctx.pose_like is not None and poses_b is not None:
             gpose = _pose_grad_to(ctx.pose_like, native.cost_pose_backward(prob, ctx.dof, ctx.z_min, poses_b, grad_b)[:, 0])
-        return gx3d, gx2d, gw2d, gdel, None, None, None, None, gpose, None, None, None, None, None
+        gcam, glb, gub = _camera_grads(ctx.cam_like, lambda want: native.cost_camera_backward(
+            prob, ctx.dof, ctx.z_min, ctx.samples, -g_logw.contiguous(), poses_b, grad_b, want=want))
+        return gx3d, gx2d, gw2d, gdel, gcam, glb, gub, None, gpose, None, None, None, None, None
 
 
 class _CostOnly(torch.autograd.Function):
@@ -148,6 +154,7 @@ class _CostOnly(torch.autograd.Function):
         ctx.needs = (x3d.requires_grad, x2d.requires_grad, w2d.requires_grad,
                      torch.is_tensor(delta) and delta.requires_grad)
         ctx.pose_like = poses if poses.requires_grad else None
+        ctx.cam_like = _camera_like(prob, cam_mats, lb, ub)
         return cost.to(x3d.dtype)
 
     @staticmethod
@@ -161,12 +168,40 @@ class _CostOnly(torch.autograd.Function):
         if ctx.pose_like is not None:
             gpose = _pose_grad_to(ctx.pose_like,
                                   native.cost_pose_backward(ctx.prob, ctx.dof, ctx.z_min, ctx.poses, g_cost).transpose(0, 1))
-        return gx3d, gx2d, gw2d, gdel, None, None, None, gpose, None, None
+        gcam, glb, gub = _camera_grads(ctx.cam_like, lambda want: native.cost_camera_backward(
+            ctx.prob, ctx.dof, ctx.z_min, ctx.poses, g_cost, want=want))
+        return gx3d, gx2d, gw2d, gdel, gcam, glb, gub, gpose, None, None
 
 
 def _pose_grad_to(like, g):
     """Native pose gradient -> dtype and shape of the pose tensor it belongs to."""
     return g.to(like.dtype).reshape(like.shape)
+
+
+def _camera_like(prob, cam_mats, lb, ub):
+    """The camera inputs that require grad (cam_mats, lb, ub; None elsewhere).  Python-float bounds get no gradient, and
+    neither does a bound while the other is missing: the projection is then not clamped."""
+    grad = lambda t: torch.is_tensor(t) and t.requires_grad
+    bounded = prob.lb is not None
+    return (cam_mats if grad(cam_mats) else None, lb if bounded and grad(lb) else None,
+            ub if bounded and grad(ub) else None)
+
+
+def _camera_grads(like, run):
+    """run(want) -> native (B, 3, 3) / (B, 2) / (B, 2) camera gradients, each reduced to the dtype and shape of the
+    tensor the caller passed: a (3, 3) camera or a (2,) bound shared by every object receives the sum over objects (an
+    expanded one receives them per object; autograd sums them through the expand)."""
+    want = tuple(t is not None for t in like)
+    if not any(want):
+        return None, None, None
+    out = []
+    for t, g in zip(like, run(want)):
+        if t is None:
+            out.append(None)
+            continue
+        g = g.to(t.dtype)
+        out.append(g.sum_to_size(t.shape) if t.dim() else g.sum())
+    return tuple(out)
 
 
 def evaluate_cost_autograd(x3d, x2d, w2d, pose, camera, cost_fun):
@@ -200,14 +235,19 @@ class _PosePlus(torch.autograd.Function):
         ctx.in_like = (x3d, x2d, w2d, delta if torch.is_tensor(delta) else None)
         ctx.needs = (x3d.requires_grad, x2d.requires_grad, w2d.requires_grad,
                      torch.is_tensor(delta) and delta.requires_grad)
+        ctx.cam_like = _camera_like(prob, cam_mats, lb, ub)
         return plus.to(x3d.dtype)
 
     @staticmethod
     def backward(ctx, grad_plus):
         z_min, eps, huber_eps = ctx.consts
-        grads = gn_plus_backward(ctx.prob, ctx.pose, grad_plus, ctx.dof, z_min, eps, huber_eps, ctx.needs)
+        grads = (None,) * 4
+        if any(ctx.needs):
+            grads = gn_plus_backward(ctx.prob, ctx.pose, grad_plus, ctx.dof, z_min, eps, huber_eps, ctx.needs)
         g3, g2, gw, gd = _grads_to(ctx.in_like, grads)
-        return g3, g2, gw, gd, None, None, None, None, None, None
+        gcam, glb, gub = _camera_grads(ctx.cam_like, lambda want: native.gn_plus_camera_backward(
+            ctx.prob, ctx.pose, grad_plus, ctx.dof, z_min, eps, huber_eps, want=want))
+        return g3, g2, gw, gd, gcam, glb, gub, None, None, None
 
 
 def native_gn_step_enabled():

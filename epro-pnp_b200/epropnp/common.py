@@ -42,6 +42,11 @@ def _needs_grad(*tensors):
     return torch.is_grad_enabled() and any(torch.is_tensor(t) and t.requires_grad for t in tensors)
 
 
+def _camera_requires_grad(camera):
+    """cam_mats or a tensor bound of `camera` requires grad."""
+    return any(torch.is_tensor(t) and t.requires_grad for t in (camera.cam_mats, camera.lb, camera.ub))
+
+
 def _store(out, value):
     """Reference semantics of the out_* arguments: a tensor is filled in place and returned."""
     if torch.is_tensor(out):
@@ -61,12 +66,14 @@ def evaluate_pnp(x3d, x2d, w2d, pose, camera, cost_fun,
     clip_jac = kwargs.pop("clip_jac", True)
     if kwargs:
         raise TypeError(f"unexpected arguments {sorted(kwargs)}")
-    if _needs_grad(x3d, x2d, w2d, pose, getattr(cost_fun, "delta", None)):
+    camera_grad = _needs_grad(camera.cam_mats, camera.lb, camera.ub)
+    if _needs_grad(x3d, x2d, w2d, pose, getattr(cost_fun, "delta", None)) or camera_grad:
         native_pose_grad = x3d.is_cuda and x3d.dtype == pose.dtype == torch.float32
-        if out_jacobian is not False or out_residual is not False or (pose.requires_grad and not native_pose_grad):
+        if out_jacobian is not False or out_residual is not False or \
+                ((pose.requires_grad or camera_grad) and not native_pose_grad):
             # differentiable residual / Jacobian (LMSolver.gn_step under autograd, reference common.py:67-100), or
-            # gradients w.r.t. the pose of CPU / float64 tensors: the torch composite of the same two methods the
-            # reference calls
+            # gradients w.r.t. the pose or the camera of CPU / float64 tensors: the torch composite of the same two
+            # methods the reference calls
             x2d_proj, jac_cam = camera.project(x3d, pose, out_jac=(out_jacobian is not False), clip_jac=clip_jac)
             residual, cost, jac = cost_fun.compute(x2d_proj, x2d, w2d, jac_cam=jac_cam, out_residual=(out_residual is not False),
                                                    out_cost=(out_cost is not False), out_jacobian=(out_jacobian is not False))

@@ -27,7 +27,7 @@ import torch
 
 from epropnp_b200 import native
 from .builder import PNP, build_pnp
-from .common import evaluate_pnp, philox_seed, pnp_normalize, pnp_denormalize
+from .common import _camera_requires_grad, evaluate_pnp, philox_seed, pnp_normalize, pnp_denormalize
 from .distributions import AngularCentralGaussian, MultivariateStudentT, VonMisesUniformMix
 
 # The steps of the AMIS loop the reference exposes as methods of the layer (epropnp.py:65-82).  Here the loop runs inside
@@ -142,7 +142,8 @@ class EProPnPBase(torch.nn.Module, metaclass=ABCMeta):
         delta = cost_fun.delta
         differentiable = torch.is_grad_enabled() and (any(t.requires_grad for t in (x3d, x2d, w2d)) or
                                                       (torch.is_tensor(delta) and delta.requires_grad) or
-                                                      (pose_init is not None and pose_init.requires_grad))
+                                                      (pose_init is not None and pose_init.requires_grad) or
+                                                      _camera_requires_grad(camera))
         if self.normalize:
             transform, x3d, pose_init = pnp_normalize(x3d, pose_init, detach_transformation=True)
         assert x3d.dim() == x2d.dim() == w2d.dim() == 3

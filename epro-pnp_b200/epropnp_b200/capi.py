@@ -72,6 +72,11 @@ _SIGNATURES = {
     "epnp_cost_backward_f32": (ctypes.c_int, [_P] * 7 + [_P, _P, _I, _P, _P, _I] + [_P] * 4 + [_I, _I, _I, _F, _P]),
     "epnp_cost_pose_backward_f32": (ctypes.c_int, [_P] * 10 + [_I, _I, _I, _I, _F, _P]),
     "epnp_cost_pose_backward_split_f32": (ctypes.c_int, [_P] * 10 + [_I, _I, _I, _I, _F, _I, _P]),
+    "epnp_cost_camera_backward_f32": (ctypes.c_int, [_P] * 7 + [_P, _P, _I, _P, _P, _I] + [_P] * 3 + [_I, _I, _I, _F, _P]),
+    "epnp_cost_camera_backward_split_f32": (ctypes.c_int, [_P] * 7 + [_P, _P, _I, _P, _P, _I] + [_P] * 3
+                                            + [_I, _I, _I, _F, _I, _P]),
+    "epnp_gn_plus_camera_backward_f32": (ctypes.c_int, [_P] * 12 + [_I, _I, _I, _F, _F, _F, _P]),
+    "epnp_gn_plus_camera_backward_split_f32": (ctypes.c_int, [_P] * 12 + [_I, _I, _I, _F, _F, _F, _I, _P]),
     "epnp_mc_epilogue_f32": (ctypes.c_int, [_P] * 8 + [_I, _I, _I, _P]),
     "epnp_mc_lse_backward_f32": (ctypes.c_int, [_P] * 4 + [_I, _I, _P]),
     "epnp_fused_workspace_bytes": (ctypes.c_size_t, [_I, _I, ctypes.POINTER(EpnpParams)]),

@@ -496,6 +496,69 @@ def cost_pose_backward(prob: Problem, dof, z_min, poses, grad, cluster_ctas=0):
     return out
 
 
+def _camera_outputs(prob, want):
+    """The (B, 3, 3) / (B, 2) / (B, 2) outputs of a camera backward that `want` asks for (None elsewhere)."""
+    if not any(want):
+        raise ValueError("want: ask for at least one of the cam_mats, lb and ub gradients")
+    if (want[1] or want[2]) and prob.lb is None:
+        raise ValueError("the gradient of a bound needs the problem's bounds")
+    B = prob.B
+    return (prob.empty(B, 3, 3) if want[0] else None, prob.empty(B, 2) if want[1] else None,
+            prob.empty(B, 2) if want[2] else None)
+
+
+def cost_camera_backward(prob: Problem, dof, z_min, poses_a, grad_a, poses_b=None, grad_b=None,
+                         want=(True, True, True), cluster_ctas=0):
+    """sum_p grad[b, p] * d cost(pose p) / d (cam_mats[b], lb[b], ub[b]) for object-major pose sets a: (B, PA, D) /
+    (B, PA) and optional b: (B, PB, D) / (B, PB) -> (grad_cam (B, 3, 3), grad_lb (B, 2), grad_ub (B, 2)), None where
+    `want` is False (epnp_cost_camera_backward_f32; above max_points(dof) its cluster-split form, `cluster_ctas` as
+    evaluate_cost_split)."""
+    D = 7 if dof == 6 else 4
+    PA = poses_a.shape[1]
+    _check_pose(poses_a, (prob.B, PA), D, "poses_a")
+    poses_a, grad_a = _f32c(poses_a), _f32c(grad_a)
+    PB = 0
+    if poses_b is not None:
+        PB = poses_b.shape[1]
+        _check_pose(poses_b, (prob.B, PB), D, "poses_b")
+        poses_b, grad_b = _f32c(poses_b), _f32c(grad_b)
+    for g, P, what in ((grad_a, PA, "grad_a"), (grad_b, PB, "grad_b")):
+        if g is not None and tuple(g.shape) != (prob.B, P):
+            raise ValueError(f"{what} must be {(prob.B, P)}; got {tuple(g.shape)}")
+    gcam, glb, gub = _camera_outputs(prob, want)
+    args = (*prob.common_ptrs(), ptr(poses_a), ptr(grad_a), PA, ptr(poses_b), ptr(grad_b), PB, ptr(gcam), ptr(glb),
+            ptr(gub), prob.B, prob.N, int(dof), ctypes.c_float(z_min))
+    with torch.cuda.device(prob.device):
+        if prob.N > max_points(dof):
+            check(lib().epnp_cost_camera_backward_split_f32(*args, int(cluster_ctas), stream_ptr(prob.device)),
+                  "epnp_cost_camera_backward_split_f32")
+        else:
+            check(lib().epnp_cost_camera_backward_f32(*args, stream_ptr(prob.device)), "epnp_cost_camera_backward_f32")
+    return gcam, glb, gub
+
+
+def gn_plus_camera_backward(prob: Problem, pose, grad_pose_plus, dof, z_min, eps, huber_eps, want=(True, True, True),
+                            cluster_ctas=0):
+    """dL/d(cam_mats, lb, ub) of pose_opt_plus = pose (+) gn_step(pose) -> (grad_cam (B, 3, 3), grad_lb (B, 2),
+    grad_ub (B, 2)), None where `want` is False (epnp_gn_plus_camera_backward_f32; above max_points(dof) its
+    cluster-split form, `cluster_ctas` as gn_plus_backward_split)."""
+    D = 7 if dof == 6 else 4
+    _check_pose(pose, (prob.B,), D, "pose")
+    _check_pose(grad_pose_plus, (prob.B,), D, "grad_pose_plus")
+    pose, gp = _f32c(pose), _f32c(grad_pose_plus)
+    gcam, glb, gub = _camera_outputs(prob, want)
+    args = (*prob.common_ptrs(), ptr(pose), ptr(gp), ptr(gcam), ptr(glb), ptr(gub), prob.B, prob.N, int(dof),
+            ctypes.c_float(z_min), ctypes.c_float(eps), ctypes.c_float(huber_eps))
+    with torch.cuda.device(prob.device):
+        if prob.N > max_points(dof):
+            check(lib().epnp_gn_plus_camera_backward_split_f32(*args, int(cluster_ctas), stream_ptr(prob.device)),
+                  "epnp_gn_plus_camera_backward_split_f32")
+        else:
+            check(lib().epnp_gn_plus_camera_backward_f32(*args, stream_ptr(prob.device)),
+                  "epnp_gn_plus_camera_backward_f32")
+    return gcam, glb, gub
+
+
 def fused_workspace_bytes(B, N, params):
     return int(lib().epnp_fused_workspace_bytes(B, N, ctypes.byref(params)))
 
@@ -588,5 +651,6 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
     return out
 
 
-__all__ = ["Problem", "adaptive_delta", "cost_backward", "evaluate_cost", "evaluate_cost_split", "evaluate_full", "lm_solve",
+__all__ = ["Problem", "adaptive_delta", "cost_backward", "cost_camera_backward", "gn_plus_camera_backward",
+           "evaluate_cost", "evaluate_cost_split", "evaluate_full", "lm_solve",
            "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "rslm", "rslm_split", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

@@ -379,6 +379,51 @@ int epnp_cost_pose_backward_split_f32(const float* x3d, const float* x2d, const 
                                       const float* grad, float* grad_pose, int P, int B, int N, int dof, float z_min,
                                       int cluster_ctas, void* stream);
 
+/* Backward of the same costs with respect to the CAMERA (the reference differentiates cam_mats through project_a /
+ * project_b and tensor lb / ub through torch.max / torch.min: camera.py:10-30,81-93):
+ *   grad_cam[b] = sum_p grad[b, p] * d cost(poses[b, p]) / d cam_mats[b]                          (B, 3, 3)
+ *   grad_lb[b], grad_ub[b] = the same with respect to lb[b], ub[b]                                   (B, 2)
+ * over the pose sets of epnp_cost_backward_f32 (a: (B, PA, D) / (B, PA); b [opt]: (B, PB, D) / (B, PB)).  A coordinate
+ * clamped at a bound passes its gradient to that bound; a depth clamped at z_min passes none.  Outputs are optional, but
+ * at least one must be given, and grad_lb / grad_ub only with bounds (EPNP_ERR_BAD_ARG otherwise).  One CTA per object
+ * and one fixed-order block reduction, no atomics: an object's result depends on nothing else in the batch.  N above
+ * epnp_max_points(dof, 0, 0): EPNP_ERR_TOO_MANY_POINTS.  B = 0 writes nothing; PA = PB = 0 writes zeros.        */
+int epnp_cost_camera_backward_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                  const float* lb, const float* ub, const float* delta,
+                                  const float* poses_a, const float* grad_a, int PA,
+                                  const float* poses_b, const float* grad_b, int PB,
+                                  float* grad_cam, float* grad_lb, float* grad_ub,
+                                  int B, int N, int dof, float z_min, void* stream);
+
+/* epnp_cost_camera_backward_f32 for objects of up to epnp_max_points_split(dof, 0, 0) points, on the clusters of
+ * epnp_evaluate_cost_split_f32: each rank sweeps its own range of the points for every pose and reduces to 13 floats,
+ * rank 0 adds the ranks' in rank order and stores.  cluster_ctas as there; the result depends on C and never on B.
+ * EPNP_ERR_UNSUPPORTED when the device cannot run one cluster of that size; nothing is launched then.           */
+int epnp_cost_camera_backward_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                        const float* lb, const float* ub, const float* delta,
+                                        const float* poses_a, const float* grad_a, int PA,
+                                        const float* poses_b, const float* grad_b, int PB,
+                                        float* grad_cam, float* grad_lb, float* grad_ub,
+                                        int B, int N, int dof, float z_min, int cluster_ctas, void* stream);
+
+/* The camera gradient of pose_opt_plus = pose (+) gn_step(pose) (epnp_gn_plus_backward_f32's function, differentiated
+ * with respect to cam_mats and the bounds instead of the correspondences): grad_cam (B, 3, 3), grad_lb / grad_ub (B, 2),
+ * optional with the rules of epnp_cost_camera_backward_f32.  K enters the projection and the Jacobian; the clip mask is
+ * held constant, as in the reference's autograd.  A separate launch: epnp_gn_plus_backward_f32 is unchanged.    */
+int epnp_gn_plus_camera_backward_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                     const float* lb, const float* ub, const float* delta, const float* pose,
+                                     const float* grad_pose_plus, float* grad_cam, float* grad_lb, float* grad_ub,
+                                     int B, int N, int dof, float z_min, float eps, float huber_eps, void* stream);
+
+/* epnp_gn_plus_camera_backward_f32 on the clusters of epnp_gn_plus_backward_split_f32 (cluster_ctas and refusals as
+ * there): every rank forms the same step and v, reduces the camera partials of its own points, and rank 0 adds the
+ * ranks' in rank order.  The result depends on C and never on B.                                                 */
+int epnp_gn_plus_camera_backward_split_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                                           const float* lb, const float* ub, const float* delta, const float* pose,
+                                           const float* grad_pose_plus, float* grad_cam, float* grad_lb,
+                                           float* grad_ub, int B, int N, int dof, float z_min, float eps,
+                                           float huber_eps, int cluster_ctas, void* stream);
+
 /* Epilogue on the AMIS outputs -- the step AFTER the path in every caller of monte_carlo_forward (one pass over the
  * object-major log-weights instead of a dozen torch ops on (M, B) views):
  *   lse (B)        = logsumexp_m logw[b, m]      -- `loss_pred` of MonteCarloPoseLoss.forward

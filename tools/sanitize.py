@@ -69,9 +69,28 @@ for dof, N, B, bounded in ((6, 64, 5, False), (6, 130, 3, True), (6, 51, 4, Fals
         bounded = native.Problem(d["x3d"], d["x2d"], d["w2d"], d["cam_mats"], 0.0, 640.0, prob.delta)
         native.rslm_split(bounded, di, ds, native.default_params(dof, lm_iter=2), want_all=True, cluster_ctas=2)
         native.gn_plus_backward(prob, out["pose_opt"], torch.randn(B, D, device=dev), dof, 0.1, 1e-5, 1e-10)
+        gp = torch.randn(B, D, device=dev)
+        cam = [native.cost_camera_backward(bounded, dof, 0.1, out["pose_samples"], torch.randn(B, 128, device=dev),
+                                           d["pose_init"].reshape(B, 1, D), torch.randn(B, 1, device=dev)),
+               native.gn_plus_camera_backward(bounded, out["pose_opt"], gp, dof, 0.1, 1e-5, 1e-10)]
+        torch.cuda.synchronize()
+        check(f"{tag}: finite camera gradients", all(torch.isfinite(t).all() for g3 in cam for t in g3))
     torch.cuda.synchronize()
     check(f"dof={dof} N={N}: finite log-weights", torch.isfinite(out["logw"]).all())
     check(f"dof={dof} N={N}: finite gradients", all(torch.isfinite(t).all() for t in g))
+# objects beyond one SM: the cluster-split camera backwards (distributed shared memory, cluster barriers)
+for dof in (6, 4):
+    N, B, D = native.max_points(dof) + 1, 2, 7 if dof == 6 else 4
+    d = {k: v.to(dev) for k, v in make_problem(B, N, seed=5 + dof, dof=dof, outlier_frac=0.1).items()}
+    prob = native.Problem(d["x3d"], d["x2d"], d["w2d"], d["cam_mats"], d["x2d"].min(1).values + 5,
+                          d["x2d"].max(1).values - 5, native.adaptive_delta(d["x2d"], d["w2d"], 0.5))
+    poses = d["pose_init"][:, None].repeat(1, 3, 1)
+    cam = [native.cost_camera_backward(prob, dof, 0.1, poses, torch.randn(B, 3, device=dev), d["pose_init"][:, None],
+                                       torch.randn(B, 1, device=dev), cluster_ctas=ctas) for ctas in (2, 3)]
+    cam += [native.gn_plus_camera_backward(prob, d["pose_init"], torch.randn(B, D, device=dev), dof, 0.1, 1e-5, 1e-10,
+                                           cluster_ctas=2)]
+    torch.cuda.synchronize()
+    check(f"dof={dof} N={N}: finite split camera gradients", all(torch.isfinite(t).all() for g3 in cam for t in g3))
 # long point set: the 8-warp LM kernel and the 512-thread AMIS kernel
 pc = make_problem(2, 2052, seed=3)
 d = {k: v.to(dev) for k, v in pc.items()}
