@@ -10,6 +10,7 @@
 //                                    4 points per thread between block barriers (DESIGN.md section 4).
 //   cost_kernel, evaluate_full_kernel, rslm_draw_kernel, rslm_kernel, cost_backward_kernel, gn_plus_backward_kernel, adaptive_delta_kernel,
 //   mc_epilogue_kernel, mc_lse_backward_kernel      the steps either side of the path (CTA per object).
+//   evaluate_backward_kernel         the backward of evaluate_full_kernel's residual / Jacobian / cost (CTA per object, any N).
 //   cost_pose_backward_kernel, cost_pose_backward_split_kernel    the cost's gradient with respect to stacked poses: thread per
 //                                    pose over the resident points; the split form on cost_split_kernel's clusters.
 //   epnp_init_kernel (pnp_epnp.cuh)  EPnP initialiser with the confidence-quantile point selection, fp64, CTA per object.
@@ -1420,6 +1421,116 @@ __global__ void __launch_bounds__(GNBW_SPLIT_T, 1) gn_plus_camera_backward_split
         (void)stored;
     }
     cluster_sync();                                     // no CTA leaves while rank 0 may still read its slot
+}
+
+// ------------------------------------------------------------------------------------------------
+// Backward of evaluate_full_kernel's residual, Jacobian and cost at S stacked poses (S, B, D): the vector-Jacobian
+// product with any of the upstream gradients g_res (S, B, 2N), g_jac (S, B, 2N, DOF) and g_cost (S, B), differentiated
+// per (pose, point) by the three forms of point_residual_jac_backward (pnp_math.cuh).  One CTA per object, the points
+// streamed from global memory as evaluate_full_kernel reads them, so there is no point limit and no split form.
+//   1. thread <-> point, the poses in order inside the thread: the point's x3d / x2d / w2d gradients are summed over the
+//      poses in registers and stored once; delta's and the camera's partials are added over the thread's points and
+//      reduced by one fixed-order block_sum each.
+//   2. per pose, thread <-> point again with the pose form, and one fixed-order block_sum of the D components.
+// No atomics; every output element is written by one thread; an object's results depend on nothing else in the batch,
+// and on which gradients were requested only through which of the passes run.
+struct EvalBwArgs {
+    KArgs k;                                // correspondences, camera, bounds, delta, poses (S, B, D), p.z_min / huber_eps
+    const float *g_res, *g_jac, *g_cost;    // [opt] (S, B, 2N), (S, B, 2N, DOF), (S, B)
+    float *gx3d, *gx2d, *gw2d, *gdelta;     // [opt] (B, N, 3|2|2), (B)
+    float* gpose;                           // [opt] (S, B, D)
+    float *gcam, *glb, *gub;                // [opt] (B, 3, 3), (B, 2), (B, 2)
+    int S, clip;
+};
+
+// The upstream of (pose row `row` = s B + b, point n); gr / gj are left unset (and null returned) when not given.
+template <int DOF>
+__device__ __forceinline__ float eval_bw_upstream(const EvalBwArgs& g, size_t row, int n, float (&gr)[2],
+                                                  float (&gj)[2 * DOF], const float*& pr, const float*& pj) {
+    const size_t p = row * g.k.N + n;
+    pr = pj = nullptr;
+    if (g.g_res) { gr[0] = __ldg(g.g_res + 2 * p); gr[1] = __ldg(g.g_res + 2 * p + 1); pr = gr; }
+    if (g.g_jac) {
+#pragma unroll
+        for (int k = 0; k < 2 * DOF; ++k) gj[k] = __ldg(g.g_jac + p * 2 * DOF + k);
+        pj = gj;
+    }
+    return g.g_cost ? __ldg(g.g_cost + row) : 0.f;
+}
+
+template <int DOF>
+__global__ void __launch_bounds__(NT) evaluate_backward_kernel(const EvalBwArgs g) {
+    __shared__ float red[2 * NW * 32];
+    const KArgs& a = g.k;
+    constexpr int PD = Dim<DOF>::POSE;
+    const int obj = blockIdx.x, tid = threadIdx.x;
+    const Cam cam = load_cam(a, obj);
+    const float delta = __ldg(a.delta + obj), heps = a.p.huber_eps;
+    const bool clip = g.clip != 0;
+    const bool want_pts = g.gx3d || g.gx2d || g.gw2d || g.gdelta, want_cam = g.gcam || g.glb || g.gub;
+    if (want_pts || want_cam) {
+        float gd = 0.f, gk[CAM_GRADS];
+#pragma unroll
+        for (int k = 0; k < CAM_GRADS; ++k) gk[k] = 0.f;
+        for (int n = tid; n < a.N; n += NT) {
+            const size_t q = (size_t)obj * a.N + n;
+            const float X = __ldg(a.x3d + q * 3), Y = __ldg(a.x3d + q * 3 + 1), Z = __ldg(a.x3d + q * 3 + 2);
+            const float u = __ldg(a.x2d + q * 2), v = __ldg(a.x2d + q * 2 + 1);
+            const float wu = __ldg(a.w2d + q * 2), wv = __ldg(a.w2d + q * 2 + 1);
+            float gp[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+            for (int s = 0; s < g.S; ++s) {
+                const size_t row = (size_t)s * a.B + obj;
+                float pose[PD], R[9], gr[2], gj[2 * DOF];
+#pragma unroll
+                for (int k = 0; k < PD; ++k) pose[k] = __ldg(a.poses + row * PD + k);
+                pose_to_rot<DOF>(pose, R);
+                const float *pr, *pj;
+                const float gc = eval_bw_upstream<DOF>(g, row, n, gr, gj, pr, pj);
+                if (want_pts)
+                    point_residual_jac_backward<DOF>(R, pose, cam, delta, heps, clip, X, Y, Z, u, v, wu, wv, pr, pj, gc, gp);
+                if (want_cam)
+                    point_residual_jac_camera_backward<DOF>(R, pose, cam, delta, heps, clip, X, Y, Z, u, v, wu, wv, pr,
+                                                            pj, gc, gk);
+            }
+            if (g.gx3d) { g.gx3d[q * 3] = gp[0]; g.gx3d[q * 3 + 1] = gp[1]; g.gx3d[q * 3 + 2] = gp[2]; }
+            if (g.gx2d) { g.gx2d[q * 2] = gp[3]; g.gx2d[q * 2 + 1] = gp[4]; }
+            if (g.gw2d) { g.gw2d[q * 2] = gp[5]; g.gw2d[q * 2 + 1] = gp[6]; }
+            gd += gp[7];
+        }
+        if (want_pts) {
+            float v[1] = {gd};
+            block_sum<1>(v, red, 0);
+            if (tid == 0 && g.gdelta) g.gdelta[obj] = v[0];
+        }
+        if (want_cam) {
+            block_sum<CAM_GRADS>(gk, red, 1);
+            if (tid == 0) store_camera_grad(g.gcam, g.glb, g.gub, obj, gk);
+        }
+    }
+    if (!g.gpose) return;
+    __syncthreads();                                    // pass 1's reductions are read: the scratch may be rewritten
+    for (int s = 0; s < g.S; ++s) {
+        const size_t row = (size_t)s * a.B + obj;
+        float pose[PD], acc[PD];
+#pragma unroll
+        for (int k = 0; k < PD; ++k) { pose[k] = __ldg(a.poses + row * PD + k); acc[k] = 0.f; }
+        for (int n = tid; n < a.N; n += NT) {
+            const size_t q = (size_t)obj * a.N + n;
+            float gr[2], gj[2 * DOF];
+            const float *pr, *pj;
+            const float gc = eval_bw_upstream<DOF>(g, row, n, gr, gj, pr, pj);
+            point_residual_jac_pose_backward<DOF>(pose, cam, delta, heps, clip, __ldg(a.x3d + q * 3),
+                                                  __ldg(a.x3d + q * 3 + 1), __ldg(a.x3d + q * 3 + 2),
+                                                  __ldg(a.x2d + q * 2), __ldg(a.x2d + q * 2 + 1),
+                                                  __ldg(a.w2d + q * 2), __ldg(a.w2d + q * 2 + 1), pr, pj, gc, acc);
+        }
+        // alternate halves: a half is rewritten only after the next reduction's barrier, which follows every read of it
+        block_sum<PD>(acc, red, s & 1);
+        if (tid == 0) {
+#pragma unroll
+            for (int k = 0; k < PD; ++k) g.gpose[row * PD + k] = acc[k];
+        }
+    }
 }
 
 // AdaptiveHuberPnPCost.set_param: delta = mean(w2d) * sqrt(var_x + var_y) * relative_delta
@@ -2890,6 +3001,34 @@ int epnp_cost_camera_backward_split_f32(const float* x3d, const float* x2d, cons
     return by_dof(dof, [&](auto D) {
         return launch_cluster<COST_SPLIT_TILE>(cost_camera_backward_split_kernel<D>, g, B, smem_bytes, ctas,
                                                (cudaStream_t)stream);
+    });
+}
+
+int epnp_evaluate_backward_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                               const float* lb, const float* ub, const float* delta, const float* poses,
+                               const float* grad_residual, const float* grad_jac, const float* grad_cost,
+                               float* grad_x3d, float* grad_x2d, float* grad_w2d, float* grad_delta, float* grad_pose,
+                               float* grad_cam, float* grad_lb, float* grad_ub, int clip_jac, int S, int B, int N,
+                               int dof, float z_min, float huber_eps, void* stream) {
+    EvalBwArgs g{};
+    KArgs& a = g.k;
+    a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
+    a.poses = poses;
+    epnp_default_params(&a.p, dof);
+    a.p.z_min = z_min; a.p.huber_eps = huber_eps;
+    g.g_res = grad_residual; g.g_jac = grad_jac; g.g_cost = grad_cost;
+    g.gx3d = grad_x3d; g.gx2d = grad_x2d; g.gw2d = grad_w2d; g.gdelta = grad_delta; g.gpose = grad_pose;
+    g.gcam = grad_cam; g.glb = grad_lb; g.gub = grad_ub;
+    g.S = S; g.clip = clip_jac;
+    const int rc = check_common(a);
+    if (rc != EPNP_OK) return rc;
+    if (!poses || S < 0 || (!grad_residual && !grad_jac && !grad_cost)) return EPNP_ERR_BAD_ARG;
+    const bool other = grad_x3d || grad_x2d || grad_w2d || grad_delta || grad_pose;
+    if (!other && !grad_cam && !grad_lb && !grad_ub) return EPNP_ERR_BAD_ARG;
+    if ((grad_lb || grad_ub) && !lb) return EPNP_ERR_BAD_ARG;
+    if (B == 0 || S == 0) return EPNP_OK;
+    return by_dof(dof, [&](auto D) {
+        return launch_plain(evaluate_backward_kernel<D>, B, NT, 0, SmemAttr::none, (cudaStream_t)stream, g);
     });
 }
 

@@ -7,6 +7,9 @@
                                     -> same native kernel, upstream gradient -dL/dlogw
     evaluate_pnp(out_cost=True)     the same two kernels (correspondences / delta, poses)
     cost_init, logweights, evaluate_pnp   d/d(cam_mats, lb, ub)   native kernel (epnp_cost_camera_backward_f32)
+    evaluate_pnp(out_residual / out_jacobian [, out_cost])   d/d(x3d, x2d, w2d, delta, pose, cam_mats, lb, ub)
+                                    native kernel (epnp_evaluate_backward_f32), hence LMSolver.gn_step under autograd;
+                                    first order only (once_differentiable)
     pose_opt_plus                   one un-damped Gauss-Newton step at the (detached) solution; differentiated
                                     by torch autograd through `PerspectiveCamera.project` + `HuberPnPCost.compute`
                                     (a single evaluation, levenberg_marquardt.py:243-253 -- not the iterated path),
@@ -84,7 +87,10 @@ def _grads_to(like_list, grads):
             out.append(None)
             continue
         g = g.to(like.dtype)
-        out.append(g.sum().reshape(like.shape) if like.numel() == 1 and g.numel() != 1 else g.reshape(like.shape))
+        if like.numel() == 1 and g.numel() != 1:
+            out.append(g.sum().reshape(like.shape))
+        else:       # a broadcast input, such as a (B, N, 1) weight, receives the sum over the axes it was expanded along
+            out.append(g.reshape(like.shape) if g.numel() == like.numel() else g.sum_to_size(like.shape))
     return out
 
 
@@ -171,6 +177,65 @@ class _CostOnly(torch.autograd.Function):
         gcam, glb, gub = _camera_grads(ctx.cam_like, lambda want: native.cost_camera_backward(
             ctx.prob, ctx.dof, ctx.z_min, ctx.poses, g_cost, want=want))
         return gx3d, gx2d, gw2d, gdel, gcam, glb, gub, gpose, None, None
+
+
+class _Evaluate(torch.autograd.Function):
+    """evaluate_pnp's residual / cost / Jacobian at poses (S, B, D) with a native backward (epnp_evaluate_backward_f32)
+    with respect to the correspondences, delta, the poses and the camera.  The forward is the no-grad path's
+    native.evaluate_full call, stacked poses replicating the problem as there, so its values are the same bits."""
+
+    @staticmethod
+    def forward(ctx, x3d, x2d, w2d, delta, cam_mats, lb, ub, poses, dof, z_min, huber_eps, clip_jac, want_r, want_j,
+                want_c):
+        ctx.set_materialize_grads(False)                 # an output the loss does not use costs the backward nothing
+        prob = native.Problem(x3d, x2d, w2d, cam_mats, lb, ub, delta)
+        S, B, N = poses.shape[0], prob.B, prob.N
+        run = prob
+        if S != 1:
+            rep = lambda t: t.unsqueeze(0).expand((S,) + t.shape).reshape((S * B,) + t.shape[1:])
+            run = native.Problem(rep(prob.x3d), rep(prob.x2d), rep(prob.w2d), rep(prob.cam),
+                                 None if prob.lb is None else rep(prob.lb), None if prob.ub is None else rep(prob.ub),
+                                 rep(prob.delta))
+        r, c, j = native.evaluate_full(run, poses.reshape(-1, poses.size(-1)), dof, z_min, huber_eps, clip_jac, want_r,
+                                       want_j, want_c)
+        ctx.prob, ctx.poses, ctx.consts = prob, poses.detach(), (dof, z_min, huber_eps, clip_jac)
+        ctx.in_like = (x3d, x2d, w2d, delta if torch.is_tensor(delta) else None)
+        ctx.needs = (x3d.requires_grad, x2d.requires_grad, w2d.requires_grad,
+                     torch.is_tensor(delta) and delta.requires_grad)
+        ctx.pose_like = poses if poses.requires_grad else None
+        ctx.cam_like = _camera_like(prob, cam_mats, lb, ub)
+        dt, empty = x3d.dtype, x3d.new_zeros(0)
+        out = (r.reshape(S, B, 2 * N).to(dt) if want_r else empty, c.reshape(S, B).to(dt) if want_c else empty,
+               j.reshape(S, B, 2 * N, dof).to(dt) if want_j else empty)
+        ctx.mark_non_differentiable(*(t for t, w in zip(out, (want_r, want_c, want_j)) if not w))
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_res, g_cost, g_jac):
+        dof, z_min, huber_eps, clip_jac = ctx.consts
+        ups = [g if g is not None and g.numel() else None for g in (g_res, g_jac, g_cost)]
+        cam_want = tuple(t is not None for t in ctx.cam_like)
+        want = ctx.needs + (ctx.pose_like is not None,) + cam_want
+        if all(g is None for g in ups) or not any(want):
+            return (None,) * 15
+        grads = native.evaluate_backward(ctx.prob, ctx.poses, dof, z_min, huber_eps, clip_jac, *ups, want=want)
+        gx3d, gx2d, gw2d, gdel = _grads_to(ctx.in_like, grads[:4])
+        gpose = None if ctx.pose_like is None else _pose_grad_to(ctx.pose_like, grads[4])
+        gcam, glb, gub = _camera_grads(ctx.cam_like, lambda _: grads[5:])
+        return gx3d, gx2d, gw2d, gdel, gcam, glb, gub, gpose, None, None, None, None, None, None, None
+
+
+def evaluate_autograd(x3d, x2d, w2d, pose, camera, cost_fun, clip_jac, want_r, want_j, want_c):
+    """residual (*, B, 2N) | None, cost (*, B) | None, jacobian (*, B, 2N, dof) | None of pose hypotheses (*, B, D), with
+    autograd w.r.t. x3d / x2d / w2d / cost_fun.delta / pose / cam_mats / lb / ub."""
+    dof = 4 if pose.size(-1) == 4 else 6
+    lead, B, N = pose.shape[:-1], x3d.shape[0], x3d.shape[1]
+    r, c, j = _Evaluate.apply(x3d, x2d, w2d, _delta_tensor(cost_fun.delta, x2d), camera.cam_mats, camera.lb, camera.ub,
+                              pose.reshape(-1, B, pose.size(-1)), dof, float(camera.z_min),
+                              float(getattr(cost_fun, "eps", 1e-10)), bool(clip_jac), want_r, want_j, want_c)
+    return (r.reshape(lead + (2 * N,)) if want_r else None, c.reshape(lead) if want_c else None,
+            j.reshape(lead + (2 * N, dof)) if want_j else None)
 
 
 def _pose_grad_to(like, g):

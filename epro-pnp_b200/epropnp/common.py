@@ -68,12 +68,19 @@ def evaluate_pnp(x3d, x2d, w2d, pose, camera, cost_fun,
         raise TypeError(f"unexpected arguments {sorted(kwargs)}")
     camera_grad = _needs_grad(camera.cam_mats, camera.lb, camera.ub)
     if _needs_grad(x3d, x2d, w2d, pose, getattr(cost_fun, "delta", None)) or camera_grad:
-        native_pose_grad = x3d.is_cuda and x3d.dtype == pose.dtype == torch.float32
-        if out_jacobian is not False or out_residual is not False or \
-                ((pose.requires_grad or camera_grad) and not native_pose_grad):
-            # differentiable residual / Jacobian (LMSolver.gn_step under autograd, reference common.py:67-100), or
-            # gradients w.r.t. the pose or the camera of CPU / float64 tensors: the torch composite of the same two
-            # methods the reference calls
+        native_grad = x3d.is_cuda and x3d.dtype == pose.dtype == torch.float32
+        want_j, want_r, want_c = out_jacobian is not False, out_residual is not False, out_cost is not False
+        if (want_j or want_r) and native_grad:
+            # differentiable residual / Jacobian (LMSolver.gn_step under autograd, reference common.py:67-100): native
+            # forward + native backward
+            from .autograd import evaluate_autograd
+            residual, cost, jac = evaluate_autograd(x3d, x2d, w2d, pose, camera, cost_fun, clip_jac, want_r, want_j,
+                                                    want_c)
+            return ((_store(out_residual, residual) if want_r else None), (_store(out_cost, cost) if want_c else None),
+                    (_store(out_jacobian, jac) if want_j else None))
+        if want_j or want_r or ((pose.requires_grad or camera_grad) and not native_grad):
+            # the same outputs, or gradients w.r.t. the pose or the camera, of CPU / float64 tensors: the torch
+            # composite of the same two methods the reference calls
             x2d_proj, jac_cam = camera.project(x3d, pose, out_jac=(out_jacobian is not False), clip_jac=clip_jac)
             residual, cost, jac = cost_fun.compute(x2d_proj, x2d, w2d, jac_cam=jac_cam, out_residual=(out_residual is not False),
                                                    out_cost=(out_cost is not False), out_jacobian=(out_jacobian is not False))

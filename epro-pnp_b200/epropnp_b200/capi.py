@@ -46,6 +46,7 @@ _SIGNATURES = {
     "epnp_adaptive_delta_f32": (ctypes.c_int, [_P, _P, _F, _P, _I, _I, _P]),
     "epnp_evaluate_cost_f32": (ctypes.c_int, [_P] * 9 + [_I, _I, _I, _I, _F, _P]),
     "epnp_evaluate_f32": (ctypes.c_int, [_P] * 11 + [_I, _I, _I, _I, _F, _F, _P]),
+    "epnp_evaluate_backward_f32": (ctypes.c_int, [_P] * 19 + [_I, _I, _I, _I, _I, _F, _F, _P]),
     "epnp_lm_solve_f32": (ctypes.c_int, [_P] * 13 + [_I, _I, ctypes.POINTER(EpnpParams), _P]),
     "epnp_gn_plus_backward_f32": (ctypes.c_int, [_P] * 13 + [_I, _I, _I, _F, _F, _F, _P]),
     "epnp_gn_plus_backward_split_f32": (ctypes.c_int, [_P] * 13 + [_I, _I, _I, _F, _F, _F, _I, _P]),

@@ -142,6 +142,39 @@ def evaluate_full(prob: Problem, pose, dof, z_min, huber_eps, clip_jac, want_res
     return res, cost, jac
 
 
+def evaluate_backward(prob: Problem, poses, dof, z_min, huber_eps, clip_jac, g_res=None, g_jac=None, g_cost=None,
+                      want=(True,) * 8):
+    """Backward of evaluate_full at stacked poses (S, B, D) (epnp_evaluate_backward_f32): the vector-Jacobian product
+    with any of g_res (S, B, 2N), g_jac (S, B, 2N, dof), g_cost (S, B).  want: (x3d, x2d, w2d, delta, pose, cam_mats,
+    lb, ub) -> the same eight gradients, (B, N, 3), (B, N, 2), (B, N, 2), (B), (S, B, D), (B, 3, 3), (B, 2), (B, 2),
+    None where `want` is False.  The correspondence, delta and camera gradients are summed over the S poses."""
+    D = 7 if dof == 6 else 4
+    S, B, N = poses.shape[0], prob.B, prob.N
+    _check_pose(poses, (S, B), D, "poses")
+    ups = []
+    for g, shape, what in ((g_res, (S, B, 2 * N), "g_res"), (g_jac, (S, B, 2 * N, dof), "g_jac"),
+                           (g_cost, (S, B), "g_cost")):
+        if g is not None and tuple(g.shape) != shape:
+            raise ValueError(f"{what} must be {shape}; got {tuple(g.shape)}")
+        ups.append(None if g is None else _f32c(g))
+    if all(g is None for g in ups):
+        raise ValueError("evaluate_backward needs at least one of g_res, g_jac and g_cost")
+    if not any(want):
+        raise ValueError("want: ask for at least one gradient")
+    if (want[6] or want[7]) and prob.lb is None:
+        raise ValueError("the gradient of a bound needs the problem's bounds")
+    poses = _f32c(poses)
+    new = (lambda *s: torch.zeros(s, dtype=torch.float32, device=prob.device)) if S == 0 else prob.empty
+    shapes = ((B, N, 3), (B, N, 2), (B, N, 2), (B,), (S, B, D), (B, 3, 3), (B, 2), (B, 2))
+    out = [new(*shape) if w else None for w, shape in zip(want, shapes)]
+    with torch.cuda.device(prob.device):
+        check(lib().epnp_evaluate_backward_f32(*prob.common_ptrs(), ptr(poses), *(ptr(g) for g in ups),
+                                               *(ptr(o) for o in out), int(clip_jac), S, B, N, int(dof),
+                                               ctypes.c_float(z_min), ctypes.c_float(huber_eps),
+                                               stream_ptr(prob.device)), "epnp_evaluate_backward_f32")
+    return tuple(out)
+
+
 def _seed(fn, seed, device):
     """The Philox seed argument of `fn`: an int goes by value; a one-element int64 tensor on `device` goes by its device
     address to fn's *_seedptr_f32 form, whose kernel reads the seed when it starts -- what a CUDA graph needs to draw
@@ -652,5 +685,5 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
 
 
 __all__ = ["Problem", "adaptive_delta", "cost_backward", "cost_camera_backward", "gn_plus_camera_backward",
-           "evaluate_cost", "evaluate_cost_split", "evaluate_full", "lm_solve",
+           "evaluate_cost", "evaluate_cost_split", "evaluate_full", "evaluate_backward", "lm_solve",
            "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "rslm", "rslm_split", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

@@ -114,6 +114,25 @@ int epnp_evaluate_f32(const float* x3d, const float* x2d, const float* w2d, cons
                       float* residual, float* jac, float* cost, int clip_jac,
                       int B, int N, int dof, float z_min, float huber_eps, void* stream);
 
+/* Backward of epnp_evaluate_f32's outputs at S stacked poses (S, B, D): the vector-Jacobian product with any of the
+ * upstream gradients grad_residual (S, B, 2N), grad_jac (S, B, 2N, dof) and grad_cost (S, B) (at least one; a null one
+ * counts as zero), differentiated as the reference's autograd differentiates evaluate_pnp(out_residual, out_jacobian,
+ * out_cost): no tangent through a depth clamped at z_min, a coordinate clamped at a bound takes that bound's tangent,
+ * the clip mask is constant, the Huber scale keeps its branches and huber_eps, the Jacobian's rows are differentiated
+ * as written with K's first two rows, and the rotation with respect to the raw pose components.  Outputs, each optional
+ * but at least one:
+ *   grad_x3d (B, N, 3), grad_x2d / grad_w2d (B, N, 2), grad_delta (B)   summed over the S poses
+ *   grad_pose (S, B, D)
+ *   grad_cam (B, 3, 3), grad_lb / grad_ub (B, 2)                         summed over the S poses; bounds' only with bounds
+ * One CTA per object over the points in global memory: any N.  Fixed-order reductions, no atomics: an object's results
+ * depend on nothing else in the batch.  B = 0 or S = 0 writes nothing.                                           */
+int epnp_evaluate_backward_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                               const float* lb, const float* ub, const float* delta, const float* poses,
+                               const float* grad_residual, const float* grad_jac, const float* grad_cost,
+                               float* grad_x3d, float* grad_x2d, float* grad_w2d, float* grad_delta, float* grad_pose,
+                               float* grad_cam, float* grad_lb, float* grad_ub, int clip_jac, int S, int B, int N,
+                               int dof, float z_min, float huber_eps, void* stream);
+
 /* Backward of the derivative-regularisation branch: pose_opt_plus = pose (+) gn_step(pose) with the pose detached
  * (LMSolver.forward :66-68, gn_step :243-253, pose_add :255-265, evaluated with autograd on in the reference:
  * camera.py:119-129, cost_fun.py:52-84).  Given dL/d pose_opt_plus (B, D), writes dL/d x3d (B, N, 3), dL/d x2d

@@ -73,8 +73,12 @@ for dof, N, B, bounded in ((6, 64, 5, False), (6, 130, 3, True), (6, 51, 4, Fals
         cam = [native.cost_camera_backward(bounded, dof, 0.1, out["pose_samples"], torch.randn(B, 128, device=dev),
                                            d["pose_init"].reshape(B, 1, D), torch.randn(B, 1, device=dev)),
                native.gn_plus_camera_backward(bounded, out["pose_opt"], gp, dof, 0.1, 1e-5, 1e-10)]
+        ev = native.evaluate_backward(bounded, out["pose_samples"][:, :3].transpose(0, 1).contiguous(), dof, 0.1, 1e-10,
+                                      True, torch.randn(3, B, 2 * N, device=dev),
+                                      torch.randn(3, B, 2 * N, dof, device=dev), torch.randn(3, B, device=dev))
         torch.cuda.synchronize()
         check(f"{tag}: finite camera gradients", all(torch.isfinite(t).all() for g3 in cam for t in g3))
+        check(f"{tag}: finite residual / Jacobian gradients", all(torch.isfinite(t).all() for t in ev))
     torch.cuda.synchronize()
     check(f"dof={dof} N={N}: finite log-weights", torch.isfinite(out["logw"]).all())
     check(f"dof={dof} N={N}: finite gradients", all(torch.isfinite(t).all() for t in g))
