@@ -9,7 +9,7 @@
     cost_init, logweights, evaluate_pnp   d/d(cam_mats, lb, ub)   native kernel (epnp_cost_camera_backward_f32)
     evaluate_pnp(out_residual / out_jacobian [, out_cost])   d/d(x3d, x2d, w2d, delta, pose, cam_mats, lb, ub)
                                     native kernel (epnp_evaluate_backward_f32), hence LMSolver.gn_step under autograd;
-                                    first order only (once_differentiable)
+                                    first order only (a second backward raises)
     pose_opt_plus                   one un-damped Gauss-Newton step at the (detached) solution; differentiated
                                     by torch autograd through `PerspectiveCamera.project` + `HuberPnPCost.compute`
                                     (a single evaluation, levenberg_marquardt.py:243-253 -- not the iterated path),
@@ -27,12 +27,17 @@ the native draw's own limit: 53,504 points at n = 16); by default it refuses obj
 
 Gradients w.r.t. poses (pose_init, stacked hypotheses) are those of the rotation the forward calls use, with respect to
 the raw pose components; pose_opt, the samples and the solver's start carry none (reference epropnp.py:139-140).
+
+The forward calls and their formulas are the epropnp custom operators of epropnp_b200.ops (register_autograd), one path
+for eager calls, torch.compile and torch.export; the functions below give them the layer's camera / cost objects and
+cast to the caller's dtype.  The operators' implementations take the resident or split call through the helpers here.
 """
 import functools
+import os
 
 import torch
 
-from epropnp_b200 import native
+from epropnp_b200 import native, ops
 
 
 @functools.lru_cache(maxsize=None)
@@ -72,254 +77,83 @@ def epnp_init(x3d, x2d, w2d, cam_mats, conf_quantile):
     return (native.epnp_init_split if split else native.epnp_init)(x3d, x2d, w2d, cam_mats, conf_quantile)
 
 
-def _delta_tensor(delta, ref):
-    if torch.is_tensor(delta):
-        return delta
-    return ref.new_tensor(float(delta))
-
-
-def _grads_to(like_list, grads):
-    """Native gradients (B,N,3) / (B,N,2) / (B,N,2) / (B) -> dtype and shape of the inputs they belong to
-    (a scalar / 1-element delta tensor receives the sum over objects)."""
-    out = []
-    for like, g in zip(like_list, grads):
-        if like is None or g is None:
-            out.append(None)
-            continue
-        g = g.to(like.dtype)
-        if like.numel() == 1 and g.numel() != 1:
-            out.append(g.sum().reshape(like.shape))
-        else:       # a broadcast input, such as a (B, N, 1) weight, receives the sum over the axes it was expanded along
-            out.append(g.reshape(like.shape) if g.numel() == like.numel() else g.sum_to_size(like.shape))
-    return out
-
-
-class _MonteCarloForward(torch.autograd.Function):
-    """Fused LM + AMIS forward; backward = native Monte-Carlo cost gradient."""
-
-    @staticmethod
-    def forward(ctx, x3d, x2d, w2d, delta, cam_mats, lb, ub, pose_start, cost_init_pose, params, noise, seed,
-                want_cost, z_min):
-        prob = native.Problem(x3d, x2d, w2d, cam_mats, lb, ub, delta)
-        out = fused_forward(prob, pose_start, params, noise=noise, seed=seed, want_cost=want_cost,
-                            want_cost_init=False, want_cov=False)
-        dof = params.dof
-        cost_init = None
-        if cost_init_pose is not None:
-            cost_init = stacked_cost(prob, cost_init_pose.detach().unsqueeze(0), dof, z_min)[0]
-        ctx.prob, ctx.dof, ctx.z_min = prob, dof, z_min
-        ctx.samples = out["pose_samples"]
-        ctx.cost_init_pose = None if cost_init_pose is None else cost_init_pose.detach()
-        ctx.in_like = (x3d, x2d, w2d, delta if torch.is_tensor(delta) else None)
-        ctx.needs = (x3d.requires_grad, x2d.requires_grad, w2d.requires_grad,
-                     torch.is_tensor(delta) and delta.requires_grad)
-        ctx.pose_like = cost_init_pose if cost_init_pose is not None and cost_init_pose.requires_grad else None
-        ctx.cam_like = _camera_like(prob, cam_mats, lb, ub)
-        cost = out["cost"] if want_cost else x3d.new_zeros(0)
-        ci = cost_init if cost_init is not None else x3d.new_zeros(0)
-        dt = x3d.dtype
-        # cast FIRST, then mark the tensors that are actually returned (for non-fp32 inputs .to() makes new tensors)
-        pose_opt, cost, samples = out["pose_opt"].to(dt), cost.to(dt), out["pose_samples"].to(dt)
-        ctx.mark_non_differentiable(pose_opt, cost, samples)
-        return pose_opt, cost, samples, out["logw"].to(dt), ci.to(dt)
-
-    @staticmethod
-    def backward(ctx, g_pose, g_cost, g_samples, g_logw, g_cost_init):
-        prob = ctx.prob
-        B = prob.B
-        if g_logw is None:
-            g_logw = torch.zeros(B, ctx.samples.shape[1], device=prob.device)
-        poses_b = grad_b = None
-        if ctx.cost_init_pose is not None and g_cost_init is not None and g_cost_init.numel() == B:
-            poses_b = ctx.cost_init_pose.reshape(B, 1, -1)
-            grad_b = g_cost_init.reshape(B, 1)
-        grads = (None,) * 4
-        if any(ctx.needs):
-            grads = native.cost_backward(prob, ctx.dof, ctx.z_min, ctx.samples, -g_logw.contiguous(), poses_b, grad_b,
-                                         want=ctx.needs)
-        gx3d, gx2d, gw2d, gdel = _grads_to(ctx.in_like, grads)
-        gpose = None
-        if ctx.pose_like is not None and poses_b is not None:
-            gpose = _pose_grad_to(ctx.pose_like, native.cost_pose_backward(prob, ctx.dof, ctx.z_min, poses_b, grad_b)[:, 0])
-        gcam, glb, gub = _camera_grads(ctx.cam_like, lambda want: native.cost_camera_backward(
-            prob, ctx.dof, ctx.z_min, ctx.samples, -g_logw.contiguous(), poses_b, grad_b, want=want))
-        return gx3d, gx2d, gw2d, gdel, gcam, glb, gub, None, gpose, None, None, None, None, None
-
-
-class _CostOnly(torch.autograd.Function):
-    """evaluate_pnp(out_cost=True) with gradients w.r.t. the correspondences / delta and the poses (S, B, D)."""
-
-    @staticmethod
-    def forward(ctx, x3d, x2d, w2d, delta, cam_mats, lb, ub, poses, dof, z_min):
-        prob = native.Problem(x3d, x2d, w2d, cam_mats, lb, ub, delta)
-        S = poses.shape[0]
-        cost = stacked_cost(prob, poses, dof, z_min)                            # (S, B)
-        ctx.prob, ctx.dof, ctx.z_min = prob, dof, z_min
-        ctx.poses = poses.detach().transpose(0, 1).contiguous()                 # object-major (B, S, D)
-        ctx.in_like = (x3d, x2d, w2d, delta if torch.is_tensor(delta) else None)
-        ctx.needs = (x3d.requires_grad, x2d.requires_grad, w2d.requires_grad,
-                     torch.is_tensor(delta) and delta.requires_grad)
-        ctx.pose_like = poses if poses.requires_grad else None
-        ctx.cam_like = _camera_like(prob, cam_mats, lb, ub)
-        return cost.to(x3d.dtype)
-
-    @staticmethod
-    def backward(ctx, g_cost):
-        g_cost = g_cost.transpose(0, 1).contiguous()                            # object-major (B, S)
-        grads = (None,) * 4
-        if any(ctx.needs):
-            grads = native.cost_backward(ctx.prob, ctx.dof, ctx.z_min, ctx.poses, g_cost, want=ctx.needs)
-        gx3d, gx2d, gw2d, gdel = _grads_to(ctx.in_like, grads)
-        gpose = None
-        if ctx.pose_like is not None:
-            gpose = _pose_grad_to(ctx.pose_like,
-                                  native.cost_pose_backward(ctx.prob, ctx.dof, ctx.z_min, ctx.poses, g_cost).transpose(0, 1))
-        gcam, glb, gub = _camera_grads(ctx.cam_like, lambda want: native.cost_camera_backward(
-            ctx.prob, ctx.dof, ctx.z_min, ctx.poses, g_cost, want=want))
-        return gx3d, gx2d, gw2d, gdel, gcam, glb, gub, gpose, None, None
-
-
-class _Evaluate(torch.autograd.Function):
-    """evaluate_pnp's residual / cost / Jacobian at poses (S, B, D) with a native backward (epnp_evaluate_backward_f32)
-    with respect to the correspondences, delta, the poses and the camera.  The forward is the no-grad path's
-    native.evaluate_full call, stacked poses replicating the problem as there, so its values are the same bits."""
-
-    @staticmethod
-    def forward(ctx, x3d, x2d, w2d, delta, cam_mats, lb, ub, poses, dof, z_min, huber_eps, clip_jac, want_r, want_j,
-                want_c):
-        ctx.set_materialize_grads(False)                 # an output the loss does not use costs the backward nothing
-        prob = native.Problem(x3d, x2d, w2d, cam_mats, lb, ub, delta)
-        S, B, N = poses.shape[0], prob.B, prob.N
-        run = prob
-        if S != 1:
-            rep = lambda t: t.unsqueeze(0).expand((S,) + t.shape).reshape((S * B,) + t.shape[1:])
-            run = native.Problem(rep(prob.x3d), rep(prob.x2d), rep(prob.w2d), rep(prob.cam),
-                                 None if prob.lb is None else rep(prob.lb), None if prob.ub is None else rep(prob.ub),
-                                 rep(prob.delta))
-        r, c, j = native.evaluate_full(run, poses.reshape(-1, poses.size(-1)), dof, z_min, huber_eps, clip_jac, want_r,
-                                       want_j, want_c)
-        ctx.prob, ctx.poses, ctx.consts = prob, poses.detach(), (dof, z_min, huber_eps, clip_jac)
-        ctx.in_like = (x3d, x2d, w2d, delta if torch.is_tensor(delta) else None)
-        ctx.needs = (x3d.requires_grad, x2d.requires_grad, w2d.requires_grad,
-                     torch.is_tensor(delta) and delta.requires_grad)
-        ctx.pose_like = poses if poses.requires_grad else None
-        ctx.cam_like = _camera_like(prob, cam_mats, lb, ub)
-        dt, empty = x3d.dtype, x3d.new_zeros(0)
-        out = (r.reshape(S, B, 2 * N).to(dt) if want_r else empty, c.reshape(S, B).to(dt) if want_c else empty,
-               j.reshape(S, B, 2 * N, dof).to(dt) if want_j else empty)
-        ctx.mark_non_differentiable(*(t for t, w in zip(out, (want_r, want_c, want_j)) if not w))
-        return out
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, g_res, g_cost, g_jac):
-        dof, z_min, huber_eps, clip_jac = ctx.consts
-        ups = [g if g is not None and g.numel() else None for g in (g_res, g_jac, g_cost)]
-        cam_want = tuple(t is not None for t in ctx.cam_like)
-        want = ctx.needs + (ctx.pose_like is not None,) + cam_want
-        if all(g is None for g in ups) or not any(want):
-            return (None,) * 15
-        grads = native.evaluate_backward(ctx.prob, ctx.poses, dof, z_min, huber_eps, clip_jac, *ups, want=want)
-        gx3d, gx2d, gw2d, gdel = _grads_to(ctx.in_like, grads[:4])
-        gpose = None if ctx.pose_like is None else _pose_grad_to(ctx.pose_like, grads[4])
-        gcam, glb, gub = _camera_grads(ctx.cam_like, lambda _: grads[5:])
-        return gx3d, gx2d, gw2d, gdel, gcam, glb, gub, gpose, None, None, None, None, None, None, None
+def _problem_args(x3d, x2d, w2d, camera, cost_fun):
+    """The seven problem arguments of the epropnp operators for a camera and a cost object (ops.problem_args)."""
+    return ops.problem_args(x3d, x2d, w2d, camera.cam_mats, camera.lb, camera.ub, cost_fun.delta)
 
 
 def evaluate_autograd(x3d, x2d, w2d, pose, camera, cost_fun, clip_jac, want_r, want_j, want_c):
     """residual (*, B, 2N) | None, cost (*, B) | None, jacobian (*, B, 2N, dof) | None of pose hypotheses (*, B, D), with
-    autograd w.r.t. x3d / x2d / w2d / cost_fun.delta / pose / cam_mats / lb / ub."""
+    autograd w.r.t. x3d / x2d / w2d / cost_fun.delta / pose / cam_mats / lb / ub (first order only)."""
     dof = 4 if pose.size(-1) == 4 else 6
     lead, B, N = pose.shape[:-1], x3d.shape[0], x3d.shape[1]
-    r, c, j = _Evaluate.apply(x3d, x2d, w2d, _delta_tensor(cost_fun.delta, x2d), camera.cam_mats, camera.lb, camera.ub,
-                              pose.reshape(-1, B, pose.size(-1)), dof, float(camera.z_min),
-                              float(getattr(cost_fun, "eps", 1e-10)), bool(clip_jac), want_r, want_j, want_c)
-    return (r.reshape(lead + (2 * N,)) if want_r else None, c.reshape(lead) if want_c else None,
-            j.reshape(lead + (2 * N, dof)) if want_j else None)
-
-
-def _pose_grad_to(like, g):
-    """Native pose gradient -> dtype and shape of the pose tensor it belongs to."""
-    return g.to(like.dtype).reshape(like.shape)
-
-
-def _camera_like(prob, cam_mats, lb, ub):
-    """The camera inputs that require grad (cam_mats, lb, ub; None elsewhere).  Python-float bounds get no gradient, and
-    neither does a bound while the other is missing: the projection is then not clamped."""
-    grad = lambda t: torch.is_tensor(t) and t.requires_grad
-    bounded = prob.lb is not None
-    return (cam_mats if grad(cam_mats) else None, lb if bounded and grad(lb) else None,
-            ub if bounded and grad(ub) else None)
-
-
-def _camera_grads(like, run):
-    """run(want) -> native (B, 3, 3) / (B, 2) / (B, 2) camera gradients, each reduced to the dtype and shape of the
-    tensor the caller passed: a (3, 3) camera or a (2,) bound shared by every object receives the sum over objects (an
-    expanded one receives them per object; autograd sums them through the expand)."""
-    want = tuple(t is not None for t in like)
-    if not any(want):
-        return None, None, None
-    out = []
-    for t, g in zip(like, run(want)):
-        if t is None:
-            out.append(None)
-            continue
-        g = g.to(t.dtype)
-        out.append(g.sum_to_size(t.shape) if t.dim() else g.sum())
-    return tuple(out)
+    r, c, j = ops.evaluate_full(*_problem_args(x3d, x2d, w2d, camera, cost_fun), pose.reshape(-1, B, pose.size(-1)),
+                                dof, float(camera.z_min), float(getattr(cost_fun, "eps", 1e-10)), bool(clip_jac),
+                                want_r, want_j, want_c)
+    dt = x3d.dtype
+    return (r.to(dt).reshape(lead + (2 * N,)) if want_r else None, c.to(dt).reshape(lead) if want_c else None,
+            j.to(dt).reshape(lead + (2 * N, dof)) if want_j else None)
 
 
 def evaluate_cost_autograd(x3d, x2d, w2d, pose, camera, cost_fun):
-    """cost (*, B) of pose hypotheses with autograd w.r.t. x3d / x2d / w2d / cost_fun.delta / pose."""
+    """cost (*, B) of pose hypotheses with autograd w.r.t. x3d / x2d / w2d / cost_fun.delta / pose / cam_mats / lb /
+    ub."""
     dof = 4 if pose.size(-1) == 4 else 6
     lead = pose.shape[:-1]
     B = x3d.shape[0]
-    cost = _CostOnly.apply(x3d, x2d, w2d, _delta_tensor(cost_fun.delta, x2d), camera.cam_mats, camera.lb, camera.ub,
-                           pose.reshape(-1, B, pose.size(-1)), dof, float(camera.z_min))
-    return cost.reshape(lead)
+    cost = ops.evaluate_cost(*_problem_args(x3d, x2d, w2d, camera, cost_fun), pose.reshape(-1, B, pose.size(-1)), dof,
+                             float(camera.z_min))
+    return cost.to(x3d.dtype).reshape(lead)
 
 
-def monte_carlo_autograd(x3d, x2d, w2d, camera, cost_fun, pose_start, pose_init, params, noise, seed, want_cost):
-    """-> pose_opt, cost | None, pose_samples (B,M,D), logw (B,M) [differentiable], cost_init | None [differentiable]."""
-    pose_opt, cost, samples, logw, cost_init = _MonteCarloForward.apply(
-        x3d, x2d, w2d, _delta_tensor(cost_fun.delta, x2d), camera.cam_mats, camera.lb, camera.ub, pose_start.detach(),
-        pose_init, params, noise, seed, bool(want_cost), float(camera.z_min))
-    return pose_opt, (cost if want_cost else None), samples, logw, (cost_init if pose_init is not None else None)
+def monte_carlo_autograd(x3d, x2d, w2d, camera, cost_fun, pose_start, pose_init, params, noise, seed, want_cost,
+                         want_plus=False, want_cost_init=False):
+    """The fused LM + AMIS operator from pose_start; `params` an (ints, floats) pair (ops.param_lists).
+    -> pose_opt, cost | None, pose_opt_plus | None, pose_samples (B, M, D), logw (B, M) [differentiable],
+    cost_init | None [differentiable when pose_init is given: the cost at pose_init]."""
+    noise = (None,) * 3 if noise is None else noise
+    pose_opt, cost, plus, cost_init, samples, logw = ops.lm_amis_fused(
+        *_problem_args(x3d, x2d, w2d, camera, cost_fun), pose_start.detach(), pose_init, *noise, *ops.seed_args(seed),
+        params[0], params[1], bool(want_cost), bool(want_plus), bool(want_cost_init))
+    dt = x3d.dtype
+    has_ci = pose_init is not None or want_cost_init
+    return (pose_opt.to(dt), cost.to(dt) if want_cost else None, plus.to(dt) if want_plus else None, samples.to(dt),
+            logw.to(dt), cost_init.to(dt) if has_ci else None)
 
 
 class _PosePlus(torch.autograd.Function):
     """pose (+) gn_step(pose) with a native backward (epnp_gn_plus_backward_f32, or its split form above the resident
-    limit)."""
+    limit; epnp_gn_plus_camera_backward_f32 for the camera): the eager form of the lm_solve operator's pose_opt_plus
+    formula, over the same operator and the same backward (ops.gn_plus_grads), kept as a Function of its own so that the
+    graph names it.  Under torch.compile pose_plus_autograd calls the operator itself.  `params` an EpnpParams or an
+    (ints, floats) pair; delta, lb and ub tensors or Python floats (those get no gradient)."""
 
     @staticmethod
     def forward(ctx, x3d, x2d, w2d, delta, cam_mats, lb, ub, pose, params, huber_eps):
-        prob = native.Problem(x3d, x2d, w2d, cam_mats, lb, ub, delta)
-        plus = native.lm_solve(prob, pose, params, want_plus=True)["pose_opt_plus"]
-        ctx.prob, ctx.pose, ctx.dof = prob, pose.detach(), params.dof
-        ctx.consts = (float(params.z_min), float(params.eps), float(huber_eps))
-        ctx.in_like = (x3d, x2d, w2d, delta if torch.is_tensor(delta) else None)
-        ctx.needs = (x3d.requires_grad, x2d.requires_grad, w2d.requires_grad,
-                     torch.is_tensor(delta) and delta.requires_grad)
-        ctx.cam_like = _camera_like(prob, cam_mats, lb, ub)
+        ints, floats = ops.param_lists(params)
+        prob = ops.problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta)
+        plus = ops.lm_solve(*prob, pose, ints, floats, False, False, True)[3]
+        ctx.save_for_backward(*(t for t in prob if t is not None), pose)
+        ctx.bounded = prob[4] is not None
+        ctx.consts = (ints[0], floats[0], floats[6], float(huber_eps))              # dof, z_min, eps, huber_eps
         return plus.to(x3d.dtype)
 
     @staticmethod
     def backward(ctx, grad_plus):
-        z_min, eps, huber_eps = ctx.consts
-        grads = (None,) * 4
-        if any(ctx.needs):
-            grads = gn_plus_backward(ctx.prob, ctx.pose, grad_plus, ctx.dof, z_min, eps, huber_eps, ctx.needs)
-        g3, g2, gw, gd = _grads_to(ctx.in_like, grads)
-        gcam, glb, gub = _camera_grads(ctx.cam_like, lambda want: native.gn_plus_camera_backward(
-            ctx.prob, ctx.pose, grad_plus, ctx.dof, z_min, eps, huber_eps, want=want))
-        return g3, g2, gw, gd, gcam, glb, gub, None, None, None
+        saved = list(ctx.saved_tensors)
+        pose = saved.pop()
+        x3d, x2d, w2d, cam_mats = saved[:4]
+        lb, ub = (saved[4], saved[5]) if ctx.bounded else (None, None)
+        prob = (x3d, x2d, w2d, cam_mats, lb, ub, saved[-1])
+        n = ctx.needs_input_grad
+        g = ops.gn_plus_grads(prob, pose, grad_plus, *ctx.consts, (n[0], n[1], n[2], n[4], n[5], n[6], n[3]))
+        return g[0], g[1], g[2], g[6], g[3], g[4], g[5], None, None, None
 
 
 def native_gn_step_enabled():
     """pose_opt_plus is differentiated by the native kernel (epnp_gn_plus_backward_f32; validated on the GPU against the
     float64 composite and the reference's own autograd).  EPNP_NATIVE_GN_STEP=0 selects the torch-autograd composite of
     PerspectiveCamera.project + HuberPnPCost.compute instead (exact in float64; used by the CPU tests and for A/B timing)."""
-    import os
     return os.environ.get("EPNP_NATIVE_GN_STEP", "1") not in ("", "0")
 
 
@@ -327,9 +161,12 @@ def pose_plus_autograd(solver, x3d, x2d, w2d, pose, camera, cost_fun):
     """Differentiable pose (+) one un-damped Gauss-Newton step at the detached `pose` (LMSolver.forward :66-68)."""
     if not native_gn_step_enabled():
         return solver.pose_add(pose, gn_step_autograd(solver, x3d, x2d, w2d, pose, camera, cost_fun), camera)
-    params = solver.native_params(camera, cost_fun, False)
-    params.lm_iter = 0                                       # evaluate the step at `pose` itself
+    params = solver.param_lists(camera, cost_fun, False, lm_iter=0)     # evaluate the step at `pose` itself
     delta = cost_fun.delta
+    if torch.compiler.is_compiling():
+        plus = ops.lm_solve(*_problem_args(x3d, x2d, w2d, camera, cost_fun), pose.detach(), *params, False, False,
+                            True)[3]
+        return plus.to(x3d.dtype)
     return _PosePlus.apply(x3d, x2d, w2d, delta if torch.is_tensor(delta) else float(delta), camera.cam_mats,
                            camera.lb, camera.ub, pose.detach(), params, float(getattr(cost_fun, "eps", 1e-10)))
 

@@ -5,7 +5,7 @@ and the normalisation transform are a few torch ops on (B, 3)-sized tensors (not
 """
 import torch
 
-from epropnp_b200 import native
+from epropnp_b200 import ops
 
 
 def skew(x):
@@ -94,23 +94,18 @@ def evaluate_pnp(x3d, x2d, w2d, pose, camera, cost_fun,
     dof = 4 if pose.size(-1) == 4 else 6
     lead = pose.shape[:-1]
     B, n = x3d.shape[0], x3d.shape[1]
-    prob = native.Problem(x3d, x2d, w2d, camera.cam_mats, camera.lb, camera.ub, cost_fun.delta)
     want_j, want_r, want_c = out_jacobian is not False, out_residual is not False, out_cost is not False
+    from .autograd import _problem_args
+    args = _problem_args(x3d, x2d, w2d, camera, cost_fun)
+    poses = pose.reshape(-1, B, pose.size(-1))
     residual = cost = jac = None
     if not want_j and not want_r:
         if want_c:
-            from .autograd import stacked_cost
-            cost = stacked_cost(prob, pose.reshape(-1, B, pose.size(-1)), dof, camera.z_min).reshape(lead)
+            cost = ops.evaluate_cost(*args, poses, dof, float(camera.z_min)).reshape(lead)
     else:
-        if pose.dim() != 2:
-            # stacked hypotheses with Jacobians: treat every (hypothesis, object) as its own object
-            S = pose.reshape(-1, B, pose.size(-1)).shape[0]
-            rep = lambda t: t.unsqueeze(0).expand((S,) + t.shape).reshape((S * B,) + t.shape[1:])
-            prob = native.Problem(rep(prob.x3d), rep(prob.x2d), rep(prob.w2d), rep(prob.cam),
-                                  None if prob.lb is None else rep(prob.lb), None if prob.ub is None else rep(prob.ub),
-                                  rep(prob.delta))
-        r, c, j = native.evaluate_full(prob, pose.reshape(-1, pose.size(-1)), dof, camera.z_min,
-                                       getattr(cost_fun, "eps", 1e-10), clip_jac, want_r, want_j, want_c)
+        # stacked hypotheses with Jacobians: every (hypothesis, object) is its own object
+        r, c, j = ops.evaluate_full(*args, poses, dof, float(camera.z_min), float(getattr(cost_fun, "eps", 1e-10)),
+                                    bool(clip_jac), want_r, want_j, want_c)
         residual = r.reshape(lead + (2 * n,)) if want_r else None
         cost = c.reshape(lead) if want_c else None
         jac = j.reshape(lead + (2 * n, dof)) if want_j else None
@@ -129,7 +124,8 @@ def philox_seed(seed, device):
     new seed and the kernels draw new samples -- an int would be baked into the graph."""
     if seed is not None:
         return seed if torch.is_tensor(seed) and seed.is_cuda else int(seed)
-    if torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing():    # (no CUDA context: no capture)
+    # under torch.compile likewise: a compiled graph (and a reduce-overhead CUDA graph) replays what was traced
+    if torch.compiler.is_compiling() or (torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing()):
         return torch.randint(0, 2 ** 62, (1,), dtype=torch.int64, device=device)
     return int(torch.randint(0, 2 ** 62, (1,)).item())
 

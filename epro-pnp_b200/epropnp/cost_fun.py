@@ -6,7 +6,7 @@ callers that already hold projected points; it is a few elementwise torch ops an
 """
 import torch
 
-from epropnp_b200 import native
+from epropnp_b200 import ops
 from .builder import COSTFUN
 
 
@@ -102,7 +102,7 @@ class AdaptiveHuberPnPCost(HuberPnPCost):
     def set_param(self, x2d, w2d):
         needs_graph = torch.is_grad_enabled() and (x2d.requires_grad or w2d.requires_grad)
         if x2d.is_cuda and x2d.dim() == 3 and not needs_graph:
-            self.delta = native.adaptive_delta(x2d, w2d, self.relative_delta).to(x2d.dtype)   # one native kernel
+            self.delta = ops.adaptive_delta(x2d, w2d, float(self.relative_delta)).to(x2d.dtype)   # one native kernel
             return
         # differentiable / generic-shape path: the same formula in torch so autograd reaches w2d (and x2d)
         spread = torch.var(x2d, dim=-2).sum(dim=-1).sqrt()

@@ -14,7 +14,7 @@ refused with ValueError at the first solve.
 import torch
 import torch.nn as nn
 
-from epropnp_b200 import native
+from epropnp_b200 import ops
 from . import autograd
 from .builder import PNP
 
@@ -36,9 +36,9 @@ class EPnPSolver(nn.Module):
     def solve(self, x3d, x2d, w2d, camera, cost_fun, with_cost=False, **kwargs):
         """-> pose (B, 7), None, cost (B) | None.  With with_cost, the cost is evaluate_pnp's at the EPnP pose (what
         LMSolver compares against pose_init under force_init_solve)."""
-        pose = autograd.epnp_init(x3d.detach(), x2d.detach(), w2d.detach(), camera.cam_mats, self.conf_quantile)
+        pose = ops.epnp_init(x3d.detach(), x2d.detach(), w2d.detach(), camera.cam_mats, self.conf_quantile)
         cost = None
         if with_cost:
-            prob = native.Problem(x3d, x2d, w2d, camera.cam_mats, camera.lb, camera.ub, cost_fun.delta)
-            cost = autograd.stacked_cost(prob, pose[None], 6, float(camera.z_min))[0].to(x2d.dtype)
+            cost = ops.evaluate_cost(*autograd._problem_args(x3d, x2d, w2d, camera, cost_fun), pose[None], 6,
+                                     float(camera.z_min))[0].to(x2d.dtype)
         return pose.to(x2d.dtype), None, cost

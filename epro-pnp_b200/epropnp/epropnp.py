@@ -25,7 +25,6 @@ from abc import ABCMeta, abstractmethod
 
 import torch
 
-from epropnp_b200 import native
 from .builder import PNP, build_pnp
 from .common import _camera_requires_grad, evaluate_pnp, philox_seed, pnp_normalize, pnp_denormalize
 from .distributions import AngularCentralGaussian, MultivariateStudentT, VonMisesUniformMix
@@ -77,9 +76,10 @@ class EProPnPBase(torch.nn.Module, metaclass=ABCMeta):
         pass
 
     def _amis_params(self, camera, cost_fun, fast_mode):
-        return self.solver.native_params(camera, cost_fun, fast_mode, mc_samples=int(self.mc_samples),
-                                         mc_iter=int(self.num_iter), amis_eps=float(self.eps),
-                                         **self._extra_native_params())
+        """(ints, floats) of the fused operator (ops.param_lists)."""
+        return self.solver.param_lists(camera, cost_fun, fast_mode, mc_samples=int(self.mc_samples),
+                                       mc_iter=int(self.num_iter), amis_eps=float(self.eps),
+                                       **self._extra_native_params())
 
     def _extra_native_params(self):
         return {}
@@ -172,18 +172,14 @@ class EProPnPBase(torch.nn.Module, metaclass=ABCMeta):
                 seed = philox_seed(amis_seed, x3d.device)
                 params = self._amis_params(camera, cost_fun, fast_mode)
                 if not differentiable:
-                    prob = native.Problem(x3d, x2d, w2d, camera.cam_mats, camera.lb, camera.ub, cost_fun.delta)
-                    from .autograd import fused_forward
-                    out = fused_forward(prob, start, params, noise=amis_noise, seed=seed, want_cost=with_cost,
-                                        want_plus=with_plus,
-                                        want_cost_init=(pose_init is not None and not needs_init_solver),
-                                        want_cov=False)
-                    cast = lambda t: None if t is None else t.to(x3d.dtype)
-                    pose_opt, cost, pose_opt_plus = cast(out["pose_opt"]), cast(out["cost"]), cast(out["pose_opt_plus"])
+                    from .autograd import monte_carlo_autograd
+                    pose_opt, cost, pose_opt_plus, samples_bm, logw_bm, ci = monte_carlo_autograd(
+                        x3d, x2d, w2d, camera, cost_fun, start, None, params, amis_noise, seed, with_cost,
+                        want_plus=with_plus, want_cost_init=(pose_init is not None and not needs_init_solver))
                     if cost_init is None:
-                        cost_init = cast(out["cost_init"])
-                    pose_samples = cast(out["pose_samples"]).transpose(0, 1)      # (M, B, D) view
-                    logw = cast(out["logw"]).transpose(0, 1)                      # (M, B) view
+                        cost_init = ci
+                    pose_samples = samples_bm.transpose(0, 1)      # (M, B, D) view
+                    logw = logw_bm.transpose(0, 1)                 # (M, B) view
 
         if num_obj == 0 and torch.is_grad_enabled():
             # an empty batch must still be part of the graph (reference epropnp.py:184-187 and its differentiable
@@ -199,7 +195,7 @@ class EProPnPBase(torch.nn.Module, metaclass=ABCMeta):
         if num_obj > 0 and differentiable:
             # training path: forward = the same fused kernel, backward = native Monte-Carlo cost gradient
             from .autograd import monte_carlo_autograd, pose_plus_autograd
-            pose_opt, cost, samples_bm, logw_bm, cost_init = monte_carlo_autograd(
+            pose_opt, cost, _, samples_bm, logw_bm, cost_init = monte_carlo_autograd(
                 x3d, x2d, w2d, camera, cost_fun, start, pose_init, params, amis_noise, seed, with_cost)
             pose_samples, logw = samples_bm.transpose(0, 1), logw_bm.transpose(0, 1)
             pose_opt_plus = None

@@ -15,8 +15,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from epropnp_b200 import native
-from .autograd import rslm_solve
+from epropnp_b200 import ops
+from .autograd import _problem_args
 from .builder import PNP, build_pnp
 from .common import _camera_requires_grad, evaluate_pnp, philox_seed, pnp_normalize, pnp_denormalize
 
@@ -51,13 +51,19 @@ class LMSolver(nn.Module):
 
     # ------------------------------------------------------------------ native parameter block
     def native_params(self, camera, cost_fun, fast_mode=False, **extra):
-        return native.default_params(
-            self.dof, lm_iter=int(self.num_iter), fast_mode=int(bool(fast_mode)), z_min=float(camera.z_min),
-            min_lm_diagonal=float(self.min_lm_diagonal), max_lm_diagonal=float(self.max_lm_diagonal),
-            min_relative_decrease=float(self.min_relative_decrease),
-            initial_radius=float(self.initial_trust_region_radius),
-            max_radius=float(self.max_trust_region_radius), eps=float(self.eps),
-            huber_eps=float(getattr(cost_fun, "eps", 1e-10)), **extra)
+        """The solver's EpnpParams block (ctypes), as the C ABI takes it."""
+        return ops.make_params(*self.param_lists(camera, cost_fun, fast_mode, **extra))
+
+    def param_lists(self, camera, cost_fun, fast_mode=False, **extra):
+        """The same block as the (ints, floats) lists the epropnp operators take (ops.param_lists; traceable)."""
+        fields = dict(lm_iter=int(self.num_iter), fast_mode=int(bool(fast_mode)), z_min=float(camera.z_min),
+                      min_lm_diagonal=float(self.min_lm_diagonal), max_lm_diagonal=float(self.max_lm_diagonal),
+                      min_relative_decrease=float(self.min_relative_decrease),
+                      initial_radius=float(self.initial_trust_region_radius),
+                      max_radius=float(self.max_trust_region_radius), eps=float(self.eps),
+                      huber_eps=float(getattr(cost_fun, "eps", 1e-10)))
+        fields.update(extra)
+        return ops.param_lists(None, self.dof, **fields)
 
     def _pose_dim(self):
         return 4 if self.dof == 4 else 7
@@ -119,11 +125,11 @@ class LMSolver(nn.Module):
                     torch.empty((0,), **kw) if with_cost else None,
                     torch.empty((0, self._pose_dim()), **kw) if with_pose_opt_plus else None)
         start = self._starting_pose(x3d, x2d, w2d, camera, cost_fun, pose_init, cost_init, force_init_solve, fast_mode)
-        prob = native.Problem(x3d, x2d, w2d, camera.cam_mats, camera.lb, camera.ub, cost_fun.delta)
-        out = native.lm_solve(prob, start, self.native_params(camera, cost_fun, fast_mode), want_cov=with_pose_cov,
-                              want_cost=with_cost, want_plus=with_pose_opt_plus)
-        cast = lambda t: None if t is None else t.to(x2d.dtype)
-        return cast(out["pose_opt"]), cast(out["pose_cov"]), cast(out["cost"]), cast(out["pose_opt_plus"])
+        out = ops.lm_solve(*_problem_args(x3d, x2d, w2d, camera, cost_fun), start,
+                           *self.param_lists(camera, cost_fun, fast_mode), with_pose_cov, with_cost, with_pose_opt_plus)
+        cast = lambda t, want: t.to(x2d.dtype) if want else None
+        return (cast(out[0], True), cast(out[1], with_pose_cov), cast(out[2], with_cost),
+                cast(out[3], with_pose_opt_plus))
 
     def gn_step(self, x3d, x2d, w2d, pose, camera, cost_fun):
         """Undamped Gauss-Newton increment -(J^T J + eps I)^-1 J^T r at `pose` (levenberg_marquardt.py:243-253)."""
@@ -256,9 +262,8 @@ class RSLMSolver(LMSolver):
             # a subclass that overrides center_based_init keeps its say; otherwise the kernel computes the guess itself
             own_guess = type(self).center_based_init is not RSLMSolver.center_based_init
             t_init = self.center_based_init(x2d, x3d, camera) if own_guess else None
-            inds, start = native.rslm_draw(x3d, x2d, w2d, camera.cam_mats, P, n, self.dof, eps=self.eps, seed=seed,
-                                           t_init=t_init)
-        prob = native.Problem(x3d, x2d, w2d, camera.cam_mats, camera.lb, camera.ub, cost_fun.delta)
-        out = rslm_solve(prob, inds, start, self.native_params(camera, cost_fun, kwargs.get("fast_mode", False)),
-                         allow_split=self.cluster_split)
-        return out["pose"].to(x2d.dtype), None, out["cost"].to(x2d.dtype)
+            inds, start = ops.rslm_draw(x3d, x2d, w2d, camera.cam_mats, t_init, P, n, self.dof, float(self.eps),
+                                        *ops.seed_args(seed))
+        pose, cost = ops.rslm(*_problem_args(x3d, x2d, w2d, camera, cost_fun), inds, start,
+                              *self.param_lists(camera, cost_fun, kwargs.get("fast_mode", False)), self.cluster_split)
+        return pose.to(x2d.dtype), None, cost.to(x2d.dtype)

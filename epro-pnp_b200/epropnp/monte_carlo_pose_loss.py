@@ -21,7 +21,7 @@ import os
 import torch
 import torch.nn as nn
 
-from epropnp_b200 import native
+from epropnp_b200 import ops
 
 
 def _use_native(t):
@@ -33,24 +33,12 @@ def _object_major(t):
     return t.transpose(0, 1).contiguous()
 
 
-class _McLse(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, logw_mb):
-        bm = _object_major(logw_mb.detach())
-        lse = native.mc_epilogue(bm, want_lse=True)["lse"]
-        ctx.save_for_backward(bm, lse)
-        return lse.to(logw_mb.dtype)
-
-    @staticmethod
-    def backward(ctx, g):
-        bm, lse = ctx.saved_tensors
-        return native.mc_lse_backward(bm, lse, g.to(torch.float32)).to(g.dtype).transpose(0, 1)
-
-
 def mc_logsumexp(pose_sample_logweights):
-    """(mc_samples, num_obj) -> (num_obj,) = logsumexp over the samples (the loss's `loss_pred`)."""
+    """(mc_samples, num_obj) -> (num_obj,) = logsumexp over the samples (the loss's `loss_pred`); differentiable through
+    the epilogue operator's formula (epnp_mc_lse_backward_f32)."""
     if pose_sample_logweights.dim() == 2 and _use_native(pose_sample_logweights):
-        return _McLse.apply(pose_sample_logweights)
+        lse = ops.mc_epilogue(_object_major(pose_sample_logweights), None, None, None, True, False, False, False)[0]
+        return lse.to(pose_sample_logweights.dtype)
     return torch.logsumexp(pose_sample_logweights, dim=0)
 
 
@@ -58,8 +46,7 @@ def mc_sample_weights(pose_sample_logweights):
     """softmax over the samples, returned as an (mc_samples, num_obj) view like the log-weights themselves."""
     if pose_sample_logweights.dim() == 2 and _use_native(pose_sample_logweights) \
             and not pose_sample_logweights.requires_grad:
-        bm = _object_major(pose_sample_logweights)
-        w = native.mc_epilogue(bm, want_lse=False, want_weights=True)["weights"]
+        w = ops.mc_epilogue(_object_major(pose_sample_logweights), None, None, None, False, False, True, False)[2]
         return w.to(pose_sample_logweights.dtype).transpose(0, 1)
     return pose_sample_logweights.softmax(dim=0)
 
@@ -68,9 +55,9 @@ def mc_score_te(pose_samples, pose_opt, pose_sample_logweights):
     """Monte-Carlo 'te' score (num_obj,): expectation over the weighted samples of
     clamp((-log2 ||(x, z)_sample - (x, z)_opt|| + 2.5) / 4, 0, 1)   (deform_pnp_head.py:533-536)."""
     if pose_sample_logweights.dim() == 2 and _use_native(pose_sample_logweights):
-        out = native.mc_epilogue(_object_major(pose_sample_logweights.detach()), _object_major(pose_samples.detach()),
-                                 pose_opt.detach(), want_lse=False, want_score=True)
-        return out["score_te"].to(pose_samples.dtype)
+        out = ops.mc_epilogue(_object_major(pose_sample_logweights.detach()), _object_major(pose_samples.detach()),
+                              pose_opt.detach(), None, False, False, False, True)
+        return out[3].to(pose_samples.dtype)
     sample_dev = (pose_samples[..., [0, 2]] - pose_opt[:, [0, 2]]).norm(dim=-1)
     score = ((-sample_dev.log2() + 2.5) / 4).clamp(min=0, max=1)
     return (score * pose_sample_logweights.softmax(dim=0)).sum(dim=0)
