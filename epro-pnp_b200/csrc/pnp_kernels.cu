@@ -559,6 +559,37 @@ struct GnBwArgs {
     float* gdelta;              // [opt] (B)
 };
 
+// The serial lane of the GN-plus backward kernels: step = the damped step at the pose, v = -(H + eps I)^-1 dL/dstep.
+template <int DOF>
+__device__ __forceinline__ void gn_plus_step_and_v(const float* ev, const float* pose_sh, const float* gplus, float eps,
+                                                   float* step, float* vvec) {
+    constexpr int PD = Dim<DOF>::POSE, NA = Dim<DOF>::NA;
+    float add[DOF], st[DOF], sbar[DOF], vv[DOF], gout[PD], pose[PD];
+#pragma unroll
+    for (int i = 0; i < DOF; ++i) add[i] = eps;
+#pragma unroll
+    for (int i = 0; i < PD; ++i) { pose[i] = pose_sh[i]; gout[i] = __ldg(gplus + i); }
+    damped_step_refined<DOF>(ev, ev + NA, add, st);
+    pose_add_backward<DOF>(pose, st, gout, sbar);
+    damped_step_refined<DOF>(ev, sbar, add, vv);
+#pragma unroll
+    for (int i = 0; i < DOF; ++i) { step[i] = st[i]; vvec[i] = vv[i]; }
+}
+
+// The per-point pass's registers: R and t of the pose, step and v (step = [step, v], as the serial lane left them).
+template <int DOF>
+__device__ __forceinline__ void gn_plus_regs(const float* pose_sh, const float* step, float (&R)[9], float (&t)[3],
+                                             float (&sv)[DOF], float (&vv)[DOF]) {
+    constexpr int PD = Dim<DOF>::POSE;
+    float ps[PD];
+#pragma unroll
+    for (int i = 0; i < PD; ++i) ps[i] = pose_sh[i];
+    pose_to_rot<DOF>(ps, R);
+    t[0] = ps[0]; t[1] = ps[1]; t[2] = ps[2];
+#pragma unroll
+    for (int i = 0; i < DOF; ++i) { sv[i] = step[i]; vv[i] = step[DOF + i]; }
+}
+
 template <int DOF>
 __global__ void __launch_bounds__(NT, 2) gn_plus_backward_kernel(const GnBwArgs g) {
     const KArgs& a = g.k;
@@ -567,7 +598,7 @@ __global__ void __launch_bounds__(NT, 2) gn_plus_backward_kernel(const GnBwArgs 
     float* dyn = reinterpret_cast<float*>(smem_raw);
     const ObjPlan pl = plan_obj<DOF>(a.N);
     float* pts = dyn + pl.pts;
-    constexpr int PD = Dim<DOF>::POSE, NA = Dim<DOF>::NA;
+    constexpr int PD = Dim<DOF>::POSE;
     const int tid = threadIdx.x, obj = blockIdx.x;
     Loader ld(a, sh.bar, dyn + pl.stage);
     ld.load_object(obj, pts);
@@ -576,31 +607,10 @@ __global__ void __launch_bounds__(NT, 2) gn_plus_backward_kernel(const GnBwArgs 
     if (tid < PD) sh.pose[tid] = __ldg(a.poses + (size_t)obj * PD + tid);
     __syncthreads();
     eval_normal_eq<DOF, true>(pts, a.N, sh.pose, cam, delta, a.p.huber_eps, sh.red, sh.ev);
-    float* step = sh.step;              // [DOF]
-    float* vvec = sh.step + DOF;        // [DOF]
-    if (tid == 0) {
-        float add[DOF], st[DOF], sbar[DOF], vv[DOF], gout[PD], pose[PD];
-#pragma unroll
-        for (int i = 0; i < DOF; ++i) add[i] = a.p.eps;
-#pragma unroll
-        for (int i = 0; i < PD; ++i) { pose[i] = sh.pose[i]; gout[i] = __ldg(g.gplus + (size_t)obj * PD + i); }
-        damped_step_refined<DOF>(sh.ev, sh.ev + NA, add, st);
-        pose_add_backward<DOF>(pose, st, gout, sbar);
-        damped_step_refined<DOF>(sh.ev, sbar, add, vv);
-#pragma unroll
-        for (int i = 0; i < DOF; ++i) { step[i] = st[i]; vvec[i] = vv[i]; }
-    }
+    if (tid == 0) gn_plus_step_and_v<DOF>(sh.ev, sh.pose, g.gplus + (size_t)obj * PD, a.p.eps, sh.step, sh.step + DOF);
     __syncthreads();
     float R[9], t[3], sv[DOF], vv[DOF];
-    {
-        float ps[PD];
-#pragma unroll
-        for (int i = 0; i < PD; ++i) ps[i] = sh.pose[i];
-        pose_to_rot<DOF>(ps, R);
-        t[0] = ps[0]; t[1] = ps[1]; t[2] = ps[2];
-#pragma unroll
-        for (int i = 0; i < DOF; ++i) { sv[i] = step[i]; vv[i] = vvec[i]; }
-    }
+    gn_plus_regs<DOF>(sh.pose, sh.step, R, t, sv, vv);
     float gd[1] = {0.f};
     for (int n = tid; n < a.N; n += NT) {
         const float* q = pts + (n >> 1) * 16 + (n & 1);
@@ -1288,39 +1298,13 @@ struct GnCamBwArgs {
     float *gcam, *glb, *gub;    // [opt] (B, 3, 3), (B, 2), (B, 2)
 };
 
-// The serial lane of both GN-plus camera kernels: step = the damped step at the pose, v = -(H + eps I)^-1 dL/dstep.
-template <int DOF>
-__device__ __forceinline__ void gn_plus_step_and_v(const float* ev, const float* pose_sh, const float* gplus, float eps,
-                                                   float* step, float* vvec) {
-    constexpr int PD = Dim<DOF>::POSE, NA = Dim<DOF>::NA;
-    float add[DOF], st[DOF], sbar[DOF], vv[DOF], gout[PD], pose[PD];
-#pragma unroll
-    for (int i = 0; i < DOF; ++i) add[i] = eps;
-#pragma unroll
-    for (int i = 0; i < PD; ++i) { pose[i] = pose_sh[i]; gout[i] = __ldg(gplus + i); }
-    damped_step_refined<DOF>(ev, ev + NA, add, st);
-    pose_add_backward<DOF>(pose, st, gout, sbar);
-    damped_step_refined<DOF>(ev, sbar, add, vv);
-#pragma unroll
-    for (int i = 0; i < DOF; ++i) { step[i] = st[i]; vvec[i] = vv[i]; }
-}
-
 // acc += the camera gradient of the points [0, cnt) of the pair records, thread tid of T.
 template <int DOF, int T>
 __device__ __forceinline__ void gn_plus_camera_points(const float* pts, int cnt, const float* pose_sh, const float* step,
                                                       const Cam& cam, float delta, float huber_eps,
                                                       float (&acc)[CAM_GRADS]) {
-    constexpr int PD = Dim<DOF>::POSE;
     float R[9], t[3], sv[DOF], vv[DOF];
-    {
-        float ps[PD];
-#pragma unroll
-        for (int i = 0; i < PD; ++i) ps[i] = pose_sh[i];
-        pose_to_rot<DOF>(ps, R);
-        t[0] = ps[0]; t[1] = ps[1]; t[2] = ps[2];
-#pragma unroll
-        for (int i = 0; i < DOF; ++i) { sv[i] = step[i]; vv[i] = step[DOF + i]; }
-    }
+    gn_plus_regs<DOF>(pose_sh, step, R, t, sv, vv);
     for (int n = threadIdx.x; n < cnt; n += T) {
         const float* q = pts + (n >> 1) * 16 + (n & 1);
         gn_step_point_camera_backward<DOF>(R, t, cam, delta, huber_eps, q[0], q[2], q[4], -q[6], -q[8], q[10], q[12], vv,
