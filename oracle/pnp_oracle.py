@@ -331,10 +331,12 @@ def acg_draw(normal4, L, eps=1e-6):
 
 # ----------------------------------------------------------------------------- AMIS (6DoF)
 def amis_6dof(x3d, x2d, w2d, cam: Camera, delta, pose_opt, pose_cov, noise, mc_samples=512,
-              num_iter=4, eps=1e-5, acg_mle_iter=3, acg_dispersion=1e-3):
+              num_iter=4, eps=1e-5, acg_mle_iter=3, acg_dispersion=1e-3, return_refit=False):
     """noise = (normal3 (I,S,B,3), chi2 (I,S,B), normal4 (I,S,B,4)).
     Returns dict(samples (M,B,7), logw (M,B), trans_mode (I,B,3), trans_tril (I,B,3,3),
-    rot_tril (I,B,4,4), cost (I,S,B))."""
+    rot_tril (I,B,4,4), cost (I,S,B)).  return_refit: also refit_trans (I-1,B,3,3) and refit_rot (I-1,B,4,4), the
+    matrices each refit hands to robust_cholesky (the weighted translation covariance; the dispersed ACG scatter), and
+    refit_logw, per refit the log-weights ((i+1)S,B) it weighs the samples by."""
     n3, c2, n4 = noise
     I, S = num_iter, mc_samples // num_iter
     B, dt = x3d.shape[0], x3d.dtype
@@ -343,8 +345,10 @@ def amis_6dof(x3d, x2d, w2d, cam: Camera, delta, pose_opt, pose_cov, noise, mc_s
     Lt = torch.zeros(I, B, 3, 3, dtype=dt)
     Lr = torch.zeros(I, B, 4, 4, dtype=dt)
 
-    def dispersed_chol(c):
-        return robust_cholesky(c + torch.linalg.det(c)[:, None, None] ** 0.25 * (acg_dispersion * eye4))
+    refit_t, refit_r, refit_w = [], [], []
+
+    def dispersed(c):
+        return c + torch.linalg.det(c)[:, None, None] ** 0.25 * (acg_dispersion * eye4)
 
     # proposal 0 from the local solution and its covariance
     mode[0] = pose_opt[:, :3]
@@ -352,7 +356,7 @@ def amis_6dof(x3d, x2d, w2d, cam: Camera, delta, pose_opt, pose_cov, noise, mc_s
     T = quat_tangent_map(pose_opt[:, 3:])
     rc = torch.linalg.inv(T @ torch.linalg.inv(pose_cov[:, 3:, 3:]) @ T.transpose(-1, -2) + eye4)
     rc = rc / rc.diagonal(dim1=-2, dim2=-1).sum(-1)[:, None, None]
-    Lr[0] = dispersed_chol(rc)
+    Lr[0] = robust_cholesky(dispersed(rc))
 
     samples = torch.zeros(I, S, B, 7, dtype=dt)
     cost = torch.zeros(I, S, B, dtype=dt)
@@ -373,12 +377,14 @@ def amis_6dof(x3d, x2d, w2d, cam: Camera, delta, pose_opt, pose_cov, noise, mc_s
         if i == I - 1:
             break
         # refit the next proposal to the weighted samples
-        w = torch.softmax(logw.reshape(-1, B), dim=0)              # (n, B)
+        refit_w.append(logw.reshape(-1, B))
+        w = torch.softmax(refit_w[-1], dim=0)                       # (n, B)
         smp = samples[:i + 1].reshape(-1, B, 7)
         t, q = smp[..., :3], smp[..., 3:]
         mode[i + 1] = (w[..., None] * t).sum(0)
         dev = t - mode[i + 1]
-        Lt[i + 1] = robust_cholesky((w[..., None, None] * dev[..., :, None] * dev[..., None, :]).sum(0))
+        refit_t.append((w[..., None, None] * dev[..., :, None] * dev[..., None, :]).sum(0))
+        Lt[i + 1] = robust_cholesky(refit_t[-1])
         qq = q[..., :, None] * q[..., None, :]
         lam = eye4.expand(B, 4, 4).clone()
         for _ in range(acg_mle_iter):
@@ -386,9 +392,15 @@ def amis_6dof(x3d, x2d, w2d, cam: Camera, delta, pose_opt, pose_cov, noise, mc_s
             wm = w / m.clamp(min=eps)
             wm = wm / wm.sum(0)
             lam = (wm[..., None, None] * qq).sum(0) + eps * eye4
-        Lr[i + 1] = dispersed_chol(lam)
-    return dict(samples=samples.reshape(I * S, B, 7), logw=logw.reshape(I * S, B), trans_mode=mode,
-                trans_tril=Lt, rot_tril=Lr, cost=cost)
+        refit_r.append(dispersed(lam))
+        Lr[i + 1] = robust_cholesky(refit_r[-1])
+    out = dict(samples=samples.reshape(I * S, B, 7), logw=logw.reshape(I * S, B), trans_mode=mode,
+               trans_tril=Lt, rot_tril=Lr, cost=cost)
+    if return_refit:
+        out.update(refit_trans=torch.stack(refit_t) if refit_t else torch.zeros(0, B, 3, 3, dtype=dt),
+                   refit_rot=torch.stack(refit_r) if refit_r else torch.zeros(0, B, 4, 4, dtype=dt),
+                   refit_logw=refit_w)
+    return out
 
 
 def monte_carlo_forward_6dof(x3d, x2d, w2d, cam: Camera, delta, pose_init, noise, mc_samples=512,
@@ -427,9 +439,12 @@ def vm_mix_logpdf(yaw, loc, kappa, uniform_mix=0.25):
     return torch.logaddexp(vm, torch.full_like(vm, math.log(uniform_mix / (2 * math.pi))))
 
 
-def amis_4dof(x3d, x2d, w2d, cam: Camera, delta, pose_opt, pose_cov, noise, mc_samples=512, num_iter=4, eps=1e-5):
+def amis_4dof(x3d, x2d, w2d, cam: Camera, delta, pose_opt, pose_cov, noise, mc_samples=512, num_iter=4, eps=1e-5,
+              return_refit=False):
     """noise = (normal3 (I,S,B,3), chi2 (I,S,B), yaw draws (I,S,B)) -- the reference draws yaw with numpy on
-    the host, so the draws themselves are the injected quantity.  Returns samples (M,B,4), logw (M,B), ..."""
+    the host, so the draws themselves are the injected quantity.  Returns samples (M,B,4), logw (M,B), ...
+    return_refit: also refit_trans (I-1,B,3,3), the matrix each refit hands to robust_cholesky, and refit_logw, per
+    refit the log-weights ((i+1)S,B) it weighs the samples by."""
     n3, c2, yaw = noise
     I, S = num_iter, mc_samples // num_iter
     B, dt = x3d.shape[0], x3d.dtype
@@ -446,6 +461,7 @@ def amis_4dof(x3d, x2d, w2d, cam: Camera, delta, pose_opt, pose_cov, noise, mc_s
     cost = torch.zeros(I, S, B, dtype=dt)
     logp = torch.zeros(I, I, S, B, dtype=dt)
     logw = None
+    refit_t, refit_w = [], []
     for i in range(I):
         samples[i, ..., :3] = mvt_draw(n3[i], c2[i], mode[i], Lt[i])
         samples[i, ..., 3] = yaw[i]
@@ -459,16 +475,21 @@ def amis_4dof(x3d, x2d, w2d, cam: Camera, delta, pose_opt, pose_cov, noise, mc_s
         logw = -cost[:i + 1] - mix
         if i == I - 1:
             break
-        w = torch.softmax(logw.reshape(-1, B), dim=0)
+        refit_w.append(logw.reshape(-1, B))
+        w = torch.softmax(refit_w[-1], dim=0)
         smp = samples[:i + 1].reshape(-1, B, 4)
         t = smp[..., :3]
         mode[i + 1] = (w[..., None] * t).sum(0)
         dev = t - mode[i + 1]
-        Lt[i + 1] = robust_cholesky((w[..., None, None] * dev[..., :, None] * dev[..., None, :]).sum(0), dd)
+        refit_t.append((w[..., None, None] * dev[..., :, None] * dev[..., None, :]).sum(0))
+        Lt[i + 1] = robust_cholesky(refit_t[-1], dd)
         s_sum = (w * smp[..., 3].sin()).sum(0)
         c_sum = (w * smp[..., 3].cos()).sum(0)
         rmode[i + 1] = torch.atan2(s_sum, c_sum)
         r_sq = s_sum ** 2 + c_sum ** 2
         kappa[i + 1] = 0.33 * r_sq.sqrt().clamp(min=eps) * (2 - r_sq) / (1 - r_sq).clamp(min=eps)
-    return dict(samples=samples.reshape(I * S, B, 4), logw=logw.reshape(I * S, B), trans_mode=mode, trans_tril=Lt,
-                rot_mode=rmode, rot_kappa=kappa, cost=cost)
+    out = dict(samples=samples.reshape(I * S, B, 4), logw=logw.reshape(I * S, B), trans_mode=mode, trans_tril=Lt,
+               rot_mode=rmode, rot_kappa=kappa, cost=cost)
+    if return_refit:
+        out.update(refit_trans=torch.stack(refit_t) if refit_t else torch.zeros(0, B, 3, 3, dtype=dt), refit_logw=refit_w)
+    return out
