@@ -2226,14 +2226,15 @@ int split_ctas_for(int dof, int N, int mc_samples, int mc_iter, int requested) {
 
 unsigned long long* g_prof_buffer = nullptr;     // set by epnp_debug_set_phase_buffer (profiling build)
 
-// Objects the device works on at once in the AMIS kernel: SMs x resident CTAs per SM.  Used by the host-buffer entry
-// point to cut the batch at whole waves.  0 when it cannot be determined.
+// Objects the device works on at once in a CTA-per-object kernel: SMs x resident CTAs per SM.  Used by the host-buffer
+// entry points to cut the batch at whole waves.  `attr`: what the kernel's own launch sets.  0 when it cannot be
+// determined.
 template <int T, class Kern>
-int resident_objects(Kern kern, int smem_bytes) {
+int resident_objects(Kern kern, int smem_bytes, SmemAttr attr = SmemAttr::size_and_carveout) {
     int sms = 0, occ = 0;
     if ((size_t)smem_bytes > SMEM_LIMIT) return 0;
     if (device_sms(&sms) != EPNP_OK) return 0;
-    if (set_smem_attr(kern, smem_bytes, SmemAttr::size_and_carveout) != cudaSuccess) return 0;
+    if (set_smem_attr(kern, smem_bytes, attr) != cudaSuccess) return 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, T, smem_bytes) != cudaSuccess) return 0;
     return sms * occ;
 }
@@ -2652,6 +2653,12 @@ int epnp_rslm_split_f32(const float* x3d, const float* x2d, const float* w2d, co
     });
 }
 
+// The draw kernel's shared memory: the weights (N rounded up to 4), n indices and floats per thread.  With its 2 KB of
+// static shared memory it must fit SMEM_LIMIT.
+static size_t rslm_draw_smem(int N, int n) {
+    return (size_t)((N + 3) & ~3) * sizeof(float) + (size_t)n * NT * (sizeof(float) + sizeof(int));
+}
+
 // epnp_rslm_draw_f32 and, with seed_ptr != NULL, epnp_rslm_draw_seedptr_f32 (the seed then comes from *seed_ptr).
 static int rslm_draw(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats, const float* t_init,
                      uint64_t seed, const uint64_t* seed_ptr, uint32_t obj_offset, int* inds, float* start, float* t_out,
@@ -2660,7 +2667,7 @@ static int rslm_draw(const float* x3d, const float* x2d, const float* w2d, const
         return EPNP_ERR_BAD_ARG;
     if (!t_init && (!x3d || !x2d || !cam_mats)) return EPNP_ERR_BAD_ARG;
     if (B == 0) return EPNP_OK;
-    const size_t smem = (size_t)((N + 3) & ~3) * sizeof(float) + (size_t)n * NT * (sizeof(float) + sizeof(int));
+    const size_t smem = rslm_draw_smem(N, n);
     if (smem + 2048 > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
     const RslmDrawArgs r{x3d, x2d, w2d, cam_mats, t_init, inds, start, t_out, seed, obj_offset, P, n, B, N, eps};
     const cudaStream_t s = (cudaStream_t)stream;
@@ -3016,15 +3023,23 @@ int epnp_evaluate_backward_f32(const float* x3d, const float* x2d, const float* 
     });
 }
 
-// ---- host-buffer entry point: chunked H2D -> fused kernel -> D2H on two internal streams
-static size_t align256(size_t x) { return (x + 255) / 256 * 256; }
+}  // extern "C"
+
+// ---- host-buffer entry points: chunked H2D -> solve -> D2H on two internal streams
+namespace {
+
+size_t align256(size_t x) { return (x + 255) / 256 * 256; }
 
 struct WsLayout {
-    size_t x3d, x2d, w2d, cam, lb, ub, delta, pose_init, pose_opt, pose_cov, cost, samples, logw, total;
+    size_t x3d, x2d, w2d, cam, lb, ub, delta, pose_init, pose_opt, pose_cov, cost, samples, logw;
+    size_t inds, start, pose_all, cost_all, cost_best;   // the RSLM initialiser's (P, B, .) and (B) scratch
+    size_t P, n, total;                                  // P = n = 0 without it
 };
 
-static WsLayout ws_layout(int B, int N, const EpnpParams* p) {
+// init [opt]: the initialiser of epnp_solve_host_f32; without it (the fused host calls) the layout ends at logw.
+WsLayout ws_layout(int B, int N, const EpnpParams* p, const EpnpInit* init = nullptr) {
     const size_t D = (p->dof == 6) ? 7 : 4, dof = p->dof, M = p->mc_samples;
+    const bool rslm = init && init->kind == EPNP_INIT_RSLM;
     WsLayout w; size_t o = 0;
     w.x3d = o; o += align256((size_t)B * N * 3 * 4);
     w.x2d = o; o += align256((size_t)B * N * 2 * 4);
@@ -3039,16 +3054,18 @@ static WsLayout ws_layout(int B, int N, const EpnpParams* p) {
     w.cost = o; o += align256((size_t)B * 4);
     w.samples = o; o += align256((size_t)B * M * D * 4);
     w.logw = o; o += align256((size_t)B * M * 4);
+    w.P = rslm && init->num_proposals > 0 ? (size_t)init->num_proposals : 0;
+    w.n = rslm && init->num_points > 0 ? (size_t)init->num_points : 0;
+    w.inds = o; o += align256(w.P * B * w.n * 4);
+    w.start = o; o += align256(w.P * B * D * 4);
+    w.pose_all = o; o += align256(w.P * B * D * 4);
+    w.cost_all = o; o += align256(w.P * B * 4);
+    w.cost_best = o; o += align256(rslm ? (size_t)B * 4 : 0);
     w.total = o;
     return w;
 }
 
-size_t epnp_fused_workspace_bytes(int B, int N, const EpnpParams* p) {
-    if (!p || B < 0 || N <= 0) return 0;
-    return ws_layout(B, N, p).total;
-}
-
-// Helper streams of the host-buffer entry point: one copy-in, two compute, one copy-out stream per host
+// Helper streams of the host-buffer entry points: one copy-in, two compute, one copy-out stream per host
 // thread, created on first use and kept for the life of the thread (the only resource the library owns;
 // creating and destroying four streams per call costs more than a whole chunk of work).
 struct HostPipe {
@@ -3068,49 +3085,71 @@ struct HostPipe {
         return cudaSuccess;
     }
 };
-static thread_local HostPipe g_pipe;
+thread_local HostPipe g_pipe;
 
-// The argument checks both host-buffer calls make first: EPNP_OK or EPNP_ERR_BAD_ARG.
-static int check_host_args(const float* x3d_host, const float* x2d_host, const float* w2d_host,
-                           const float* cam_mats_host, const float* lb_host, const float* ub_host,
-                           const float* delta_host, const float* pose_init_host, float* pose_opt_host, float* logw_host,
-                           void* workspace, size_t workspace_bytes, int B, int N, const EpnpParams* p) {
-    if (!p || !workspace || !x3d_host || !x2d_host || !w2d_host || !cam_mats_host || !delta_host || !pose_init_host ||
-        !pose_opt_host || !logw_host)
+// The caller's host arrays of a host-buffer call.
+struct HostBufs {
+    const float *x3d, *x2d, *w2d, *cam, *lb, *ub, *delta, *pose_init;     // lb / ub, pose_init [opt]
+    float *pose_opt, *pose_cov, *cost, *samples, *logw;                     // all but pose_opt [opt]
+};
+
+// One chunk's rows [b0, b0 + nb) of every workspace array, the global index of its first object and its stream.
+struct Chunk {
+    const float *x3d, *x2d, *w2d, *cam, *lb, *ub, *delta;
+    float *pose_init, *pose_opt, *pose_cov, *cost, *samples, *logw;
+    int* inds;
+    float *start, *pose_all, *cost_all, *cost_best;
+    uint32_t obj_offset;
+    int nb;
+    cudaStream_t stream;
+};
+
+Chunk chunk_at(char* ws, const WsLayout& w, int b0, int nb, int N, const EpnpParams* p, bool bounded,
+                      uint32_t obj_offset, cudaStream_t stream) {
+    const size_t D = (p->dof == 6) ? 7 : 4, dof = p->dof, M = p->mc_samples, b = (size_t)b0;
+    const auto at = [&](size_t field, size_t per) { return (float*)(ws + field) + b * per; };
+    Chunk c;
+    c.x3d = at(w.x3d, (size_t)N * 3); c.x2d = at(w.x2d, (size_t)N * 2); c.w2d = at(w.w2d, (size_t)N * 2);
+    c.cam = at(w.cam, 9); c.delta = at(w.delta, 1);
+    c.lb = bounded ? at(w.lb, 2) : nullptr; c.ub = bounded ? at(w.ub, 2) : nullptr;
+    c.pose_init = at(w.pose_init, D); c.pose_opt = at(w.pose_opt, D); c.pose_cov = at(w.pose_cov, dof * dof);
+    c.cost = at(w.cost, 1); c.samples = at(w.samples, M * D); c.logw = at(w.logw, M);
+    c.inds = (int*)at(w.inds, w.P * w.n); c.start = at(w.start, w.P * D); c.pose_all = at(w.pose_all, w.P * D);
+    c.cost_all = at(w.cost_all, w.P); c.cost_best = at(w.cost_best, 1);
+    c.obj_offset = obj_offset + (uint32_t)b0;
+    c.nb = nb;
+    c.stream = stream;
+    return c;
+}
+
+// The argument checks both fused host-buffer calls make first: EPNP_OK or EPNP_ERR_BAD_ARG.
+int check_host_args(const HostBufs& h, void* workspace, size_t workspace_bytes, int B, int N, const EpnpParams* p) {
+    if (!p || !workspace || !h.x3d || !h.x2d || !h.w2d || !h.cam || !h.delta || !h.pose_init || !h.pose_opt || !h.logw)
         return EPNP_ERR_BAD_ARG;
-    if ((lb_host == nullptr) != (ub_host == nullptr)) return EPNP_ERR_BAD_ARG;
+    if ((h.lb == nullptr) != (h.ub == nullptr)) return EPNP_ERR_BAD_ARG;
     if (B < 0 || N <= 0) return EPNP_ERR_BAD_ARG;
     if (workspace_bytes < ws_layout(B, N, p).total) return EPNP_ERR_BAD_ARG;
     return EPNP_OK;
 }
 
-// The solve of one chunk: epnp_lm_amis_fused_split_f32's arguments; the resident form ignores cluster_ctas.
-using ChunkSolve = decltype(&epnp_lm_amis_fused_split_f32);
-static int fused_resident_chunk(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
-                                const float* lb, const float* ub, const float* delta, const float* pose_init,
-                                const float* noise_normal, const float* noise_chi2, const float* noise_rot,
-                                uint64_t seed, uint32_t obj_offset,
-                                float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus, float* cost_init,
-                                float* pose_samples, float* logw, float* proposals,
-                                int B, int N, const EpnpParams* p, int, void* stream) {
-    return epnp_lm_amis_fused_f32(x3d, x2d, w2d, cam_mats, lb, ub, delta, pose_init, noise_normal, noise_chi2, noise_rot,
-                                  seed, obj_offset, pose_opt, pose_cov, cost, pose_opt_plus, cost_init, pose_samples, logw,
-                                  proposals, B, N, p, stream);
+// LM + AMIS on one chunk: epnp_lm_amis_fused_f32, or its split form with cluster_ctas.
+int lm_amis_chunk(const Chunk& c, uint64_t seed, int N, const EpnpParams* p, bool split, int cluster_ctas) {
+    if (split)
+        return epnp_lm_amis_fused_split_f32(c.x3d, c.x2d, c.w2d, c.cam, c.lb, c.ub, c.delta, c.pose_init, nullptr, nullptr,
+                                            nullptr, seed, c.obj_offset, c.pose_opt, c.pose_cov, c.cost, nullptr, nullptr,
+                                            c.samples, c.logw, nullptr, c.nb, N, p, cluster_ctas, c.stream);
+    return epnp_lm_amis_fused_f32(c.x3d, c.x2d, c.w2d, c.cam, c.lb, c.ub, c.delta, c.pose_init, nullptr, nullptr, nullptr,
+                                  seed, c.obj_offset, c.pose_opt, c.pose_cov, c.cost, nullptr, nullptr, c.samples, c.logw,
+                                  nullptr, c.nb, N, p, c.stream);
 }
 
-// The chunked copy-in / solve / copy-out pipeline of the host-buffer calls, after their checks (B > 0): `solve` with
-// `ctas` on every chunk.  n_chunks = 0: cut the batch at whole waves of `wave` objects the device solves at once (a
-// chunk of 1.7 waves costs 2), as few waves per chunk as the 64-chunk limit allows (one chunk when wave = 0);
-// n_chunks >= 1: that many equal chunks.
-static int host_pipeline(ChunkSolve solve, int ctas, int wave,
-                         const float* x3d_host, const float* x2d_host, const float* w2d_host,
-                         const float* cam_mats_host, const float* lb_host, const float* ub_host,
-                         const float* delta_host, const float* pose_init_host,
-                         uint64_t seed, uint32_t obj_offset,
-                         float* pose_opt_host, float* pose_cov_host, float* cost_host,
-                         float* pose_samples_host, float* logw_host,
-                         void* workspace, int n_chunks, int B, int N, const EpnpParams* p, void* stream_) {
-    const WsLayout w = ws_layout(B, N, p);
+// The chunked copy-in / solve / copy-out pipeline of the host-buffer calls, after their checks (B > 0): solve(chunk)
+// enqueues a chunk's work on chunk.stream.  n_chunks = 0: cut the batch at whole waves of `wave` objects the device
+// solves at once (a chunk of 1.7 waves costs 2), as few waves per chunk as the 64-chunk limit allows (one chunk when
+// wave = 0); n_chunks >= 1: that many equal chunks.  h.pose_init and h.logw are copied only when given.
+template <class Solve>
+int host_pipeline(Solve solve, int wave, const HostBufs& h, void* workspace, const WsLayout& w,
+                         uint32_t obj_offset, int n_chunks, int B, int N, const EpnpParams* p, void* stream_) {
     int chunk_objects = 0;
     if (n_chunks == 0) {
         if (wave > 0) {
@@ -3148,30 +3187,23 @@ static int host_pipeline(ChunkSolve solve, int ctas, int wave,
         cudaStream_t sk = g_pipe.k[c & 1];
 #define H2D(field, host, per) EPNP_TRY(cudaMemcpyAsync(ws + w.field + (size_t)b0 * (per) * 4, (host) + (size_t)b0 * (per), (size_t)nb * (per) * 4, cudaMemcpyHostToDevice, g_pipe.in))
 #define D2H(field, host, per) EPNP_TRY(cudaMemcpyAsync((host) + (size_t)b0 * (per), ws + w.field + (size_t)b0 * (per) * 4, (size_t)nb * (per) * 4, cudaMemcpyDeviceToHost, g_pipe.out))
-        H2D(x3d, x3d_host, (size_t)N * 3); H2D(x2d, x2d_host, (size_t)N * 2); H2D(w2d, w2d_host, (size_t)N * 2);
-        H2D(cam, cam_mats_host, 9); H2D(delta, delta_host, 1); H2D(pose_init, pose_init_host, D);
-        if (lb_host) { H2D(lb, lb_host, 2); H2D(ub, ub_host, 2); }
+        H2D(x3d, h.x3d, (size_t)N * 3); H2D(x2d, h.x2d, (size_t)N * 2); H2D(w2d, h.w2d, (size_t)N * 2);
+        H2D(cam, h.cam, 9); H2D(delta, h.delta, 1);
+        if (h.pose_init) H2D(pose_init, h.pose_init, D);
+        if (h.lb) { H2D(lb, h.lb, 2); H2D(ub, h.ub, 2); }
         EPNP_TRY(cudaEventCreateWithFlags(&ev_in[c], cudaEventDisableTiming));
         EPNP_TRY(cudaEventRecord(ev_in[c], g_pipe.in));
         EPNP_TRY(cudaStreamWaitEvent(sk, ev_in[c], 0));
-        rc = solve(
-            (float*)(ws + w.x3d) + (size_t)b0 * N * 3, (float*)(ws + w.x2d) + (size_t)b0 * N * 2,
-            (float*)(ws + w.w2d) + (size_t)b0 * N * 2, (float*)(ws + w.cam) + (size_t)b0 * 9,
-            lb_host ? (float*)(ws + w.lb) + (size_t)b0 * 2 : nullptr, lb_host ? (float*)(ws + w.ub) + (size_t)b0 * 2 : nullptr,
-            (float*)(ws + w.delta) + b0, (float*)(ws + w.pose_init) + (size_t)b0 * D,
-            nullptr, nullptr, nullptr, seed, obj_offset + (uint32_t)b0,
-            (float*)(ws + w.pose_opt) + (size_t)b0 * D, (float*)(ws + w.pose_cov) + (size_t)b0 * dof * dof,
-            (float*)(ws + w.cost) + b0, nullptr, nullptr,
-            (float*)(ws + w.samples) + (size_t)b0 * M * D, (float*)(ws + w.logw) + (size_t)b0 * M, nullptr,
-            nb, N, p, ctas, sk);
+        rc = solve(chunk_at(ws, w, b0, nb, N, p, h.lb != nullptr, obj_offset, sk));
         if (rc != EPNP_OK) goto done;
         EPNP_TRY(cudaEventCreateWithFlags(&ev_k[c], cudaEventDisableTiming));
         EPNP_TRY(cudaEventRecord(ev_k[c], sk));
         EPNP_TRY(cudaStreamWaitEvent(g_pipe.out, ev_k[c], 0));
-        D2H(pose_opt, pose_opt_host, D); D2H(logw, logw_host, M);
-        if (pose_cov_host) D2H(pose_cov, pose_cov_host, dof * dof);
-        if (cost_host) D2H(cost, cost_host, 1);
-        if (pose_samples_host) D2H(samples, pose_samples_host, M * D);
+        D2H(pose_opt, h.pose_opt, D);
+        if (h.logw) D2H(logw, h.logw, M);
+        if (h.pose_cov) D2H(pose_cov, h.pose_cov, dof * dof);
+        if (h.cost) D2H(cost, h.cost, 1);
+        if (h.samples) D2H(samples, h.samples, M * D);
 #undef H2D
 #undef D2H
     }
@@ -3192,6 +3224,163 @@ done:
     return rc;
 }
 
+// ---- host-buffer solve from a given pose or from scratch (epnp_solve_host_f32, epnp_solve_split_host_f32)
+
+// What the two calls compose on every chunk.
+struct SolveSpec {
+    const EpnpInit* init;                       // [opt]: NULL when the caller gives pose_init
+    uint64_t seed;                              // the AMIS seed
+    const EpnpParams* p;
+    int N;
+    bool split;
+    int cluster_ctas;                           // as the caller gave it: 0 lets each split stage pick its own C
+    bool want_cov, want_cost;                   // LM only: passed to epnp_lm_solve_f32 when the caller asked
+};
+
+// The refusals of the composed device calls that only a non-empty batch gets -- a resident launch's shared memory, a
+// cluster the device cannot co-schedule -- checked without launching, and `wave`: the objects the heaviest stage
+// (the AMIS kernel, else the initialiser's) solves at once, asked for when n_chunks = 0.
+struct SolvePlan {
+    int B;
+    bool want_wave;
+    int wave;
+};
+
+int plan_rslm(const SolveSpec& s, SolvePlan& plan) {
+    const int dof = s.p->dof, N = s.N;
+    int* wave = plan.want_wave ? &plan.wave : nullptr;
+    if (rslm_draw_smem(N, s.init->num_points) + 2048 > SMEM_LIMIT) return EPNP_ERR_TOO_MANY_POINTS;
+    return by_dof(dof, [&](auto D) {
+        if (!s.split) {
+            const int smem_bytes = plan_obj<D>(N).total_bytes;
+            if ((size_t)smem_bytes > SMEM_LIMIT) return (int)EPNP_ERR_TOO_MANY_POINTS;
+            if (wave) *wave = resident_objects<NT>(rslm_kernel<D>, smem_bytes, SmemAttr::size);
+            return (int)EPNP_OK;
+        }
+        const int ctas = split_ctas_for(dof, N, 0, 0, s.cluster_ctas);
+        KArgs unused{};                         // launch = false: launch_cluster does not read the kernel's arguments
+        return launch_cluster<COST_SPLIT_TILE>(cost_split_kernel<D>, unused, plan.B, split_smem_bytes(dof, N, ctas, 0, 0),
+                                               ctas, nullptr, false, wave);
+    });
+}
+
+int plan_epnp(const SolveSpec& s, SolvePlan& plan) {
+    int* wave = plan.want_wave ? &plan.wave : nullptr;
+    if (!s.split) {
+        if (wave) *wave = resident_objects<NT>(epnp_init_kernel, epnp_init_smem_bytes(s.N), SmemAttr::size);
+        return EPNP_OK;
+    }
+    const int ctas = split_ctas_for(6, s.N, 0, 0, s.cluster_ctas);
+    EpnpInitArgs unused{};
+    return launch_cluster<EPNP_SPLIT_T>(epnp_init_split_kernel, unused, plan.B, epnp_split_smem_bytes(split_share(s.N, ctas)),
+                                        ctas, nullptr, false, wave);
+}
+
+int plan_amis(const SolveSpec& s, SolvePlan& plan) {
+    const EpnpParams& p = *s.p;
+    if (s.split) {
+        int wave = 0;
+        const int ctas = split_lm_amis_plan(p, plan.B, s.N, s.cluster_ctas, &wave);
+        if (plan.want_wave) plan.wave = wave;
+        return ctas < 0 ? ctas : EPNP_OK;
+    }
+    if (plan.want_wave)
+        plan.wave = by_dof(p.dof, [&](auto D) {
+            return by_amis_threads(s.N, [&](auto T) {
+                return resident_objects<T>(amis_kernel<D, T>, amis_smem_bytes<D>(s.N, p.mc_samples));
+            });
+        });
+    return EPNP_OK;
+}
+
+// One chunk of the composed solve, stage by stage, each a public device call on chunk c.  With `plan` (c.nb = 0, a dry
+// run that enqueues nothing) every call returns what it refuses for an empty batch, and, when plan->B > 0, the stage's
+// plan adds what it refuses only for a non-empty one: the first refusal is the one the composition would meet.
+int solve_chunk(const SolveSpec& s, const Chunk& c, SolvePlan* plan) {
+    const EpnpInit* in = s.init;
+    const EpnpParams* p = s.p;
+    const bool check = plan && plan->B > 0;
+    int rc = EPNP_OK;
+    if (in && in->kind == EPNP_INIT_RSLM) {
+        const int P = in->num_proposals, n = in->num_points;
+        rc = epnp_rslm_draw_f32(c.x3d, c.x2d, c.w2d, c.cam, nullptr, in->seed, c.obj_offset, c.inds, c.start, nullptr, P,
+                                n, c.nb, s.N, p->dof, in->rslm.eps, c.stream);
+        if (rc != EPNP_OK) return rc;
+        rc = s.split ? epnp_rslm_split_f32(c.x3d, c.x2d, c.w2d, c.cam, c.lb, c.ub, c.delta, c.inds, c.start, c.pose_init,
+                                           c.cost_best, c.pose_all, c.cost_all, P, n, c.nb, s.N, &in->rslm,
+                                           s.cluster_ctas, c.stream)
+                     : epnp_rslm_f32(c.x3d, c.x2d, c.w2d, c.cam, c.lb, c.ub, c.delta, c.inds, c.start, c.pose_init,
+                                     c.cost_best, nullptr, nullptr, P, n, c.nb, s.N, &in->rslm, c.stream);
+        if (rc == EPNP_OK && check) rc = plan_rslm(s, *plan);
+    } else if (in) {
+        rc = s.split ? epnp_epnp_init_split_f32(c.x3d, c.x2d, c.w2d, c.cam, in->conf_quantile, c.pose_init, nullptr, c.nb,
+                                                s.N, s.cluster_ctas, c.stream)
+                     : epnp_epnp_init_f32(c.x3d, c.x2d, c.w2d, c.cam, in->conf_quantile, c.pose_init, nullptr, c.nb, s.N,
+                                          c.stream);
+        if (rc == EPNP_OK && check) rc = plan_epnp(s, *plan);
+    }
+    if (rc != EPNP_OK) return rc;
+    if (p->mc_samples == 0)
+        return epnp_lm_solve_f32(c.x3d, c.x2d, c.w2d, c.cam, c.lb, c.ub, c.delta, c.pose_init, c.pose_opt,
+                                 s.want_cov ? c.pose_cov : nullptr, s.want_cost ? c.cost : nullptr, nullptr, nullptr,
+                                 c.nb, s.N, p, c.stream);
+    rc = lm_amis_chunk(c, s.seed, s.N, p, s.split, s.cluster_ctas);
+    if (rc == EPNP_OK && check) rc = plan_amis(s, *plan);
+    return rc;
+}
+
+// The argument checks of the two calls that no composed device call makes: EPNP_OK or EPNP_ERR_BAD_ARG.
+int check_solve_host_args(const HostBufs& h, const EpnpInit* init, void* workspace, size_t workspace_bytes,
+                                 int B, int N, const EpnpParams* p) {
+    if (!p || !workspace || !h.x3d || !h.x2d || !h.w2d || !h.cam || !h.delta || !h.pose_opt) return EPNP_ERR_BAD_ARG;
+    if ((h.lb == nullptr) != (h.ub == nullptr)) return EPNP_ERR_BAD_ARG;
+    if (B < 0 || N <= 0 || p->mc_samples < 0) return EPNP_ERR_BAD_ARG;
+    if ((h.pose_init == nullptr) == (init == nullptr)) return EPNP_ERR_BAD_ARG;        // exactly one start
+    if (p->mc_samples == 0 ? (h.logw || h.samples) : !h.logw) return EPNP_ERR_BAD_ARG;
+    if (init) {
+        if (init->kind == EPNP_INIT_RSLM) {
+            if (init->rslm.dof != p->dof) return EPNP_ERR_BAD_ARG;
+        } else if (init->kind != EPNP_INIT_EPNP || p->dof != 6) {                  // EPnP gives 6DoF poses only
+            return EPNP_ERR_BAD_ARG;
+        }
+    }
+    if (workspace_bytes < ws_layout(B, N, p, init).total) return EPNP_ERR_BAD_ARG;
+    return EPNP_OK;
+}
+
+int solve_host(const HostBufs& h, const EpnpInit* init, uint64_t seed, uint32_t obj_offset, void* workspace,
+                      size_t workspace_bytes, int n_chunks, int B, int N, const EpnpParams* p, bool split,
+                      int cluster_ctas, void* stream) {
+    int rc = check_solve_host_args(h, init, workspace, workspace_bytes, B, N, p);
+    if (rc != EPNP_OK) return rc;
+    const WsLayout w = ws_layout(B, N, p, init);
+    const SolveSpec s{init, seed, p, N, split, cluster_ctas, h.pose_cov != nullptr, h.cost != nullptr};
+    SolvePlan plan{B, n_chunks == 0, 0};
+    // every refusal before the first copy: the whole composition dry-run on an empty chunk
+    rc = solve_chunk(s, chunk_at((char*)workspace, w, 0, 0, N, p, h.lb != nullptr, obj_offset, (cudaStream_t)stream),
+                     &plan);
+    if (rc != EPNP_OK || B == 0) return rc;
+    return host_pipeline([&](const Chunk& c) { return solve_chunk(s, c, nullptr); }, plan.wave, h, workspace, w,
+                         obj_offset, n_chunks, B, N, p, stream);
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t epnp_fused_workspace_bytes(int B, int N, const EpnpParams* p) {
+    if (!p || B < 0 || N <= 0) return 0;
+    return ws_layout(B, N, p).total;
+}
+
+size_t epnp_solve_workspace_bytes(int B, int N, const EpnpParams* p, const EpnpInit* init) {
+    if (!p || B < 0 || N <= 0) return 0;
+    if (init && init->kind != EPNP_INIT_EPNP &&
+        (init->kind != EPNP_INIT_RSLM || init->num_proposals <= 0 || init->num_points <= 0))
+        return 0;
+    return ws_layout(B, N, p, init).total;
+}
+
 int epnp_lm_amis_fused_host_f32(const float* x3d_host, const float* x2d_host, const float* w2d_host,
                                 const float* cam_mats_host, const float* lb_host, const float* ub_host,
                                 const float* delta_host, const float* pose_init_host,
@@ -3200,8 +3389,9 @@ int epnp_lm_amis_fused_host_f32(const float* x3d_host, const float* x2d_host, co
                                 float* pose_samples_host, float* logw_host,
                                 void* workspace, size_t workspace_bytes, int n_chunks,
                                 int B, int N, const EpnpParams* p, void* stream) {
-    const int rc = check_host_args(x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host, ub_host, delta_host,
-                                   pose_init_host, pose_opt_host, logw_host, workspace, workspace_bytes, B, N, p);
+    const HostBufs h{x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host, ub_host, delta_host, pose_init_host,
+                     pose_opt_host, pose_cov_host, cost_host, pose_samples_host, logw_host};
+    const int rc = check_host_args(h, workspace, workspace_bytes, B, N, p);
     if (rc != EPNP_OK || B == 0) return rc;
     int wave = 0;                               // objects in flight: SMs x resident AMIS CTAs per SM
     if (n_chunks == 0) {
@@ -3212,9 +3402,8 @@ int epnp_lm_amis_fused_host_f32(const float* x3d_host, const float* x2d_host, co
             });
         });
     }
-    return host_pipeline(fused_resident_chunk, 0, wave, x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host, ub_host,
-                         delta_host, pose_init_host, seed, obj_offset, pose_opt_host, pose_cov_host, cost_host,
-                         pose_samples_host, logw_host, workspace, n_chunks, B, N, p, stream);
+    return host_pipeline([&](const Chunk& c) { return lm_amis_chunk(c, seed, N, p, false, 0); }, wave, h, workspace,
+                         ws_layout(B, N, p), obj_offset, n_chunks, B, N, p, stream);
 }
 
 int epnp_lm_amis_fused_split_host_f32(const float* x3d_host, const float* x2d_host, const float* w2d_host,
@@ -3225,8 +3414,9 @@ int epnp_lm_amis_fused_split_host_f32(const float* x3d_host, const float* x2d_ho
                                       float* pose_samples_host, float* logw_host,
                                       void* workspace, size_t workspace_bytes, int n_chunks,
                                       int B, int N, const EpnpParams* p, int cluster_ctas, void* stream) {
-    int rc = check_host_args(x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host, ub_host, delta_host,
-                             pose_init_host, pose_opt_host, logw_host, workspace, workspace_bytes, B, N, p);
+    const HostBufs h{x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host, ub_host, delta_host, pose_init_host,
+                     pose_opt_host, pose_cov_host, cost_host, pose_samples_host, logw_host};
+    int rc = check_host_args(h, workspace, workspace_bytes, B, N, p);
     if (rc != EPNP_OK || B == 0) return rc;
     // every refusal of the chunk solves, made here, before the first copy is enqueued
     if ((p->dof != 4 && p->dof != 6) || check_amis_params(*p) != EPNP_OK || p->lm_iter < 0 || fast_mode_without_steps(*p))
@@ -3234,9 +3424,35 @@ int epnp_lm_amis_fused_split_host_f32(const float* x3d_host, const float* x2d_ho
     int wave = 0;                               // objects in flight: co-resident clusters
     const int ctas = split_lm_amis_plan(*p, B, N, cluster_ctas, &wave);
     if (ctas < 0) return ctas;
-    return host_pipeline(epnp_lm_amis_fused_split_f32, ctas, wave, x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host,
-                         ub_host, delta_host, pose_init_host, seed, obj_offset, pose_opt_host, pose_cov_host, cost_host,
-                         pose_samples_host, logw_host, workspace, n_chunks, B, N, p, stream);
+    return host_pipeline([&](const Chunk& c) { return lm_amis_chunk(c, seed, N, p, true, ctas); }, wave, h, workspace,
+                         ws_layout(B, N, p), obj_offset, n_chunks, B, N, p, stream);
+}
+
+int epnp_solve_host_f32(const float* x3d_host, const float* x2d_host, const float* w2d_host,
+                        const float* cam_mats_host, const float* lb_host, const float* ub_host,
+                        const float* delta_host, const float* pose_init_host, const EpnpInit* init,
+                        uint64_t seed, uint32_t obj_offset,
+                        float* pose_opt_host, float* pose_cov_host, float* cost_host,
+                        float* pose_samples_host, float* logw_host,
+                        void* workspace, size_t workspace_bytes, int n_chunks,
+                        int B, int N, const EpnpParams* p, void* stream) {
+    const HostBufs h{x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host, ub_host, delta_host, pose_init_host,
+                     pose_opt_host, pose_cov_host, cost_host, pose_samples_host, logw_host};
+    return solve_host(h, init, seed, obj_offset, workspace, workspace_bytes, n_chunks, B, N, p, false, 0, stream);
+}
+
+int epnp_solve_split_host_f32(const float* x3d_host, const float* x2d_host, const float* w2d_host,
+                              const float* cam_mats_host, const float* lb_host, const float* ub_host,
+                              const float* delta_host, const float* pose_init_host, const EpnpInit* init,
+                              uint64_t seed, uint32_t obj_offset,
+                              float* pose_opt_host, float* pose_cov_host, float* cost_host,
+                              float* pose_samples_host, float* logw_host,
+                              void* workspace, size_t workspace_bytes, int n_chunks,
+                              int B, int N, const EpnpParams* p, int cluster_ctas, void* stream) {
+    const HostBufs h{x3d_host, x2d_host, w2d_host, cam_mats_host, lb_host, ub_host, delta_host, pose_init_host,
+                     pose_opt_host, pose_cov_host, cost_host, pose_samples_host, logw_host};
+    return solve_host(h, init, seed, obj_offset, workspace, workspace_bytes, n_chunks, B, N, p, true, cluster_ctas,
+                      stream);
 }
 
 }  // extern "C"

@@ -25,6 +25,16 @@ class EpnpParams(ctypes.Structure):
                 ("amis_eps", ctypes.c_float), ("acg_mle_iter", ctypes.c_int32), ("acg_dispersion", ctypes.c_float)]
 
 
+INIT_RSLM, INIT_EPNP = 1, 2      # EPNP_INIT_RSLM / EPNP_INIT_EPNP
+
+
+class EpnpInit(ctypes.Structure):
+    """The initialiser of a host-buffer solve from scratch (EpnpInit of include/epropnp_b200.h, 96 bytes)."""
+    _fields_ = [("kind", ctypes.c_int32), ("num_proposals", ctypes.c_int32), ("num_points", ctypes.c_int32),
+                ("reserved0", ctypes.c_int32), ("seed", ctypes.c_uint64), ("conf_quantile", ctypes.c_float),
+                ("reserved1", ctypes.c_int32), ("rslm", EpnpParams)]
+
+
 def lib_path():
     return _LIB_PATH
 
@@ -85,6 +95,11 @@ _SIGNATURES = {
                                     + [_P, ctypes.c_size_t, _I, _I, _I, ctypes.POINTER(EpnpParams), _P]),
     "epnp_lm_amis_fused_split_host_f32": (ctypes.c_int, [_P] * 8 + [ctypes.c_uint64, ctypes.c_uint32] + [_P] * 5
                                           + [_P, ctypes.c_size_t, _I, _I, _I, ctypes.POINTER(EpnpParams), _I, _P]),
+    "epnp_solve_workspace_bytes": (ctypes.c_size_t, [_I, _I, ctypes.POINTER(EpnpParams), ctypes.POINTER(EpnpInit)]),
+    "epnp_solve_host_f32": (ctypes.c_int, [_P] * 8 + [ctypes.POINTER(EpnpInit), ctypes.c_uint64, ctypes.c_uint32]
+                            + [_P] * 5 + [_P, ctypes.c_size_t, _I, _I, _I, ctypes.POINTER(EpnpParams), _P]),
+    "epnp_solve_split_host_f32": (ctypes.c_int, [_P] * 8 + [ctypes.POINTER(EpnpInit), ctypes.c_uint64, ctypes.c_uint32]
+                                  + [_P] * 5 + [_P, ctypes.c_size_t, _I, _I, _I, ctypes.POINTER(EpnpParams), _I, _P]),
 }
 
 

@@ -637,6 +637,92 @@ def _fused_host(fn, extra, host, params, workspace, n_chunks, seed, obj_offset, 
     return out
 
 
+def rslm_spec(dof, num_points=16, num_proposals=64, num_iter=3, seed=0, **kwargs):
+    """The initialiser RSLMSolver(num_points, num_proposals, num_iter, **kwargs) as an EpnpInit for solve_host: kwargs
+    are EpnpParams fields of the RSLM solver's own LM (fast_mode, eps, z_min, ...); its eps is also the draw's.  seed:
+    the Philox seed of the draw (the layer's rslm_seed, apart from the AMIS seed)."""
+    init = capi.EpnpInit(kind=capi.INIT_RSLM, num_proposals=int(num_proposals), num_points=int(num_points),
+                         seed=int(seed))
+    init.rslm = default_params(dof, lm_iter=int(num_iter), **kwargs)
+    return init
+
+
+def epnp_spec(conf_quantile=0.8):
+    """The EPnP initialiser of the 6DoF test loop (EPnPSolver(conf_quantile)) as an EpnpInit for solve_host."""
+    return capi.EpnpInit(kind=capi.INIT_EPNP, conf_quantile=float(conf_quantile))
+
+
+def initial_pose(prob: Problem, init, dof, obj_offset=0):
+    """What `init` (rslm_spec / epnp_spec) computes on the device for a problem: the RSLM draw keyed by
+    obj_offset + object and the RSLM solve, or the EPnP initialisation; each in its resident form up to
+    max_points(dof) and its cluster-split form (automatic C) above -- RSLMSolver(cluster_split=True)'s and EPnPSolver's
+    rule.  -> pose (B, D)."""
+    split = prob.N > max_points(dof)
+    if init.kind == capi.INIT_RSLM:
+        if init.rslm.dof != dof:
+            raise ValueError(f"the RSLM spec is for dof {init.rslm.dof}, the solve for dof {dof}")
+        inds, start = rslm_draw(prob.x3d, prob.x2d, prob.w2d, prob.cam, init.num_proposals, init.num_points, dof,
+                                eps=init.rslm.eps, seed=init.seed, obj_offset=obj_offset)
+        return (rslm_split if split else rslm)(prob, inds, start, init.rslm)["pose"]
+    if init.kind == capi.INIT_EPNP:
+        if dof != 6:
+            raise ValueError("EPnP initialises 6DoF poses only")
+        return (epnp_init_split if split else epnp_init)(prob.x3d, prob.x2d, prob.w2d, prob.cam, init.conf_quantile)
+    raise ValueError(f"unknown initialiser kind {init.kind}")
+
+
+def solve_workspace_bytes(B, N, params, init=None):
+    return int(lib().epnp_solve_workspace_bytes(B, N, ctypes.byref(params),
+                                                None if init is None else ctypes.byref(init)))
+
+
+def solve_host(host, params, workspace, init=None, n_chunks=8, seed=0, obj_offset=0, out=None, want_samples=True,
+               want_cov=True, want_cost=True):
+    """Host-buffer solve from host["pose_init"] or, with `init` (rslm_spec / epnp_spec) and no pose_init, from scratch
+    (epnp_solve_host_f32): LM only when params.mc_samples = 0, else LM + AMIS, in the chunked pipeline of
+    lm_amis_fused_host.  host = dict(x3d, x2d, w2d, cam_mats, lb, ub, delta[, pose_init]) of CPU float32 tensors;
+    `workspace` a CUDA uint8 tensor of solve_workspace_bytes().  Results land in `out` (pinned CPU tensors, allocated
+    when None: pose_opt, pose_cov / cost as asked, logw / pose_samples with AMIS).  Synchronise the workspace device's
+    current stream before reading them."""
+    return _solve_host("epnp_solve_host_f32", (), host, params, workspace, init, n_chunks, seed, obj_offset, out,
+                       want_samples, want_cov, want_cost)
+
+
+def solve_split_host(host, params, workspace, init=None, n_chunks=8, seed=0, obj_offset=0, out=None, want_samples=True,
+                     want_cov=True, want_cost=True, cluster_ctas=0):
+    """solve_host for objects larger than one SM holds (epnp_solve_split_host_f32): every stage that has a split form
+    takes it; cluster_ctas = 0 lets each stage pick its own cluster size, otherwise every split stage uses that one."""
+    return _solve_host("epnp_solve_split_host_f32", (int(cluster_ctas),), host, params, workspace, init, n_chunks, seed,
+                       obj_offset, out, want_samples, want_cov, want_cost)
+
+
+def _solve_host(fn, extra, host, params, workspace, init, n_chunks, seed, obj_offset, out, want_samples, want_cov,
+                want_cost):
+    B, N = host["x3d"].shape[0], host["x3d"].shape[1]
+    D = 7 if params.dof == 6 else 4
+    M = params.mc_samples
+    if out is None:
+        pin = dict(dtype=torch.float32, pin_memory=True)
+        out = dict(pose_opt=torch.empty(B, D, **pin),
+                   pose_cov=torch.empty(B, params.dof, params.dof, **pin) if want_cov else None,
+                   cost=torch.empty(B, **pin) if want_cost else None,
+                   logw=torch.empty(B, M, **pin) if M > 0 else None,
+                   pose_samples=torch.empty(B, M, D, **pin) if M > 0 and want_samples else None)
+    for k in ("x3d", "x2d", "w2d", "cam_mats", "delta", "lb", "ub", "pose_init"):
+        t = host.get(k)
+        assert t is None or ((not t.is_cuda) and t.dtype == torch.float32 and t.is_contiguous()), k
+    dev = workspace.device
+    with torch.cuda.device(dev):
+        check(getattr(lib(), fn)(
+            ptr(host["x3d"]), ptr(host["x2d"]), ptr(host["w2d"]), ptr(host["cam_mats"]), ptr(host.get("lb")),
+            ptr(host.get("ub")), ptr(host["delta"]), ptr(host.get("pose_init")),
+            None if init is None else ctypes.byref(init), ctypes.c_uint64(seed), ctypes.c_uint32(obj_offset),
+            ptr(out["pose_opt"]), ptr(out.get("pose_cov")), ptr(out.get("cost")), ptr(out.get("pose_samples")),
+            ptr(out.get("logw")), ctypes.c_void_p(workspace.data_ptr()), ctypes.c_size_t(workspace.numel()),
+            int(n_chunks), B, N, ctypes.byref(params), *extra, stream_ptr(dev)), fn)
+    return out
+
+
 def mc_epilogue(logw_bm, pose_samples_bmd=None, pose_opt=None, cost_target=None, want_lse=True, want_loss=False,
                 want_weights=False, want_score=False):
     """One pass over the object-major AMIS outputs (epnp_mc_epilogue_f32): logw (B, M) [, pose_samples (B, M, D),
@@ -686,4 +772,4 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
 
 __all__ = ["Problem", "adaptive_delta", "cost_backward", "cost_camera_backward", "gn_plus_camera_backward",
            "evaluate_cost", "evaluate_cost_split", "evaluate_full", "evaluate_backward", "lm_solve",
-           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "rslm", "rslm_split", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]
+           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "solve_host", "solve_split_host", "solve_workspace_bytes", "rslm_spec", "epnp_spec", "initial_pose", "rslm", "rslm_split", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

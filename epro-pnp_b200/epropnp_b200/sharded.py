@@ -264,12 +264,19 @@ class PushGather(_DeviceHooks):
         self.step = 0
         dist.barrier(group=group)
 
-    def solve(self, prob, pose_init, params, seed=0, want_cost=False, want_cov=False):
+    def solve(self, prob, pose_init, params, seed=0, want_cost=False, want_cov=False, init=None):
         """Enqueue batch `step`: fused solve with in-kernel push.  Returns (local result dict, PendingGather of the
-        full-batch pose_opt / logw)."""
+        full-batch pose_opt / logw).  pose_init None: `init` (native.rslm_spec / epnp_spec) first computes it on this
+        rank's shard, on the current stream, with the RSLM draws keyed by the global object index, so the assembled
+        batch equals the single-process run from the same initialiser."""
         t = self.step
         s = t % self.depth
         lo, hi = self.rank * self.per_rank, (self.rank + 1) * self.per_rank
+        if init is not None:
+            if pose_init is not None:
+                raise ValueError("PushGather.solve takes pose_init or an initialiser (init), not both")
+            from . import native
+            pose_init = native.initial_pose(prob, init, params.dof, obj_offset=lo)
         cur = self._current_stream()
         gate = self.met.get(t - (self.depth - self.valid_for))
         if gate is not None:

@@ -11,7 +11,7 @@
  *   - every pointer is a DEVICE pointer to contiguous row-major fp32 unless the name ends in _host;
  *   - the caller owns and allocates every buffer; the library allocates no memory, is re-entrant, and only enqueues work
  *     on `stream` (a cudaStream_t passed as void*).  Per-host-thread state, exactly two items: the cudaError_t of the
- *     last failed call (epnp_last_cuda_error) and the four helper streams of epnp_lm_amis_fused_host_f32, created on that
+ *     last failed call (epnp_last_cuda_error) and the four helper streams of the host-buffer calls, created on that
  *     thread's first host-buffer call and kept for its lifetime;
  *   - return value: EPNP_OK or a negative EPNP_ERR_* code (never throws, never aborts);
  *     CUDA launch errors come back as EPNP_ERR_CUDA (epnp_last_cuda_error() has the cudaError_t);
@@ -494,6 +494,71 @@ int epnp_lm_amis_fused_split_host_f32(const float* x3d_host, const float* x2d_ho
                                       float* pose_samples_host, float* logw_host,
                                       void* workspace, size_t workspace_bytes, int n_chunks,
                                       int B, int N, const EpnpParams* p, int cluster_ctas, void* stream);
+
+/* The initialiser of a host-buffer solve from scratch (epnp_solve_host_f32): where LMSolver.solve gets its start
+ * when no pose_init is given (levenberg_marquardt.py:113-124, init_solver.solve).
+ *   EPNP_INIT_RSLM: RSLMSolver (levenberg_marquardt.py:271-353) -- epnp_rslm_draw_f32 with `seed` (the layer's
+ *     rslm_seed, drawn apart from the AMIS seed) and rslm.eps, then epnp_rslm_f32 with `rslm` as its parameters
+ *     (RSLMSolver(num_iter=..., **kwargs) has its own lm_iter, fast_mode, eps, z_min ...; rslm.dof must equal the
+ *     solve's dof).  num_proposals = P, num_points = n.
+ *   EPNP_INIT_EPNP: EPnPSolver of the 6DoF test loop (EPro-PnP-6DoF/lib/test.py:178-194) -- epnp_epnp_init_f32 with
+ *     conf_quantile; dof 6 only.
+ * Fields a kind does not use are ignored; the reserved ones keep the layout explicit (sizeof = 96 on every ABI).   */
+enum { EPNP_INIT_RSLM = 1, EPNP_INIT_EPNP = 2 };
+typedef struct EpnpInit {
+    int32_t    kind;                /* EPNP_INIT_RSLM or EPNP_INIT_EPNP                          */
+    int32_t    num_proposals;       /* RSLMSolver.num_proposals (P)                               */
+    int32_t    num_points;          /* RSLMSolver.num_points (n)                                  */
+    int32_t    reserved0;
+    uint64_t   seed;                /* Philox seed of the RSLM draw                               */
+    float      conf_quantile;       /* EPnP: keep the points with confidence >= this quantile     */
+    int32_t    reserved1;
+    EpnpParams rslm;                /* the RSLM solver's own parameters                          */
+} EpnpInit;
+
+/* Host-buffer solve from a given pose or from scratch, in the chunked copy-in / solve / copy-out pipeline of
+ * epnp_lm_amis_fused_host_f32 (same helper streams, n_chunks rule, obj_offset and outputs).  It replaces the two
+ * default inference paths of the reference, which have no AMIS:
+ *   Det inference (EPro-PnP-Det/configs/epropnp_det_v1b_220411.py:158-160, deform_pnp_head.py:520-527): RSLM
+ *     (P = 64, n = 16, 3 iterations), then LM with 5 iterations in fast mode -- init = RSLM, p->mc_samples = 0;
+ *   6DoF test (EPro-PnP-6DoF/lib/test.py:91-96,178-211): EPnP on the points kept by the confidence quantile, then
+ *     LMSolver(dof=6, num_iter=3) in fast mode -- init = EPNP, p->mc_samples = 0.
+ * Start: exactly one of pose_init_host and init (EPNP_ERR_BAD_ARG for both or neither).
+ * p->mc_samples = 0: LM only (EProPnP.forward / LMSolver.forward): epnp_lm_solve_f32 per chunk; logw_host and
+ *   pose_samples_host must be NULL; pose_cov_host and cost_host stay optional under epnp_lm_solve_f32's rule (fast
+ *   mode with lm_iter = 0 has none).
+ * p->mc_samples > 0: LM + AMIS (monte_carlo_forward): epnp_lm_amis_fused_f32 per chunk; logw_host required.
+ * Per chunk, on its compute stream after its copy-in: the RSLM draw (with obj_offset + the chunk's first object, so
+ * the results never depend on the chunking) and the RSLM solve, or the EPnP initialisation; then LM or LM + AMIS.  The
+ * results equal that composition of device calls on the same inputs bit for bit.
+ * workspace: device memory of at least epnp_solve_workspace_bytes(B, N, p, init) bytes (init = NULL: pose_init given;
+ * 0 for arguments no call takes).  Every refusal comes before the first copy, and is the refusal, with its code, that
+ * the composed device calls make -- EPnP with dof 4 and an RSLM spec of another dof are EPNP_ERR_BAD_ARG.
+ * n_chunks = 0 cuts the batch at whole waves of the AMIS kernel, or, with mc_samples = 0, of the initialiser's kernel
+ * (one chunk for LM alone from a given pose).                                                                       */
+size_t epnp_solve_workspace_bytes(int B, int N, const EpnpParams* p, const EpnpInit* init);
+int epnp_solve_host_f32(const float* x3d_host, const float* x2d_host, const float* w2d_host,
+                        const float* cam_mats_host, const float* lb_host, const float* ub_host,
+                        const float* delta_host, const float* pose_init_host /*[opt]*/, const EpnpInit* init /*[opt]*/,
+                        uint64_t seed, uint32_t obj_offset,
+                        float* pose_opt_host, float* pose_cov_host, float* cost_host,
+                        float* pose_samples_host, float* logw_host,
+                        void* workspace, size_t workspace_bytes, int n_chunks,
+                        int B, int N, const EpnpParams* p, void* stream);
+
+/* epnp_solve_host_f32 for objects of up to epnp_max_points_split points: every stage that has a split form takes it at
+ * any N -- epnp_rslm_split_f32 or epnp_epnp_init_split_f32, then epnp_lm_amis_fused_split_f32 (epnp_lm_solve_f32 takes
+ * any N) -- and the results equal that composition bit for bit.  cluster_ctas = 0: each stage picks its own automatic
+ * C; otherwise every split stage uses that C, which must then lie in every stage's range.  EPNP_ERR_UNSUPPORTED where
+ * a stage's cluster cannot be co-scheduled; n_chunks = 0 cuts at whole waves of co-resident clusters.              */
+int epnp_solve_split_host_f32(const float* x3d_host, const float* x2d_host, const float* w2d_host,
+                              const float* cam_mats_host, const float* lb_host, const float* ub_host,
+                              const float* delta_host, const float* pose_init_host, const EpnpInit* init,
+                              uint64_t seed, uint32_t obj_offset,
+                              float* pose_opt_host, float* pose_cov_host, float* cost_host,
+                              float* pose_samples_host, float* logw_host,
+                              void* workspace, size_t workspace_bytes, int n_chunks,
+                              int B, int N, const EpnpParams* p, int cluster_ctas, void* stream);
 
 #ifdef __cplusplus
 }
