@@ -11,6 +11,8 @@
 //   cost_kernel, evaluate_full_kernel, rslm_draw_kernel, rslm_kernel, cost_backward_kernel, gn_plus_backward_kernel, adaptive_delta_kernel,
 //   mc_epilogue_kernel, mc_lse_backward_kernel      the steps either side of the path (CTA per object).
 //   evaluate_backward_kernel         the backward of evaluate_full_kernel's residual / Jacobian / cost (CTA per object, any N).
+//   cost_hvp_point_kernel, cost_hvp_pose_kernel    second order through the cost: Hessian-vector products, point-major
+//                                    (CTA per object) and pose-major (thread per pose), points streamed from global memory.
 //   cost_pose_backward_kernel, cost_pose_backward_split_kernel    the cost's gradient with respect to stacked poses: thread per
 //                                    pose over the resident points; the split form on cost_split_kernel's clusters.
 //   epnp_init_kernel (pnp_epnp.cuh)  EPnP initialiser with the confidence-quantile point selection, fp64, CTA per object.
@@ -1285,6 +1287,269 @@ __global__ void __launch_bounds__(COST_SPLIT_TILE, 1) cost_camera_backward_split
         (void)stored;
     }
     cluster_sync();                                     // no CTA leaves while rank 0 may still read its slot
+}
+
+// ------------------------------------------------------------------------------------------------
+// Hessian-vector product of the cost f = sum_p g_p sum_i c(pose_p, point_i; K, lb, ub, delta): the backward of the three
+// cost backwards above.  One tangent v (optional parts: x3d, x2d, w2d, delta, every pose, K, lb, ub) rides along as a
+// Dual<1> through the forward of one (pose, point) pair and through its reverse-mode gradient, written out for every
+// input with the gates of the first-order kernels: no tangent and no gradient through a depth clamped at z_min; a clamped
+// coordinate takes the tangent of the bound it sits on (ub when it equals ub, the outer min, else lb) and passes its
+// gradient to that bound only; the Huber branch is the forward's (inlier c = s^2 / 2, outlier c = delta s - delta^2 / 2).
+// The gradient's tangents are the Hessian's rows times v, the cost's own tangent is grad c . v.  The arithmetic is the
+// math of the first-order kernels, not their instruction sequence (exact divides and square roots here).
+typedef Dual<1> D1;
+__device__ __forceinline__ D1 d1(float v, float d) { D1 r; r.v = v; r.d[0] = d; return r; }
+
+struct HvpPair {
+    D1 cost;
+    D1 g[8];            // d c / d (X, Y, Z, u, v, wu, wv, delta)
+    D1 gxc[3];          // d c / d x_cam (= d c / d t)
+    D1 h[3], xc[3];     // d c / d (K x_cam) and x_cam: d c / d K = h xc^T
+    D1 gb[4];           // d c / d (lbx, lby, ubx, uby)
+};
+
+__device__ __forceinline__ void pair_cost_hvp(const D1 (&R)[9], const D1 (&t)[3], const D1 (&K)[9], const D1 (&bnd)[4],
+                                              const Cam& cam, const D1& delta, const D1 (&pt)[7], HvpPair& o) {
+    const D1 &X = pt[0], &Y = pt[1], &Z = pt[2], &u = pt[3], &v = pt[4], &wu = pt[5], &wv = pt[6];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) o.xc[r] = R[3 * r] * X + R[3 * r + 1] * Y + R[3 * r + 2] * Z + t[r];
+    const D1 xh = K[0] * o.xc[0] + K[1] * o.xc[1] + K[2] * o.xc[2];
+    const D1 yh = K[3] * o.xc[0] + K[4] * o.xc[1] + K[5] * o.xc[2];
+    const D1 zh = K[6] * o.xc[0] + K[7] * o.xc[1] + K[8] * o.xc[2];
+    const bool z_free = zh.v >= cam.z_min;
+    const D1 iz = dual_recip(dual_gate(zh, fmaxf(zh.v, cam.z_min), z_free));
+    const D1 px = xh * iz, py = yh * iz;
+    D1 pxc = px, pyc = py;
+    bool lx = false, ux = false, ly = false, uy = false;     // coordinate clamped at lb / at ub
+    if (cam.bounded) {
+        const float cx = fminf(fmaxf(px.v, cam.lbx), cam.ubx), cy = fminf(fmaxf(py.v, cam.lby), cam.uby);
+        ux = cx != px.v && cx == cam.ubx; lx = cx != px.v && !ux;
+        uy = cy != py.v && cy == cam.uby; ly = cy != py.v && !uy;
+        if (ux || lx) pxc = ux ? bnd[2] : bnd[0];
+        if (uy || ly) pyc = uy ? bnd[3] : bnd[1];
+    }
+    const D1 ex = pxc - u, ey = pyc - v;
+    const D1 rx = ex * wu, ry = ey * wv;
+    const D1 s2 = rx * rx + ry * ry;
+    D1 k;
+    if (sqrtf(s2.v) <= delta.v) {
+        o.cost = s2 * 0.5f;
+        k = dual_const<1>(1.f);
+        o.g[7] = dual_const<1>(0.f);
+    } else {
+        const D1 s = dual_sqrt(s2);
+        o.cost = delta * s - delta * delta * 0.5f;
+        k = delta * dual_recip(s);
+        o.g[7] = s - delta;
+    }
+    const D1 grx = k * rx, gry = k * ry;
+    o.g[5] = grx * ex; o.g[6] = gry * ey;
+    const D1 gex = grx * wu, gey = gry * wv;
+    o.g[3] = gex * -1.f; o.g[4] = gey * -1.f;
+    const D1 zero = dual_const<1>(0.f);
+    o.gb[0] = lx ? gex : zero; o.gb[1] = ly ? gey : zero; o.gb[2] = ux ? gex : zero; o.gb[3] = uy ? gey : zero;
+    o.h[0] = (lx || ux) ? zero : gex * iz;
+    o.h[1] = (ly || uy) ? zero : gey * iz;
+    o.h[2] = z_free ? (o.h[0] * px + o.h[1] * py) * -1.f : zero;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o.gxc[c] = K[c] * o.h[0] + K[3 + c] * o.h[1] + K[6 + c] * o.h[2];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o.g[c] = R[c] * o.gxc[0] + R[3 + c] * o.gxc[1] + R[6 + c] * o.gxc[2];
+}
+
+struct HvpArgs {
+    KArgs k;                    // correspondences, camera, bounds, delta, poses = (B, P, D) object-major, p.z_min
+    const float* grad;          // (B, P)  g_p
+    const float *tx3d, *tx2d, *tw2d, *tdelta, *tpose, *tcam, *tlb, *tub;          // [opt] the tangent v
+    float *hx3d, *hx2d, *hw2d, *hdelta, *hpose, *hgrad, *hcam, *hlb, *hub;         // [opt] H v and grad c_p . v
+    int P;
+};
+
+__device__ __forceinline__ float tan_at(const float* t, size_t i) { return t ? __ldg(t + i) : 0.f; }
+
+// K, the bounds and delta of one object with their tangents
+__device__ __forceinline__ void hvp_object(const HvpArgs& g, int obj, Cam& cam, D1 (&K)[9], D1 (&bnd)[4], D1& delta) {
+    cam = load_cam(g.k, obj);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) K[i] = d1(cam.k[i], tan_at(g.tcam, (size_t)obj * 9 + i));
+    bnd[0] = d1(cam.lbx, tan_at(g.tlb, 2 * (size_t)obj)); bnd[1] = d1(cam.lby, tan_at(g.tlb, 2 * (size_t)obj + 1));
+    bnd[2] = d1(cam.ubx, tan_at(g.tub, 2 * (size_t)obj)); bnd[3] = d1(cam.uby, tan_at(g.tub, 2 * (size_t)obj + 1));
+    delta = d1(__ldg(g.k.delta + obj), tan_at(g.tdelta, obj));
+}
+
+__device__ __forceinline__ void hvp_point(const HvpArgs& g, size_t q, D1 (&pt)[7]) {
+    const KArgs& a = g.k;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) pt[c] = d1(__ldg(a.x3d + q * 3 + c), tan_at(g.tx3d, q * 3 + c));
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+        pt[3 + c] = d1(__ldg(a.x2d + q * 2 + c), tan_at(g.tx2d, q * 2 + c));
+        pt[5 + c] = d1(__ldg(a.w2d + q * 2 + c), tan_at(g.tw2d, q * 2 + c));
+    }
+}
+
+// R and t of pose row `row` with their tangents; p[] the raw components (t, then w x y z or the yaw)
+template <int DOF>
+__device__ __forceinline__ void hvp_pose(const HvpArgs& g, size_t row, D1 (&R)[9], D1 (&t)[3], D1 (&p)[Dim<DOF>::POSE]) {
+    constexpr int PD = Dim<DOF>::POSE;
+#pragma unroll
+    for (int k = 0; k < PD; ++k) p[k] = d1(__ldg(g.k.poses + row * PD + k), tan_at(g.tpose, row * PD + k));
+#pragma unroll
+    for (int i = 0; i < 3; ++i) t[i] = p[i];
+    if (DOF == 6) {
+        const D1 &w = p[3], &x = p[4], &y = p[5], &z = p[6];
+        const D1 ww = w * w, xx = x * x, yy = y * y, zz = z * z;
+        R[0] = ww + xx - yy - zz; R[1] = (x * y - w * z) * 2.f; R[2] = (x * z + w * y) * 2.f;
+        R[3] = (x * y + w * z) * 2.f; R[4] = ww - xx + yy - zz; R[5] = (y * z - w * x) * 2.f;
+        R[6] = (x * z - w * y) * 2.f; R[7] = (y * z + w * x) * 2.f; R[8] = ww - xx - yy + zz;
+    } else {
+        float r[9];
+        yaw_to_rot(p[3].v, r);                                  // d cos = -sin, d sin = cos
+        const float dy = p[3].d[0];
+#pragma unroll
+        for (int i = 0; i < 9; ++i) R[i] = dual_const<1>(r[i]);
+        R[0].d[0] = -r[2] * dy; R[2].d[0] = r[0] * dy; R[6].d[0] = -r[0] * dy; R[8].d[0] = -r[2] * dy;
+    }
+}
+
+// Point-major: one CTA per object, thread <-> point, every thread sweeping the object's poses (lifted once per tile into
+// shared memory).  Writes g_p-weighted H v at the points, and reduces the delta, K and bound rows with one fixed-order
+// block sum.  No atomics.
+constexpr int HVP_POSE_TILE = 128;
+constexpr int HVP_POSE_REC = 25;                // R, t: value and tangent (24), g_p
+
+template <int DOF>
+__global__ void __launch_bounds__(NT) cost_hvp_point_kernel(const HvpArgs g) {
+    __shared__ float rec[HVP_POSE_TILE * HVP_POSE_REC];
+    __shared__ float red[2 * NW * 32];
+    constexpr int PD = Dim<DOF>::POSE;
+    const KArgs& a = g.k;
+    const int obj = blockIdx.x, tid = threadIdx.x;
+    Cam cam;
+    D1 K[9], bnd[4], delta;
+    hvp_object(g, obj, cam, K, bnd, delta);
+    float acc[14];                              // delta, K (row-major), lbx lby ubx uby
+#pragma unroll
+    for (int k = 0; k < 14; ++k) acc[k] = 0.f;
+    for (int base = 0; base < a.N; base += NT) {
+        const int n = base + tid;
+        const bool ok = n < a.N;
+        const size_t q = (size_t)obj * a.N + (ok ? n : 0);
+        D1 pt[7];
+        hvp_point(g, q, pt);
+        float hp[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        for (int p0 = 0; p0 < g.P; p0 += HVP_POSE_TILE) {
+            const int np = min(HVP_POSE_TILE, g.P - p0);
+            __syncthreads();                    // the previous tile is consumed
+            for (int j = tid; j < np; j += NT) {
+                const size_t row = (size_t)obj * g.P + p0 + j;
+                D1 R[9], t[3], p[PD];
+                hvp_pose<DOF>(g, row, R, t, p);
+                float* r = rec + j * HVP_POSE_REC;
+#pragma unroll
+                for (int i = 0; i < 9; ++i) { r[2 * i] = R[i].v; r[2 * i + 1] = R[i].d[0]; }
+#pragma unroll
+                for (int i = 0; i < 3; ++i) { r[18 + 2 * i] = t[i].v; r[19 + 2 * i] = t[i].d[0]; }
+                r[24] = __ldg(g.grad + row);
+            }
+            __syncthreads();
+            if (!ok) continue;
+            for (int j = 0; j < np; ++j) {
+                const float* r = rec + j * HVP_POSE_REC;
+                D1 R[9], t[3];
+#pragma unroll
+                for (int i = 0; i < 9; ++i) R[i] = d1(r[2 * i], r[2 * i + 1]);
+#pragma unroll
+                for (int i = 0; i < 3; ++i) t[i] = d1(r[18 + 2 * i], r[19 + 2 * i]);
+                const float gj = r[24];
+                HvpPair o;
+                pair_cost_hvp(R, t, K, bnd, cam, delta, pt, o);
+#pragma unroll
+                for (int k = 0; k < 7; ++k) hp[k] = fmaf(gj, o.g[k].d[0], hp[k]);
+                acc[0] = fmaf(gj, o.g[7].d[0], acc[0]);
+#pragma unroll
+                for (int i = 0; i < 3; ++i) {
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) acc[1 + 3 * i + c] = fmaf(gj, (o.h[i] * o.xc[c]).d[0], acc[1 + 3 * i + c]);
+                }
+#pragma unroll
+                for (int k = 0; k < 4; ++k) acc[10 + k] = fmaf(gj, o.gb[k].d[0], acc[10 + k]);
+            }
+        }
+        if (ok) {
+            if (g.hx3d) { g.hx3d[q * 3] = hp[0]; g.hx3d[q * 3 + 1] = hp[1]; g.hx3d[q * 3 + 2] = hp[2]; }
+            if (g.hx2d) { g.hx2d[q * 2] = hp[3]; g.hx2d[q * 2 + 1] = hp[4]; }
+            if (g.hw2d) { g.hw2d[q * 2] = hp[5]; g.hw2d[q * 2 + 1] = hp[6]; }
+        }
+    }
+    block_sum<14>(acc, red, 0);
+    if (tid == 0) {
+        if (g.hdelta) g.hdelta[obj] = acc[0];
+        float cg[CAM_GRADS];
+#pragma unroll
+        for (int k = 0; k < CAM_GRADS; ++k) cg[k] = acc[1 + k];
+        store_camera_grad(g.hcam, g.hlb, g.hub, obj, cg);
+    }
+}
+
+// Pose-major: thread <-> pose, every thread streaming its object's points from global memory (the same point for all
+// threads of a CTA at a time: L1 broadcasts).  Per pose it sums d c / d t and G = d c / d R = sum (d c / d x_cam) X^T
+// with their tangents, then contracts them with the lifted raw pose components as pose_grad_contract does: the tangent of
+// that contraction times g_p is the pose's H v; the summed tangent of the cost is grad c_p . v.
+template <int DOF>
+__global__ void __launch_bounds__(NT) cost_hvp_pose_kernel(const HvpArgs g, const int tiles) {
+    constexpr int PD = Dim<DOF>::POSE;
+    const KArgs& a = g.k;
+    const int obj = blockIdx.x / tiles, p = (blockIdx.x % tiles) * NT + threadIdx.x;
+    if (p >= g.P) return;
+    const size_t row = (size_t)obj * g.P + p;
+    Cam cam;
+    D1 K[9], bnd[4], delta, R[9], t[3], q[PD];
+    hvp_object(g, obj, cam, K, bnd, delta);
+    hvp_pose<DOF>(g, row, R, t, q);
+    D1 gt[3], G[9];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) gt[i] = dual_const<1>(0.f);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) G[i] = dual_const<1>(0.f);
+    float dc = 0.f;
+    for (int n = 0; n < a.N; ++n) {
+        D1 pt[7];
+        hvp_point(g, (size_t)obj * a.N + n, pt);
+        HvpPair o;
+        pair_cost_hvp(R, t, K, bnd, cam, delta, pt, o);
+        dc += o.cost.d[0];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            gt[i] = gt[i] + o.gxc[i];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) G[3 * i + c] = G[3 * i + c] + o.gxc[i] * pt[c];
+        }
+    }
+    D1 out[PD];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) out[i] = gt[i];
+    if (DOF == 6) {
+        const D1 &w = q[3], &x = q[4], &y = q[5], &z = q[6];
+        const D1 a01 = G[1] + G[3], a02 = G[2] + G[6], a12 = G[5] + G[7];
+        const D1 d10 = G[3] - G[1], d02 = G[2] - G[6], d21 = G[7] - G[5];
+        out[3] = (w * (G[0] + G[4] + G[8]) + x * d21 + y * d02 + z * d10) * 2.f;
+        out[4] = (x * (G[0] - G[4] - G[8]) + w * d21 + y * a01 + z * a02) * 2.f;
+        out[5] = (y * (G[4] - G[0] - G[8]) + w * d02 + x * a01 + z * a12) * 2.f;
+        out[6] = (z * (G[8] - G[0] - G[4]) + w * d10 + x * a02 + y * a12) * 2.f;
+    } else {
+        float sn, cs;
+        sincosf(q[3].v, &sn, &cs);
+        const D1 s = d1(sn, cs * q[3].d[0]), c = d1(cs, -sn * q[3].d[0]);
+        out[3] = c * (G[2] - G[6]) - s * (G[0] + G[8]);
+    }
+    const float gp = __ldg(g.grad + row);
+    if (g.hpose) {
+#pragma unroll
+        for (int k = 0; k < PD; ++k) g.hpose[row * PD + k] = gp * out[k].d[0];
+    }
+    if (g.hgrad) g.hgrad[row] = dc;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2888,6 +3153,41 @@ int epnp_cost_backward_f32(const float* x3d, const float* x2d, const float* w2d,
     const int grid = B < sms * 4 ? B : sms * 4;
     return by_dof(dof, [&](auto D) {
         return launch_plain(cost_backward_kernel<D>, grid, NT, smem, SmemAttr::size, (cudaStream_t)stream, a);
+    });
+}
+
+int epnp_cost_hvp_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                      const float* lb, const float* ub, const float* delta, const float* poses, const float* grad, int P,
+                      const float* t_x3d, const float* t_x2d, const float* t_w2d, const float* t_delta,
+                      const float* t_pose, const float* t_cam, const float* t_lb, const float* t_ub,
+                      float* h_x3d, float* h_x2d, float* h_w2d, float* h_delta, float* h_pose, float* h_grad,
+                      float* h_cam, float* h_lb, float* h_ub, int B, int N, int dof, float z_min, void* stream) {
+    HvpArgs g{};
+    KArgs& a = g.k;
+    a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
+    a.poses = poses;
+    epnp_default_params(&a.p, dof);
+    a.p.z_min = z_min;
+    const int rc = check_common(a);
+    if (rc != EPNP_OK) return rc;
+    if (P < 0 || (P > 0 && (!poses || !grad))) return EPNP_ERR_BAD_ARG;
+    if (!lb && (t_lb || t_ub || h_lb || h_ub)) return EPNP_ERR_BAD_ARG;
+    if (B == 0) return EPNP_OK;
+    if (N > epnp_max_points_split(dof, 0, 0)) return EPNP_ERR_TOO_MANY_POINTS;
+    g.grad = grad; g.P = P;
+    g.tx3d = t_x3d; g.tx2d = t_x2d; g.tw2d = t_w2d; g.tdelta = t_delta; g.tpose = t_pose; g.tcam = t_cam;
+    g.tlb = t_lb; g.tub = t_ub;
+    g.hx3d = h_x3d; g.hx2d = h_x2d; g.hw2d = h_w2d; g.hdelta = h_delta; g.hpose = h_pose; g.hgrad = h_grad;
+    g.hcam = h_cam; g.hlb = h_lb; g.hub = h_ub;
+    const bool points = h_x3d || h_x2d || h_w2d || h_delta || h_cam || h_lb || h_ub;
+    const bool poses_out = P > 0 && (h_pose || h_grad);
+    const int tiles = (P + NT - 1) / NT;
+    return by_dof(dof, [&](auto D) {
+        int r = EPNP_OK;
+        if (points) r = launch_plain(cost_hvp_point_kernel<D>, B, NT, 0, SmemAttr::none, (cudaStream_t)stream, g);
+        if (r == EPNP_OK && poses_out)
+            r = launch_plain(cost_hvp_pose_kernel<D>, B * tiles, NT, 0, SmemAttr::none, (cudaStream_t)stream, g, tiles);
+        return r;
     });
 }
 

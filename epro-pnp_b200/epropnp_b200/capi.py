@@ -86,6 +86,7 @@ _SIGNATURES = {
     "epnp_cost_camera_backward_f32": (ctypes.c_int, [_P] * 7 + [_P, _P, _I, _P, _P, _I] + [_P] * 3 + [_I, _I, _I, _F, _P]),
     "epnp_cost_camera_backward_split_f32": (ctypes.c_int, [_P] * 7 + [_P, _P, _I, _P, _P, _I] + [_P] * 3
                                             + [_I, _I, _I, _F, _I, _P]),
+    "epnp_cost_hvp_f32": (ctypes.c_int, [_P] * 9 + [_I] + [_P] * 8 + [_P] * 9 + [_I, _I, _I, _F, _P]),
     "epnp_gn_plus_camera_backward_f32": (ctypes.c_int, [_P] * 12 + [_I, _I, _I, _F, _F, _F, _P]),
     "epnp_gn_plus_camera_backward_split_f32": (ctypes.c_int, [_P] * 12 + [_I, _I, _I, _F, _F, _F, _I, _P]),
     "epnp_mc_epilogue_f32": (ctypes.c_int, [_P] * 8 + [_I, _I, _I, _P]),

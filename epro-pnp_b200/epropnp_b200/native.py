@@ -570,6 +570,48 @@ def cost_camera_backward(prob: Problem, dof, z_min, poses_a, grad_a, poses_b=Non
     return gcam, glb, gub
 
 
+HVP_TANGENTS = ("x3d", "x2d", "w2d", "delta", "pose", "cam", "lb", "ub")
+HVP_OUTPUTS = ("x3d", "x2d", "w2d", "delta", "pose", "grad", "cam", "lb", "ub")
+
+
+def cost_hvp(prob: Problem, dof, z_min, poses, grad, tangents, want):
+    """The Hessian-vector product of f = sum_p grad[b, p] * cost(poses[b, p]) for object-major poses (B, P, D) and grad
+    (B, P) (epnp_cost_hvp_f32).  `tangents`: the parts of v by name (HVP_TANGENTS; missing or None: zero), shaped
+    (B, N, 3), (B, N, 2), (B, N, 2), (B), (B, P, D), (B, 3, 3), (B, 2), (B, 2).  `want`: nine flags in HVP_OUTPUTS order.
+    Returns H v with respect to x3d, x2d, w2d, delta, the poses (times grad), d cost_p . v (B, P), and H v with respect to
+    cam_mats, lb, ub; None where `want` is False."""
+    B, N = prob.B, prob.N
+    D = 7 if dof == 6 else 4
+    P = poses.shape[1]
+    _check_pose(poses, (B, P), D, "poses")
+    if tuple(grad.shape) != (B, P):
+        raise ValueError(f"grad must be {(B, P)}; got {tuple(grad.shape)}")
+    if len(want) != len(HVP_OUTPUTS):
+        raise ValueError(f"want: {len(HVP_OUTPUTS)} flags ({', '.join(HVP_OUTPUTS)})")
+    unknown = set(tangents) - set(HVP_TANGENTS)
+    if unknown:
+        raise ValueError(f"unknown tangents {sorted(unknown)}; expected some of {HVP_TANGENTS}")
+    shapes = dict(x3d=(B, N, 3), x2d=(B, N, 2), w2d=(B, N, 2), delta=(B,), pose=(B, P, D), cam=(B, 3, 3), lb=(B, 2),
+                  ub=(B, 2), grad=(B, P))
+    if prob.lb is None and (any(tangents.get(k) is not None for k in ("lb", "ub")) or want[7] or want[8]):
+        raise ValueError("a bound's tangent or second-order gradient needs the problem's bounds")
+    tan = []
+    for k in HVP_TANGENTS:
+        t = tangents.get(k)
+        if t is not None:
+            if tuple(t.shape) != shapes[k]:
+                raise ValueError(f"tangent {k} must be {shapes[k]}; got {tuple(t.shape)}")
+            t = _f32c(t)
+        tan.append(t)
+    poses, grad = _f32c(poses), _f32c(grad)
+    outs = [prob.empty(*shapes[k]) if w else None for k, w in zip(HVP_OUTPUTS, want)]
+    with torch.cuda.device(prob.device):
+        check(lib().epnp_cost_hvp_f32(*prob.common_ptrs(), ptr(poses), ptr(grad), P, *(ptr(t) for t in tan),
+                                      *(ptr(o) for o in outs), B, N, int(dof), ctypes.c_float(z_min),
+                                      stream_ptr(prob.device)), "epnp_cost_hvp_f32")
+    return tuple(outs)
+
+
 def gn_plus_camera_backward(prob: Problem, pose, grad_pose_plus, dof, z_min, eps, huber_eps, want=(True, True, True),
                             cluster_ctas=0):
     """dL/d(cam_mats, lb, ub) of pose_opt_plus = pose (+) gn_step(pose) -> (grad_cam (B, 3, 3), grad_lb (B, 2),
@@ -772,4 +814,4 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
 
 __all__ = ["Problem", "adaptive_delta", "cost_backward", "cost_camera_backward", "gn_plus_camera_backward",
            "evaluate_cost", "evaluate_cost_split", "evaluate_full", "evaluate_backward", "lm_solve",
-           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "solve_host", "solve_split_host", "solve_workspace_bytes", "rslm_spec", "epnp_spec", "initial_pose", "rslm", "rslm_split", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]
+           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "solve_host", "solve_split_host", "solve_workspace_bytes", "rslm_spec", "epnp_spec", "initial_pose", "rslm", "rslm_split", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "cost_hvp", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

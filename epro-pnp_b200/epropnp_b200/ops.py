@@ -13,12 +13,14 @@ Seeds of the Philox draws: `seed` (an int) or `seed_t` (a one-element int64 tens
 native's *_seedptr_f32 entry points); seed_t wins when given.
 
 Autograd (register_autograd) is registered on evaluate_cost, evaluate_full, lm_solve (pose_opt_plus), lm_amis_fused and
-mc_epilogue; the backward operators themselves have none.  evaluate_full's residual / Jacobian are first-order only: a
-second backward through them raises.
+mc_epilogue, and for second order on the cost backwards (cost_backward, cost_pose_backward, cost_camera_backward: the
+Hessian-vector product cost_hvp) and on mc_lse_backward.  cost_hvp has none, so a third derivative through the cost
+raises.  evaluate_full's residual / Jacobian and pose_opt_plus are first-order only: a second backward through
+evaluate_backward or the gn_plus backwards raises.
 
 The module's names (adaptive_delta, ..., mc_lse_backward) are the entry points the layer calls (_entry): the operator
-while anything traces, its implementation directly in eager code.  The operators themselves are FORWARD / BACKWARD and
-torch.ops.epropnp.*; each entry point's `.op` is its operator.
+while anything traces, its implementation directly in eager code.  The operators themselves are FORWARD / BACKWARD /
+SECOND_ORDER and torch.ops.epropnp.*; each entry point's `.op` is its operator.
 """
 from typing import List, Optional
 
@@ -409,6 +411,28 @@ def _(x3d, x2d, w2d, cam_mats, lb, ub, delta, poses, dof, z_min, huber_eps, clip
                                    (B, 2)))
 
 
+@_op("cost_hvp")
+def cost_hvp(x3d: Tensor, x2d: Tensor, w2d: Tensor, cam_mats: Tensor, lb: Optional[Tensor], ub: Optional[Tensor],
+             delta: Tensor, poses: Tensor, grad: Tensor, t_x3d: Optional[Tensor], t_x2d: Optional[Tensor],
+             t_w2d: Optional[Tensor], t_delta: Optional[Tensor], t_pose: Optional[Tensor], t_cam: Optional[Tensor],
+             t_lb: Optional[Tensor], t_ub: Optional[Tensor], dof: int, z_min: float,
+             want: List[bool]) -> tuple[Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """native.cost_hvp: poses (B, P, D), grad (B, P) and the tangent's parts (None: zero) -> H v with respect to x3d,
+    x2d, w2d, delta, the poses (times grad), d cost_p . v (B, P), H v with respect to cam_mats, lb, ub."""
+    prob = _problem(x3d, x2d, w2d, cam_mats, lb, ub, delta)
+    tangents = dict(zip(native.HVP_TANGENTS, (t_x3d, t_x2d, t_w2d, t_delta, t_pose, t_cam, t_lb, t_ub)))
+    out = native.cost_hvp(prob, dof, z_min, poses, grad, tangents, tuple(want))
+    return tuple(_or_empty(t, x3d) for t in out)
+
+
+@cost_hvp.register_fake
+def _(x3d, x2d, w2d, cam_mats, lb, ub, delta, poses, grad, t_x3d, t_x2d, t_w2d, t_delta, t_pose, t_cam, t_lb, t_ub,
+      dof, z_min, want):
+    B, N, P = x3d.shape[0], x3d.shape[1], poses.shape[1]
+    return _grad_fakes(x3d, want, ((B, N, 3), (B, N, 2), (B, N, 2), (B,), (B, P, _pose_dim(dof)), (B, P), (B, 3, 3),
+                                   (B, 2), (B, 2)))
+
+
 @_op("mc_lse_backward")
 def mc_lse_backward(logw_bm: Tensor, lse: Tensor, grad_lse: Tensor) -> Tensor:
     """grad_logw (B, M) = grad_lse[b] * exp(logw[b, m] - lse[b]) (native.mc_lse_backward)."""
@@ -457,7 +481,8 @@ def _save_problem(ctx, inputs, extra=()):
 
 
 def _load_problem(ctx, n_extra=0):
-    """-> the seven problem inputs (detached: the backward operators are first-order) and the extra saved tensors."""
+    """-> the seven problem inputs and the extra saved tensors, as saved: under create_graph a formula's backward
+    operators see the graph (the cost backwards have second-order formulas; the others raise)."""
     saved = ctx.saved_tensors
     n = len(saved) - n_extra
     x3d, x2d, w2d, cam_mats, delta = saved[:5]
@@ -484,10 +509,11 @@ def _problem_grads(prob, corr, cam):
 
 
 def _cost_grads(ctx, prob, poses_a, grad_a, poses_b=None, grad_b=None):
-    """Correspondence / delta and camera gradients of sum_p grad[p] * cost(pose p) (two native launches at most)."""
+    """Correspondence / delta and camera gradients of sum_p grad[p] * cost(pose p) (two native launches at most).  The
+    inputs are passed as they are: under create_graph the backward operators' own formulas (_cost_hvp_backward) make
+    these gradients differentiable."""
     want_corr, want_cam = _problem_wants(ctx)
-    d = lambda t: None if t is None else t.detach()
-    p = tuple(d(t) for t in prob)
+    p = prob
     corr = (None,) * 4
     if any(want_corr):
         out = cost_backward(*p, poses_a, grad_a, poses_b, grad_b, ctx.dof, ctx.z_min, list(want_corr))
@@ -507,13 +533,12 @@ def _evaluate_cost_setup(ctx, inputs, output):
 
 def _evaluate_cost_backward(ctx, g_cost):
     prob, (poses,) = _load_problem(ctx, 1)
-    poses_bm = poses.detach().transpose(0, 1).contiguous()                       # object-major (B, S, D)
+    poses_bm = poses.transpose(0, 1).contiguous()                                # object-major (B, S, D)
     g = g_cost.transpose(0, 1).contiguous()                                        # object-major (B, S)
     grads = _cost_grads(ctx, prob, poses_bm, g)
     gpose = None
     if ctx.needs_input_grad[7]:
-        d = tuple(None if t is None else t.detach() for t in prob)
-        gpose = cost_pose_backward(*d, poses_bm, g, ctx.dof, ctx.z_min).transpose(0, 1).to(poses.dtype) \
+        gpose = cost_pose_backward(*prob, poses_bm, g, ctx.dof, ctx.z_min).transpose(0, 1).to(poses.dtype) \
             .reshape(poses.shape)
     return grads + (gpose, None, None)
 
@@ -568,15 +593,14 @@ def _fused_backward(ctx, g_pose, g_cost, g_plus, g_cost_init, g_samples, g_logw)
     poses_b = grad_b = None
     if ctx.has_ci and g_cost_init is not None and g_cost_init.numel() == B:
         cost_init_pose = extra[1]
-        poses_b = cost_init_pose.detach().reshape(B, 1, -1)
+        poses_b = cost_init_pose.reshape(B, 1, -1)
         grad_b = g_cost_init.reshape(B, 1)
     if g_logw is None:
         g_logw = torch.zeros(B, samples.shape[1], device=samples.device)
     grads = _cost_grads(ctx, prob, samples, -g_logw.contiguous(), poses_b, grad_b)
     gpose = None
     if ctx.has_ci and ctx.needs_input_grad[8] and poses_b is not None:
-        d = tuple(None if t is None else t.detach() for t in prob)
-        gpose = cost_pose_backward(*d, poses_b, grad_b, ctx.dof, ctx.z_min)[:, 0].to(extra[1].dtype) \
+        gpose = cost_pose_backward(*prob, poses_b, grad_b, ctx.dof, ctx.z_min)[:, 0].to(extra[1].dtype) \
             .reshape(extra[1].shape)
     return grads + (None, gpose) + (None,) * 10
 
@@ -630,16 +654,87 @@ def _mc_epilogue_backward(ctx, g_lse, g_loss, g_weights, g_score):
     logw_bm, lse = ctx.saved_tensors
     g = None
     if g_lse is not None and ctx.needs_input_grad[0]:
-        g = mc_lse_backward(logw_bm.detach(), lse, g_lse).to(logw_bm.dtype)
+        g = mc_lse_backward(logw_bm, lse, g_lse).to(logw_bm.dtype)
     return (g,) + (None,) * 7
 
 
 _register_autograd(mc_epilogue, _mc_epilogue_backward, _mc_epilogue_setup)
 
 
+# ---------------------------------------------------------------------------------------------- second-order formulas
+def _cost_hvp_setup(ctx, inputs, output):
+    """cost_backward / cost_camera_backward (two pose sets) and cost_pose_backward (one): the problem and the sets."""
+    ctx.set_materialize_grads(False)
+    two_sets = len(inputs) == 14
+    ctx.dof, ctx.z_min = (inputs[11], inputs[12]) if two_sets else (inputs[9], inputs[10])
+    sets = [inputs[7:9]] + ([inputs[9:11]] if two_sets and inputs[9] is not None else [])
+    ctx.n_sets, ctx.n_inputs = len(sets), len(inputs)
+    _save_problem(ctx, inputs, tuple(t for s in sets for t in s))
+
+
+def _cost_hvp_backward(ctx, tangents):
+    """The gradients of a cost backward's inputs from the tangents of its outputs (a dict by native.HVP_TANGENTS name):
+    one cost_hvp over the pose sets laid side by side, then each output back to its input's shape."""
+    prob, extra = _load_problem(ctx, 2 * ctx.n_sets)
+    sets = [extra[2 * i:2 * i + 2] for i in range(ctx.n_sets)]
+    n = ctx.needs_input_grad
+    want_corr, want_cam = _problem_wants(ctx)
+    want_pose = any(n[7 + 2 * i] for i in range(ctx.n_sets))
+    want_grad = any(n[8 + 2 * i] for i in range(ctx.n_sets))
+    want = list(want_corr) + [want_pose, want_grad] + list(want_cam)
+    tangents = {k: t for k, t in tangents.items() if t is not None and t.numel()}
+    if not any(want) or not tangents:
+        return (None,) * ctx.n_inputs
+    poses = torch.cat([s[0] for s in sets], 1) if ctx.n_sets > 1 else sets[0][0]
+    grad = torch.cat([s[1] for s in sets], 1) if ctx.n_sets > 1 else sets[0][1]
+    h = cost_hvp(*prob, poses, grad, *(tangents.get(k) for k in native.HVP_TANGENTS), ctx.dof, ctx.z_min, want)
+    h = [t if w else None for t, w in zip(h, want)]
+    out = list(_problem_grads(prob, h[:4], h[6:]))
+    sizes = [s[1].shape[1] for s in sets]
+    for i, (p, g) in enumerate(sets):
+        lo = sum(sizes[:i])
+        out.append(None if h[4] is None or not n[7 + 2 * i] else h[4][:, lo:lo + sizes[i]].to(p.dtype))
+        out.append(None if h[5] is None or not n[8 + 2 * i] else h[5][:, lo:lo + sizes[i]].to(g.dtype))
+    return tuple(out) + (None,) * (ctx.n_inputs - len(out))
+
+
+def _cost_backward_backward(ctx, v_x3d, v_x2d, v_w2d, v_delta):
+    return _cost_hvp_backward(ctx, dict(x3d=v_x3d, x2d=v_x2d, w2d=v_w2d, delta=v_delta))
+
+
+def _cost_pose_backward_backward(ctx, v_pose):
+    return _cost_hvp_backward(ctx, dict(pose=v_pose))
+
+
+def _cost_camera_backward_backward(ctx, v_cam, v_lb, v_ub):
+    return _cost_hvp_backward(ctx, dict(cam=v_cam, lb=v_lb, ub=v_ub))
+
+
+_register_autograd(cost_backward, _cost_backward_backward, _cost_hvp_setup)
+_register_autograd(cost_pose_backward, _cost_pose_backward_backward, _cost_hvp_setup)
+_register_autograd(cost_camera_backward, _cost_camera_backward_backward, _cost_hvp_setup)
+
+
+def _mc_lse_backward_setup(ctx, inputs, output):
+    ctx.save_for_backward(*inputs)
+
+
+def _mc_lse_backward_backward(ctx, v):
+    """out = grad_lse[b] exp(logw[b, m] - lse[b]) with lse an input of its own (its graph carries the softmax part):
+    torch ops on (B, M), differentiable again."""
+    logw_bm, lse, grad_lse = ctx.saved_tensors
+    w = torch.exp(logw_bm - lse.unsqueeze(1))
+    vo = v * w * grad_lse.unsqueeze(1)
+    return vo, -vo.sum(1), (v * w).sum(1)
+
+
+_register_autograd(mc_lse_backward, _mc_lse_backward_backward, _mc_lse_backward_setup)
+
+
 FORWARD = (adaptive_delta, evaluate_cost, evaluate_full, lm_solve, lm_amis_fused, rslm_draw, rslm, epnp_init, mc_epilogue)
 BACKWARD = (cost_backward, cost_pose_backward, cost_camera_backward, gn_plus_backward, gn_plus_camera_backward,
             evaluate_backward, mc_lse_backward)
+SECOND_ORDER = (cost_hvp,)
 
 
 def _entry(op):
@@ -665,3 +760,4 @@ def _entry(op):
  mc_epilogue) = (_entry(op) for op in FORWARD)
 (cost_backward, cost_pose_backward, cost_camera_backward, gn_plus_backward, gn_plus_camera_backward, evaluate_backward,
  mc_lse_backward) = (_entry(op) for op in BACKWARD)
+cost_hvp = _entry(cost_hvp)

@@ -425,6 +425,26 @@ int epnp_cost_camera_backward_split_f32(const float* x3d, const float* x2d, cons
                                         float* grad_cam, float* grad_lb, float* grad_ub,
                                         int B, int N, int dof, float z_min, int cluster_ctas, void* stream);
 
+/* Second order through the same costs: the Hessian-vector product of f = sum_b sum_p grad[b, p] * cost(poses[b, p]),
+ * which is the backward of the three cost backwards above.  Tangent v [opt, NULL = zero]: t_x3d (B,N,3), t_x2d (B,N,2),
+ * t_w2d (B,N,2), t_delta (B), t_pose (B,P,D), t_cam (B,3,3), t_lb / t_ub (B,2).  Outputs [opt]:
+ *   h_x3d, h_x2d, h_w2d, h_delta, h_cam, h_lb, h_ub   (H v) with respect to the correspondences, delta and the camera
+ *   h_pose (B,P,D)                                    grad[b, p] * (H_p v) with respect to pose p (raw components)
+ *   h_grad (B,P)                                      d cost(poses[b, p]) . v   (the derivative with respect to grad)
+ * The gates are those of the first-order backwards: nothing passes a depth clamped at z_min, a coordinate clamped at a
+ * bound follows that bound, each side of the Huber threshold takes its own branch.  Two launches: point-major (one CTA
+ * per object, fixed-order block reduction) when a problem output is given, pose-major (thread per pose) when h_pose or
+ * h_grad is; both stream the points from global memory, so any N up to epnp_max_points_split(dof, 0, 0) runs, above it
+ * EPNP_ERR_TOO_MANY_POINTS.  No atomics: results are bit-identical from run to run.  Refusals as
+ * epnp_cost_backward_f32 (a single pose set, P >= 0), and t_lb / t_ub / h_lb / h_ub without bounds: EPNP_ERR_BAD_ARG.
+ * B = 0 writes nothing; P = 0 writes zeros to the problem outputs.                                               */
+int epnp_cost_hvp_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                      const float* lb, const float* ub, const float* delta, const float* poses, const float* grad, int P,
+                      const float* t_x3d, const float* t_x2d, const float* t_w2d, const float* t_delta,
+                      const float* t_pose, const float* t_cam, const float* t_lb, const float* t_ub,
+                      float* h_x3d, float* h_x2d, float* h_w2d, float* h_delta, float* h_pose, float* h_grad,
+                      float* h_cam, float* h_lb, float* h_ub, int B, int N, int dof, float z_min, void* stream);
+
 /* The camera gradient of pose_opt_plus = pose (+) gn_step(pose) (epnp_gn_plus_backward_f32's function, differentiated
  * with respect to cam_mats and the bounds instead of the correspondences): grad_cam (B, 3, 3), grad_lb / grad_ub (B, 2),
  * optional with the rules of epnp_cost_camera_backward_f32.  K enters the projection and the Jacobian; the clip mask is
