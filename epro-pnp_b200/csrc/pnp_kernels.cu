@@ -1673,6 +1673,368 @@ __global__ void __launch_bounds__(GNBW_SPLIT_T, 1) gn_plus_camera_backward_split
 }
 
 // ------------------------------------------------------------------------------------------------
+// Second order through pose_opt_plus = pose (+) gn_step(pose): the backward of gn_plus_backward_kernel and
+// gn_plus_camera_backward_kernel.  With f(theta, gplus) = gplus . (pose (+) step(theta)), theta = (x3d, x2d, w2d, delta,
+// K, lb, ub) and the pose detached, those kernels compute grad_theta f.  Along a tangent u of theta this kernel returns
+// H u = d(grad_theta f) / d theta . u for every input of theta, and J u = d pose_opt_plus / d theta . u (the derivative
+// of u . grad_theta f with respect to gplus).  u rides along as a Dual<1> through the whole first-order computation:
+//   1. the normal equations H = sum J~^T J~, g = sum J~^T r~ and their tangents, in one fixed-order block reduction;
+//   2. the serial lane: step and dstep = -(H + eps I)^-1 (dH step + dg); sbar = pose_add_backward(step) and its tangent
+//      (the second derivative of the quaternion normalisation); v = -(H + eps I)^-1 sbar and dv = -(H + eps I)^-1
+//      (dH v + dsbar); J u, pose_add's tangent;
+//   3. thread <-> correspondence: gn_step_vjp's scalar b . (J~ v) + a . (r~ + J~ step), a = J~ v, b = r~ + J~ step, with
+//      its derivatives with respect to the point's inputs and delta (or K and the bounds) carried by a Dual<ND> whose
+//      scalar is itself a Dual<1> (HD<ND>): the value parts are the first-order rows, their tangents the rows of H u.
+// The gates are the first-order kernels': the depth's tangent passes iff zh >= z_min, a clamped coordinate is its bound
+// (value, tangent and seed), the clip mask is constant, and each Huber side keeps its branch, huber_eps included.  A body
+// of its own rather than gn_step_vjp over a generic scalar: that would put a nested Dual through pnp_math.cuh's operators,
+// which every validated backward kernel is built from.  The points stream from global memory, so any N up to
+// epnp_max_points_split runs; no atomics.  The arguments are HvpArgs with grad = gplus (B, D) and hgrad = J u (B, D);
+// the pose fields (tpose, hpose, P) are unused.
+template <int ND> struct HD {
+    D1 v;
+    D1 d[ND];
+};
+template <int ND> __device__ __forceinline__ HD<ND> hd(const D1& c) {
+    HD<ND> r; r.v = c;
+#pragma unroll
+    for (int i = 0; i < ND; ++i) r.d[i] = dual_const<1>(0.f);
+    return r;
+}
+template <int ND> __device__ __forceinline__ HD<ND> hd_seed(const D1& c, int k) {
+    HD<ND> r = hd<ND>(c); r.d[k] = dual_const<1>(1.f); return r;
+}
+template <int ND> __device__ __forceinline__ HD<ND> operator+(const HD<ND>& a, const HD<ND>& b) {
+    HD<ND> r; r.v = a.v + b.v;
+#pragma unroll
+    for (int i = 0; i < ND; ++i) r.d[i] = a.d[i] + b.d[i];
+    return r;
+}
+template <int ND> __device__ __forceinline__ HD<ND> operator-(const HD<ND>& a, const HD<ND>& b) {
+    HD<ND> r; r.v = a.v - b.v;
+#pragma unroll
+    for (int i = 0; i < ND; ++i) r.d[i] = a.d[i] - b.d[i];
+    return r;
+}
+template <int ND> __device__ __forceinline__ HD<ND> operator*(const HD<ND>& a, const HD<ND>& b) {
+    HD<ND> r; r.v = a.v * b.v;
+#pragma unroll
+    for (int i = 0; i < ND; ++i) r.d[i] = a.v * b.d[i] + a.d[i] * b.v;
+    return r;
+}
+template <int ND> __device__ __forceinline__ HD<ND> operator*(const HD<ND>& a, const D1& b) {
+    HD<ND> r; r.v = a.v * b;
+#pragma unroll
+    for (int i = 0; i < ND; ++i) r.d[i] = a.d[i] * b;
+    return r;
+}
+template <int ND> __device__ __forceinline__ HD<ND> operator*(const HD<ND>& a, float c) {
+    HD<ND> r; r.v = a.v * c;
+#pragma unroll
+    for (int i = 0; i < ND; ++i) r.d[i] = a.d[i] * c;
+    return r;
+}
+template <int ND> __device__ __forceinline__ HD<ND> operator+(const HD<ND>& a, const D1& b) { HD<ND> r = a; r.v = a.v + b; return r; }
+template <int ND> __device__ __forceinline__ HD<ND> operator+(const HD<ND>& a, float c) { HD<ND> r = a; r.v = a.v + c; return r; }
+
+// The scalar operations the per-point body below needs, for S = D1 (the normal equations) and S = HD<ND>.
+__device__ __forceinline__ float hval(const D1& a) { return a.v; }
+template <int ND> __device__ __forceinline__ float hval(const HD<ND>& a) { return a.v.v; }
+__device__ __forceinline__ D1 hconst(const D1&, float c) { return dual_const<1>(c); }
+template <int ND> __device__ __forceinline__ HD<ND> hconst(const HD<ND>&, float c) { return hd<ND>(dual_const<1>(c)); }
+__device__ __forceinline__ D1 hlift(const D1&, const D1& w) { return w; }
+template <int ND> __device__ __forceinline__ HD<ND> hlift(const HD<ND>&, const D1& w) { return hd<ND>(w); }
+__device__ __forceinline__ D1 hgate(const D1& a, float value, bool pass) { return dual_gate(a, value, pass); }
+template <int ND> __device__ __forceinline__ HD<ND> hgate(const HD<ND>& a, float value, bool pass) {
+    HD<ND> r; r.v = dual_gate(a.v, value, pass);
+#pragma unroll
+    for (int i = 0; i < ND; ++i) r.d[i] = pass ? a.d[i] : dual_const<1>(0.f);
+    return r;
+}
+__device__ __forceinline__ D1 hrecip(const D1& a) { return dual_recip(a); }
+template <int ND> __device__ __forceinline__ HD<ND> hrecip(const HD<ND>& a) {
+    HD<ND> r; r.v = dual_recip(a.v);
+    const D1 k = r.v * r.v * -1.f;
+#pragma unroll
+    for (int i = 0; i < ND; ++i) r.d[i] = a.d[i] * k;
+    return r;
+}
+__device__ __forceinline__ D1 hsqrt(const D1& a) { return dual_sqrt(a); }
+template <int ND> __device__ __forceinline__ HD<ND> hsqrt(const HD<ND>& a) {            // a > 0
+    HD<ND> r; r.v = dual_sqrt(a.v);
+    const D1 k = dual_recip(r.v) * 0.5f;
+#pragma unroll
+    for (int i = 0; i < ND; ++i) r.d[i] = a.d[i] * k;
+    return r;
+}
+
+// One correspondence at the detached pose (R, t), in the scalar S: the rotated point, the (clamped) projection and its
+// inverse depth, the Huber-scaled residual r~ and the row factors wu sqrt(rho') / wv sqrt(rho') (0 on a clipped row).
+template <class S> struct GnPt { S xr, yr, zr, iz, px, py, rx, ry, sx, sy; };
+
+template <class S>
+__device__ __forceinline__ void gn_pt_eval(const float (&R)[9], const float (&t)[3], const S (&K)[9], const S (&bnd)[4],
+                                           const Cam& c, const S& delta, float huber_eps, const S (&pt)[7], GnPt<S>& o) {
+    const S &X = pt[0], &Y = pt[1], &Z = pt[2], &u = pt[3], &v = pt[4], &wu = pt[5], &wv = pt[6];
+    o.xr = X * R[0] + Y * R[1] + Z * R[2];
+    o.yr = X * R[3] + Y * R[4] + Z * R[5];
+    o.zr = X * R[6] + Y * R[7] + Z * R[8];
+    const S xc = o.xr + t[0], yc = o.yr + t[1], zc = o.zr + t[2];
+    const S xh = K[0] * xc + K[1] * yc + K[2] * zc;
+    const S yh = K[3] * xc + K[4] * yc + K[5] * zc;
+    const S zh = K[6] * xc + K[7] * yc + K[8] * zc;
+    const float z = fmaxf(hval(zh), c.z_min);
+    o.iz = hrecip(hgate(zh, z, hval(zh) >= c.z_min));
+    o.px = xh * o.iz; o.py = yh * o.iz;
+    if (c.bounded) {
+        const float cx = fminf(fmaxf(hval(o.px), c.lbx), c.ubx), cy = fminf(fmaxf(hval(o.py), c.lby), c.uby);
+        if (cx != hval(o.px)) o.px = cx == c.ubx ? bnd[2] : bnd[0];
+        if (cy != hval(o.py)) o.py = cy == c.uby ? bnd[3] : bnd[1];
+    }
+    const S rx = (o.px - u) * wu, ry = (o.py - v) * wv;
+    const S s2 = rx * rx + ry * ry;
+    const float s = sqrtf(hval(s2)), dl = hval(delta);
+    S sc = hconst(s2, 1.0f);                                // sqrt(rho') = sqrt(min(delta / max(s, eps), 1))
+    if (!(s <= dl && dl >= huber_eps)) {
+        const float sm = fmaxf(s, huber_eps);
+        if (dl / sm < 1.0f) {
+            const S sd = (s >= huber_eps && s > 0.f) ? hsqrt(s2) : hconst(s2, sm);
+            sc = hsqrt(delta * hrecip(sd));
+        }
+    }
+    o.rx = rx * sc; o.ry = ry * sc;
+    const bool cz = z == c.z_min;
+    const bool clip_x = cz || (c.bounded && (hval(o.px) == c.lbx || hval(o.px) == c.ubx));
+    const bool clip_y = cz || (c.bounded && (hval(o.py) == c.lby || hval(o.py) == c.uby));
+    o.sx = clip_x ? hconst(sc, 0.f) : wu * sc;
+    o.sy = clip_y ? hconst(sc, 0.f) : wv * sc;
+}
+
+// (J~ w)_u and (J~ w)_v of that correspondence for a DOF-vector w
+template <int DOF, class S>
+__device__ __forceinline__ void gn_pt_jrow(const GnPt<S>& p, const S (&K)[9], const D1 (&w)[DOF], S& ju, S& jv) {
+    S mx, my, mz;
+    if constexpr (DOF == 6) {
+        mx = (p.yr * w[5] - p.zr * w[4]) * 2.0f + w[0];
+        my = (p.zr * w[3] - p.xr * w[5]) * 2.0f + w[1];
+        mz = (p.xr * w[4] - p.yr * w[3]) * 2.0f + w[2];
+    } else {
+        mx = p.zr * w[3] + w[0];
+        my = hlift(p.zr, w[1]);
+        mz = p.xr * (w[3] * -1.f) + w[2];
+    }
+    ju = (K[0] * mx + K[1] * my + (K[2] - p.px) * mz) * p.iz * p.sx;
+    jv = (K[3] * mx + K[4] * my + (K[5] - p.py) * mz) * p.iz * p.sy;
+}
+
+// hv[k] += the tangent of d(b . (J~ v) + a . (r~ + J~ step)) / d(seed k), a and b held at their values and tangents
+template <int DOF, int ND>
+__device__ __forceinline__ void gn_pt_hvp(const float (&R)[9], const float (&t)[3], const HD<ND> (&K)[9],
+                                          const HD<ND> (&bnd)[4], const Cam& c, const HD<ND>& delta, float huber_eps,
+                                          const HD<ND> (&pt)[7], const D1 (&sv)[DOF], const D1 (&vv)[DOF],
+                                          float (&hv)[ND]) {
+    GnPt<HD<ND>> p;
+    gn_pt_eval(R, t, K, bnd, c, delta, huber_eps, pt, p);
+    HD<ND> Au, Av, Bu, Bv;
+    gn_pt_jrow<DOF>(p, K, vv, Au, Av);
+    gn_pt_jrow<DOF>(p, K, sv, Bu, Bv);
+    const D1 au = Au.v, av = Av.v, bu = p.rx.v + Bu.v, bv = p.ry.v + Bv.v;
+#pragma unroll
+    for (int k = 0; k < ND; ++k)
+        hv[k] += (bu * Au.d[k] + au * (p.rx.d[k] + Bu.d[k]) + bv * Av.d[k] + av * (p.ry.d[k] + Bv.d[k])).d[0];
+}
+
+// pose (+) step and pose_add_backward with the step carrying its tangent (the pose and gplus are constants)
+template <int DOF>
+__device__ __forceinline__ void gn_hvp_quat(const float* pose, const D1* step, D1 (&q)[4], D1& inv) {
+    const float w = pose[3], x = pose[4], y = pose[5], z = pose[6];
+    const D1 &a = step[3], &b = step[4], &c = step[5];
+    q[0] = (a * x + b * y + c * z) + w;
+    q[1] = (a * -w + b * -z + c * y) + x;
+    q[2] = (a * z + b * -w + c * -x) + y;
+    q[3] = (a * -y + b * x + c * -w) + z;
+    const D1 n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+    inv = dual_recip(sqrtf(n2.v) > 1e-12f ? dual_sqrt(n2) : dual_const<1>(1e-12f));
+}
+
+template <int DOF>
+__device__ __forceinline__ void gn_hvp_pose_add(const float* pose, const D1* step, D1* out) {
+#pragma unroll
+    for (int i = 0; i < 3; ++i) out[i] = step[i] + pose[i];
+    if constexpr (DOF == 4) {
+        out[3] = step[3] + pose[3];
+    } else {
+        D1 q[4], inv;
+        gn_hvp_quat<DOF>(pose, step, q, inv);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) out[3 + i] = q[i] * inv;
+    }
+}
+
+template <int DOF>
+__device__ __forceinline__ void gn_hvp_pose_add_backward(const float* pose, const D1* step, const float* gout, D1* gstep) {
+#pragma unroll
+    for (int i = 0; i < 3; ++i) gstep[i] = dual_const<1>(gout[i]);
+    if constexpr (DOF == 4) {
+        gstep[3] = dual_const<1>(gout[3]);
+    } else {
+        const float w = pose[3], x = pose[4], y = pose[5], z = pose[6];
+        D1 q[4], inv;
+        gn_hvp_quat<DOF>(pose, step, q, inv);
+        const D1 dot = (q[0] * gout[3] + q[1] * gout[4] + q[2] * gout[5] + q[3] * gout[6]) * inv * inv;
+        D1 gq[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) gq[i] = (q[i] * dot * -1.f + gout[3 + i]) * inv;
+        gstep[3] = gq[0] * x + gq[1] * -w + gq[2] * z + gq[3] * -y;
+        gstep[4] = gq[0] * y + gq[1] * -z + gq[2] * -w + gq[3] * x;
+        gstep[5] = gq[0] * z + gq[1] * y + gq[2] * -x + gq[3] * -w;
+    }
+}
+
+// out = dH w + r, dH packed upper-triangular
+template <int DOF>
+__device__ __forceinline__ void gn_hvp_rhs(const float* dh, const float* w, const float* r, float* out) {
+#pragma unroll
+    for (int i = 0; i < DOF; ++i) {
+        float s = r[i];
+#pragma unroll
+        for (int j = 0; j < DOF; ++j) s = fmaf(dh[i <= j ? tri(i, j, DOF) : tri(j, i, DOF)], w[j], s);
+        out[i] = s;
+    }
+}
+
+template <int DOF>
+__global__ void __launch_bounds__(NT) gn_plus_hvp_kernel(const HvpArgs g) {
+    constexpr int PD = Dim<DOF>::POSE, NA = Dim<DOF>::NA, NG = NA + DOF;
+    __shared__ float red[2 * NW * 32];
+    __shared__ float sh[4 * DOF];                           // step, dstep, v, dv
+    const KArgs& a = g.k;
+    const int obj = blockIdx.x, tid = threadIdx.x;
+    Cam cam;
+    D1 K[9], bnd[4], delta;
+    hvp_object(g, obj, cam, K, bnd, delta);
+    float pose[PD], R[9], t[3];
+#pragma unroll
+    for (int i = 0; i < PD; ++i) pose[i] = __ldg(a.poses + (size_t)obj * PD + i);
+    pose_to_rot<DOF>(pose, R);
+    t[0] = pose[0]; t[1] = pose[1]; t[2] = pose[2];
+    // 1. H, g (packed as eval_normal_eq's ev, without the cost) and their tangents
+    float hv[NG], ht[NG];
+#pragma unroll
+    for (int k = 0; k < NG; ++k) { hv[k] = 0.f; ht[k] = 0.f; }
+    for (int n = tid; n < a.N; n += NT) {
+        D1 pt[7];
+        hvp_point(g, (size_t)obj * a.N + n, pt);
+        GnPt<D1> p;
+        gn_pt_eval(R, t, K, bnd, cam, delta, a.p.huber_eps, pt, p);
+        D1 ju[DOF], jv[DOF];
+#pragma unroll
+        for (int i = 0; i < DOF; ++i) {
+            D1 e[DOF];
+#pragma unroll
+            for (int j = 0; j < DOF; ++j) e[j] = dual_const<1>(i == j ? 1.f : 0.f);
+            gn_pt_jrow<DOF>(p, K, e, ju[i], jv[i]);
+        }
+        int idx = 0;
+#pragma unroll
+        for (int i = 0; i < DOF; ++i) {
+#pragma unroll
+            for (int k = i; k < DOF; ++k) {
+                const D1 h = ju[i] * ju[k] + jv[i] * jv[k];
+                hv[idx] += h.v; ht[idx] += h.d[0]; ++idx;
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < DOF; ++i) {
+            const D1 gi = ju[i] * p.rx + jv[i] * p.ry;
+            hv[NA + i] += gi.v; ht[NA + i] += gi.d[0];
+        }
+    }
+    block_sum<NG>(hv, red, 0);
+    block_sum<NG>(ht, red, 1);
+    // 2. the serial lane
+    if (tid == 0) {
+        float add[DOF], st[DOF], ds[DOF], vv[DOF], dv[DOF], rhs[DOF], sb[DOF], gout[PD];
+#pragma unroll
+        for (int i = 0; i < DOF; ++i) add[i] = a.p.eps;
+#pragma unroll
+        for (int i = 0; i < PD; ++i) gout[i] = __ldg(g.grad + (size_t)obj * PD + i);
+        damped_step_refined<DOF>(hv, hv + NA, add, st);
+        gn_hvp_rhs<DOF>(ht, st, ht + NA, rhs);
+        damped_step_refined<DOF>(hv, rhs, add, ds);
+        D1 step[DOF], sbar[DOF];
+#pragma unroll
+        for (int i = 0; i < DOF; ++i) step[i] = d1(st[i], ds[i]);
+        gn_hvp_pose_add_backward<DOF>(pose, step, gout, sbar);
+#pragma unroll
+        for (int i = 0; i < DOF; ++i) { sb[i] = sbar[i].v; rhs[i] = sbar[i].d[0]; }
+        damped_step_refined<DOF>(hv, sb, add, vv);
+        gn_hvp_rhs<DOF>(ht, vv, rhs, rhs);
+        damped_step_refined<DOF>(hv, rhs, add, dv);
+        if (g.hgrad) {
+            D1 plus[PD];
+            gn_hvp_pose_add<DOF>(pose, step, plus);
+#pragma unroll
+            for (int i = 0; i < PD; ++i) g.hgrad[(size_t)obj * PD + i] = plus[i].d[0];
+        }
+#pragma unroll
+        for (int i = 0; i < DOF; ++i) { sh[i] = st[i]; sh[DOF + i] = ds[i]; sh[2 * DOF + i] = vv[i]; sh[3 * DOF + i] = dv[i]; }
+    }
+    __syncthreads();
+    // 3. thread <-> correspondence
+    D1 sv[DOF], vv[DOF];
+#pragma unroll
+    for (int i = 0; i < DOF; ++i) { sv[i] = d1(sh[i], sh[DOF + i]); vv[i] = d1(sh[2 * DOF + i], sh[3 * DOF + i]); }
+    const bool pts_out = g.hx3d || g.hx2d || g.hw2d || g.hdelta, cam_out = g.hcam || g.hlb || g.hub;
+    float acc[1 + CAM_GRADS];                               // delta, K (row-major), lbx lby ubx uby
+#pragma unroll
+    for (int k = 0; k < 1 + CAM_GRADS; ++k) acc[k] = 0.f;
+    for (int n = tid; n < a.N; n += NT) {
+        const size_t q = (size_t)obj * a.N + n;
+        D1 pt[7];
+        hvp_point(g, q, pt);
+        if (pts_out) {
+            HD<8> P[7], Kh[9], Bh[4];
+#pragma unroll
+            for (int k = 0; k < 7; ++k) P[k] = hd_seed<8>(pt[k], k);
+#pragma unroll
+            for (int k = 0; k < 9; ++k) Kh[k] = hd<8>(K[k]);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) Bh[k] = hd<8>(bnd[k]);
+            float hp[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+            gn_pt_hvp<DOF, 8>(R, t, Kh, Bh, cam, hd_seed<8>(delta, 7), a.p.huber_eps, P, sv, vv, hp);
+            if (g.hx3d) { g.hx3d[q * 3] = hp[0]; g.hx3d[q * 3 + 1] = hp[1]; g.hx3d[q * 3 + 2] = hp[2]; }
+            if (g.hx2d) { g.hx2d[q * 2] = hp[3]; g.hx2d[q * 2 + 1] = hp[4]; }
+            if (g.hw2d) { g.hw2d[q * 2] = hp[5]; g.hw2d[q * 2 + 1] = hp[6]; }
+            acc[0] += hp[7];
+        }
+        if (cam_out) {
+            HD<CAM_GRADS> P[7], Kh[9], Bh[4];
+#pragma unroll
+            for (int k = 0; k < 7; ++k) P[k] = hd<CAM_GRADS>(pt[k]);
+#pragma unroll
+            for (int k = 0; k < 9; ++k) Kh[k] = hd_seed<CAM_GRADS>(K[k], k);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) Bh[k] = hd_seed<CAM_GRADS>(bnd[k], 9 + k);
+            float hc[CAM_GRADS];
+#pragma unroll
+            for (int k = 0; k < CAM_GRADS; ++k) hc[k] = 0.f;
+            gn_pt_hvp<DOF, CAM_GRADS>(R, t, Kh, Bh, cam, hd<CAM_GRADS>(delta), a.p.huber_eps, P, sv, vv, hc);
+#pragma unroll
+            for (int k = 0; k < CAM_GRADS; ++k) acc[1 + k] += hc[k];
+        }
+    }
+    block_sum<1 + CAM_GRADS>(acc, red, 0);
+    if (tid == 0) {
+        if (g.hdelta) g.hdelta[obj] = acc[0];
+        float cg[CAM_GRADS];
+#pragma unroll
+        for (int k = 0; k < CAM_GRADS; ++k) cg[k] = acc[1 + k];
+        store_camera_grad(g.hcam, g.hlb, g.hub, obj, cg);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Backward of evaluate_full_kernel's residual, Jacobian and cost at S stacked poses (S, B, D): the vector-Jacobian
 // product with any of the upstream gradients g_res (S, B, 2N), g_jac (S, B, 2N, DOF) and g_cost (S, B), differentiated
 // per (pose, point) by the three forms of point_residual_jac_backward (pnp_math.cuh).  One CTA per object, the points
@@ -2861,6 +3223,32 @@ int epnp_gn_plus_camera_backward_split_f32(const float* x3d, const float* x2d, c
     return by_dof(dof, [&](auto D) {
         return launch_cluster<GNBW_SPLIT_T>(gn_plus_camera_backward_split_kernel<D>, g, B, smem_bytes, ctas,
                                             (cudaStream_t)stream);
+    });
+}
+
+int epnp_gn_plus_hvp_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                         const float* lb, const float* ub, const float* delta, const float* pose,
+                         const float* grad_pose_plus, const float* t_x3d, const float* t_x2d, const float* t_w2d,
+                         const float* t_delta, const float* t_cam, const float* t_lb, const float* t_ub,
+                         float* h_x3d, float* h_x2d, float* h_w2d, float* h_delta, float* h_cam, float* h_lb,
+                         float* h_ub, float* h_grad, int B, int N, int dof, float z_min, float eps, float huber_eps,
+                         void* stream) {
+    GnBwArgs gb{};
+    const int rc = gn_bw_args(gb, x3d, x2d, w2d, cam_mats, lb, ub, delta, pose, grad_pose_plus, nullptr, nullptr,
+                              nullptr, nullptr, B, N, dof, z_min, eps, huber_eps);
+    if (rc != EPNP_OK) return rc;
+    if (!lb && (t_lb || t_ub || h_lb || h_ub)) return EPNP_ERR_BAD_ARG;
+    if (B == 0) return EPNP_OK;
+    if (N > epnp_max_points_split(dof, 0, 0)) return EPNP_ERR_TOO_MANY_POINTS;
+    HvpArgs g{};
+    g.k = gb.k;
+    g.grad = grad_pose_plus;
+    g.tx3d = t_x3d; g.tx2d = t_x2d; g.tw2d = t_w2d; g.tdelta = t_delta; g.tcam = t_cam; g.tlb = t_lb; g.tub = t_ub;
+    g.hx3d = h_x3d; g.hx2d = h_x2d; g.hw2d = h_w2d; g.hdelta = h_delta; g.hcam = h_cam; g.hlb = h_lb; g.hub = h_ub;
+    g.hgrad = h_grad;
+    if (!(h_x3d || h_x2d || h_w2d || h_delta || h_cam || h_lb || h_ub || h_grad)) return EPNP_OK;
+    return by_dof(dof, [&](auto D) {
+        return launch_plain(gn_plus_hvp_kernel<D>, B, NT, 0, SmemAttr::none, (cudaStream_t)stream, g);
     });
 }
 

@@ -88,6 +88,7 @@ _SIGNATURES = {
                                             + [_I, _I, _I, _F, _I, _P]),
     "epnp_cost_hvp_f32": (ctypes.c_int, [_P] * 9 + [_I] + [_P] * 8 + [_P] * 9 + [_I, _I, _I, _F, _P]),
     "epnp_gn_plus_camera_backward_f32": (ctypes.c_int, [_P] * 12 + [_I, _I, _I, _F, _F, _F, _P]),
+    "epnp_gn_plus_hvp_f32": (ctypes.c_int, [_P] * 9 + [_P] * 7 + [_P] * 8 + [_I, _I, _I, _F, _F, _F, _P]),
     "epnp_gn_plus_camera_backward_split_f32": (ctypes.c_int, [_P] * 12 + [_I, _I, _I, _F, _F, _F, _I, _P]),
     "epnp_mc_epilogue_f32": (ctypes.c_int, [_P] * 8 + [_I, _I, _I, _P]),
     "epnp_mc_lse_backward_f32": (ctypes.c_int, [_P] * 4 + [_I, _I, _P]),

@@ -634,6 +634,47 @@ def gn_plus_camera_backward(prob: Problem, pose, grad_pose_plus, dof, z_min, eps
     return gcam, glb, gub
 
 
+GN_HVP_TANGENTS = ("x3d", "x2d", "w2d", "delta", "cam", "lb", "ub")
+GN_HVP_OUTPUTS = ("x3d", "x2d", "w2d", "delta", "cam", "lb", "ub", "grad")
+
+
+def gn_plus_hvp(prob: Problem, pose, grad_pose_plus, dof, z_min, eps, huber_eps, tangents, want):
+    """Second order through pose_opt_plus = pose (+) gn_step(pose) (epnp_gn_plus_hvp_f32): for f = grad_pose_plus .
+    pose_opt_plus as a function of the problem inputs (the pose held constant) and a tangent u of those inputs,
+    `tangents` by name (GN_HVP_TANGENTS; missing or None: zero) shaped (B, N, 3), (B, N, 2), (B, N, 2), (B), (B, 3, 3),
+    (B, 2), (B, 2).  `want`: eight flags in GN_HVP_OUTPUTS order.  Returns H u with respect to x3d, x2d, w2d, delta,
+    cam_mats, lb, ub and d pose_opt_plus . u (B, D); None where `want` is False."""
+    B, N = prob.B, prob.N
+    D = 7 if dof == 6 else 4
+    _check_pose(pose, (B,), D, "pose")
+    _check_pose(grad_pose_plus, (B,), D, "grad_pose_plus")
+    if len(want) != len(GN_HVP_OUTPUTS):
+        raise ValueError(f"want: {len(GN_HVP_OUTPUTS)} flags ({', '.join(GN_HVP_OUTPUTS)})")
+    unknown = set(tangents) - set(GN_HVP_TANGENTS)
+    if unknown:
+        raise ValueError(f"unknown tangents {sorted(unknown)}; expected some of {GN_HVP_TANGENTS}")
+    shapes = dict(x3d=(B, N, 3), x2d=(B, N, 2), w2d=(B, N, 2), delta=(B,), cam=(B, 3, 3), lb=(B, 2), ub=(B, 2),
+                  grad=(B, D))
+    if prob.lb is None and (any(tangents.get(k) is not None for k in ("lb", "ub")) or want[5] or want[6]):
+        raise ValueError("a bound's tangent or second-order gradient needs the problem's bounds")
+    tan = []
+    for k in GN_HVP_TANGENTS:
+        t = tangents.get(k)
+        if t is not None:
+            if tuple(t.shape) != shapes[k]:
+                raise ValueError(f"tangent {k} must be {shapes[k]}; got {tuple(t.shape)}")
+            t = _f32c(t)
+        tan.append(t)
+    pose, gp = _f32c(pose), _f32c(grad_pose_plus)
+    outs = [prob.empty(*shapes[k]) if w else None for k, w in zip(GN_HVP_OUTPUTS, want)]
+    with torch.cuda.device(prob.device):
+        check(lib().epnp_gn_plus_hvp_f32(*prob.common_ptrs(), ptr(pose), ptr(gp), *(ptr(t) for t in tan),
+                                         *(ptr(o) for o in outs), B, N, int(dof), ctypes.c_float(z_min),
+                                         ctypes.c_float(eps), ctypes.c_float(huber_eps), stream_ptr(prob.device)),
+              "epnp_gn_plus_hvp_f32")
+    return tuple(outs)
+
+
 def fused_workspace_bytes(B, N, params):
     return int(lib().epnp_fused_workspace_bytes(B, N, ctypes.byref(params)))
 
@@ -814,4 +855,4 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
 
 __all__ = ["Problem", "adaptive_delta", "cost_backward", "cost_camera_backward", "gn_plus_camera_backward",
            "evaluate_cost", "evaluate_cost_split", "evaluate_full", "evaluate_backward", "lm_solve",
-           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "solve_host", "solve_split_host", "solve_workspace_bytes", "rslm_spec", "epnp_spec", "initial_pose", "rslm", "rslm_split", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "cost_hvp", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]
+           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "solve_host", "solve_split_host", "solve_workspace_bytes", "rslm_spec", "epnp_spec", "initial_pose", "rslm", "rslm_split", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "cost_hvp", "gn_plus_hvp", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

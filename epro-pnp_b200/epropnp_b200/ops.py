@@ -14,9 +14,9 @@ native's *_seedptr_f32 entry points); seed_t wins when given.
 
 Autograd (register_autograd) is registered on evaluate_cost, evaluate_full, lm_solve (pose_opt_plus), lm_amis_fused and
 mc_epilogue, and for second order on the cost backwards (cost_backward, cost_pose_backward, cost_camera_backward: the
-Hessian-vector product cost_hvp) and on mc_lse_backward.  cost_hvp has none, so a third derivative through the cost
-raises.  evaluate_full's residual / Jacobian and pose_opt_plus are first-order only: a second backward through
-evaluate_backward or the gn_plus backwards raises.
+Hessian-vector product cost_hvp), on the pose_opt_plus backwards (gn_plus_backward, gn_plus_camera_backward: the
+Hessian-vector product gn_plus_hvp) and on mc_lse_backward.  cost_hvp and gn_plus_hvp have none, so a third derivative
+raises.  evaluate_full's residual / Jacobian are first-order only: a second backward through evaluate_backward raises.
 
 The module's names (adaptive_delta, ..., mc_lse_backward) are the entry points the layer calls (_entry): the operator
 while anything traces, its implementation directly in eager code.  The operators themselves are FORWARD / BACKWARD /
@@ -433,6 +433,28 @@ def _(x3d, x2d, w2d, cam_mats, lb, ub, delta, poses, grad, t_x3d, t_x2d, t_w2d, 
                                    (B, 2), (B, 2)))
 
 
+@_op("gn_plus_hvp")
+def gn_plus_hvp(x3d: Tensor, x2d: Tensor, w2d: Tensor, cam_mats: Tensor, lb: Optional[Tensor], ub: Optional[Tensor],
+                delta: Tensor, pose: Tensor, grad_pose_plus: Tensor, t_x3d: Optional[Tensor], t_x2d: Optional[Tensor],
+                t_w2d: Optional[Tensor], t_delta: Optional[Tensor], t_cam: Optional[Tensor], t_lb: Optional[Tensor],
+                t_ub: Optional[Tensor], dof: int, z_min: float, eps: float, huber_eps: float,
+                want: List[bool]) -> tuple[Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """native.gn_plus_hvp: the tangent's parts (None: zero) -> H u with respect to x3d, x2d, w2d, delta, cam_mats, lb,
+    ub of f = grad_pose_plus . pose_opt_plus, and d pose_opt_plus . u (B, D)."""
+    prob = _problem(x3d, x2d, w2d, cam_mats, lb, ub, delta)
+    tangents = dict(zip(native.GN_HVP_TANGENTS, (t_x3d, t_x2d, t_w2d, t_delta, t_cam, t_lb, t_ub)))
+    out = native.gn_plus_hvp(prob, pose, grad_pose_plus, dof, z_min, eps, huber_eps, tangents, tuple(want))
+    return tuple(_or_empty(t, x3d) for t in out)
+
+
+@gn_plus_hvp.register_fake
+def _(x3d, x2d, w2d, cam_mats, lb, ub, delta, pose, grad_pose_plus, t_x3d, t_x2d, t_w2d, t_delta, t_cam, t_lb, t_ub,
+      dof, z_min, eps, huber_eps, want):
+    B, N = x3d.shape[0], x3d.shape[1]
+    return _grad_fakes(x3d, want, ((B, N, 3), (B, N, 2), (B, N, 2), (B,), (B, 3, 3), (B, 2), (B, 2),
+                                   (B, _pose_dim(dof))))
+
+
 @_op("mc_lse_backward")
 def mc_lse_backward(logw_bm: Tensor, lse: Tensor, grad_lse: Tensor) -> Tensor:
     """grad_logw (B, M) = grad_lse[b] * exp(logw[b, m] - lse[b]) (native.mc_lse_backward)."""
@@ -482,7 +504,7 @@ def _save_problem(ctx, inputs, extra=()):
 
 def _load_problem(ctx, n_extra=0):
     """-> the seven problem inputs and the extra saved tensors, as saved: under create_graph a formula's backward
-    operators see the graph (the cost backwards have second-order formulas; the others raise)."""
+    operators see the graph (the cost and pose_opt_plus backwards have second-order formulas; the others raise)."""
     saved = ctx.saved_tensors
     n = len(saved) - n_extra
     x3d, x2d, w2d, cam_mats, delta = saved[:5]
@@ -610,19 +632,20 @@ _register_autograd(lm_amis_fused, _fused_backward, _fused_setup)
 
 def gn_plus_grads(prob, pose, grad_plus, dof, z_min, eps, huber_eps, needs):
     """Gradients of the seven problem inputs (argument order; None where `needs` is False) through pose_opt_plus =
-    pose (+) gn_step(pose): the gn_plus backward operators, then the reduction to each input's shape."""
+    pose (+) gn_step(pose): the gn_plus backward operators, then the reduction to each input's shape.  The problem
+    inputs and grad_plus are passed as they are (the pose detached): under create_graph the backward operators' own
+    formulas (_gn_plus_hvp_backward) make these gradients differentiable."""
     lb_ub = prob[4] is not None and prob[5] is not None
     corr_w = (needs[0], needs[1], needs[2], needs[6])
     cam_w = (needs[3], lb_ub and needs[4], lb_ub and needs[5])
-    d = tuple(None if t is None else t.detach() for t in prob)
     pose = pose.detach()
     corr = (None,) * 4
     if any(corr_w):
-        out = gn_plus_backward(*d, pose, grad_plus, dof, z_min, eps, huber_eps, list(corr_w))
+        out = gn_plus_backward(*prob, pose, grad_plus, dof, z_min, eps, huber_eps, list(corr_w))
         corr = tuple(t if w else None for t, w in zip(out, corr_w))
     cam = (None,) * 3
     if any(cam_w):
-        out = gn_plus_camera_backward(*d, pose, grad_plus, dof, z_min, eps, huber_eps, list(cam_w))
+        out = gn_plus_camera_backward(*prob, pose, grad_plus, dof, z_min, eps, huber_eps, list(cam_w))
         cam = tuple(t if w else None for t, w in zip(out, cam_w))
     return _problem_grads(prob, corr, cam)
 
@@ -715,6 +738,40 @@ _register_autograd(cost_pose_backward, _cost_pose_backward_backward, _cost_hvp_s
 _register_autograd(cost_camera_backward, _cost_camera_backward_backward, _cost_hvp_setup)
 
 
+def _gn_plus_hvp_setup(ctx, inputs, output):
+    """gn_plus_backward / gn_plus_camera_backward: the problem, the (detached) pose and grad_pose_plus."""
+    ctx.set_materialize_grads(False)
+    ctx.consts = inputs[9:13]                                                  # dof, z_min, eps, huber_eps
+    _save_problem(ctx, inputs, inputs[7:9])
+
+
+def _gn_plus_hvp_backward(ctx, tangents):
+    """The gradients of a pose_opt_plus backward's inputs from the tangents of its outputs (a dict by
+    native.GN_HVP_TANGENTS name): one gn_plus_hvp, then each output back to its input's shape.  The pose gets none."""
+    prob, (pose, grad_plus) = _load_problem(ctx, 2)
+    want_corr, want_cam = _problem_wants(ctx)
+    want = list(want_corr) + list(want_cam) + [ctx.needs_input_grad[8]]
+    tangents = {k: t for k, t in tangents.items() if t is not None and t.numel()}
+    if not any(want) or not tangents:
+        return (None,) * 14
+    h = gn_plus_hvp(*prob, pose, grad_plus, *(tangents.get(k) for k in native.GN_HVP_TANGENTS), *ctx.consts, want)
+    h = [t if w else None for t, w in zip(h, want)]
+    g_plus = None if h[7] is None else h[7].to(grad_plus.dtype)
+    return _problem_grads(prob, h[:4], h[4:7]) + (None, g_plus) + (None,) * 5
+
+
+def _gn_plus_backward_backward(ctx, v_x3d, v_x2d, v_w2d, v_delta):
+    return _gn_plus_hvp_backward(ctx, dict(x3d=v_x3d, x2d=v_x2d, w2d=v_w2d, delta=v_delta))
+
+
+def _gn_plus_camera_backward_backward(ctx, v_cam, v_lb, v_ub):
+    return _gn_plus_hvp_backward(ctx, dict(cam=v_cam, lb=v_lb, ub=v_ub))
+
+
+_register_autograd(gn_plus_backward, _gn_plus_backward_backward, _gn_plus_hvp_setup)
+_register_autograd(gn_plus_camera_backward, _gn_plus_camera_backward_backward, _gn_plus_hvp_setup)
+
+
 def _mc_lse_backward_setup(ctx, inputs, output):
     ctx.save_for_backward(*inputs)
 
@@ -734,7 +791,7 @@ _register_autograd(mc_lse_backward, _mc_lse_backward_backward, _mc_lse_backward_
 FORWARD = (adaptive_delta, evaluate_cost, evaluate_full, lm_solve, lm_amis_fused, rslm_draw, rslm, epnp_init, mc_epilogue)
 BACKWARD = (cost_backward, cost_pose_backward, cost_camera_backward, gn_plus_backward, gn_plus_camera_backward,
             evaluate_backward, mc_lse_backward)
-SECOND_ORDER = (cost_hvp,)
+SECOND_ORDER = (cost_hvp, gn_plus_hvp)
 
 
 def _entry(op):
@@ -760,4 +817,4 @@ def _entry(op):
  mc_epilogue) = (_entry(op) for op in FORWARD)
 (cost_backward, cost_pose_backward, cost_camera_backward, gn_plus_backward, gn_plus_camera_backward, evaluate_backward,
  mc_lse_backward) = (_entry(op) for op in BACKWARD)
-cost_hvp = _entry(cost_hvp)
+cost_hvp, gn_plus_hvp = (_entry(op) for op in SECOND_ORDER)

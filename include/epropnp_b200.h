@@ -463,6 +463,27 @@ int epnp_gn_plus_camera_backward_split_f32(const float* x3d, const float* x2d, c
                                            float* grad_ub, int B, int N, int dof, float z_min, float eps,
                                            float huber_eps, int cluster_ctas, void* stream);
 
+/* Second order through pose_opt_plus: the backward of epnp_gn_plus_backward_f32 and epnp_gn_plus_camera_backward_f32.
+ * With f = grad_pose_plus . (pose (+) gn_step(pose)) as a function of theta = (x3d, x2d, w2d, delta, cam_mats, lb, ub)
+ * (the pose held constant), and a tangent u of theta [opt, NULL = zero]: t_x3d (B,N,3), t_x2d (B,N,2), t_w2d (B,N,2),
+ * t_delta (B), t_cam (B,3,3), t_lb / t_ub (B,2).  Outputs [opt]:
+ *   h_x3d, h_x2d, h_w2d, h_delta, h_cam, h_lb, h_ub   (H u) with respect to each input, H the Hessian of f in theta
+ *   h_grad (B,D)                                      d pose_opt_plus / d theta . u   (the derivative with respect to
+ *                                                     grad_pose_plus)
+ * The gates are those of the first-order backwards: the clip mask is constant, nothing passes a depth clamped at z_min,
+ * a coordinate clamped at a bound follows that bound, each side of the Huber threshold (huber_eps included) takes its
+ * own branch.  One CTA per object streams the points from global memory, so any N up to
+ * epnp_max_points_split(dof, 0, 0) runs; above it EPNP_ERR_TOO_MANY_POINTS.  No atomics: results are bit-identical
+ * from run to run.  Refusals as epnp_gn_plus_backward_f32, and t_lb / t_ub / h_lb / h_ub without bounds:
+ * EPNP_ERR_BAD_ARG.  B = 0, or no output, writes nothing.                                                         */
+int epnp_gn_plus_hvp_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                         const float* lb, const float* ub, const float* delta, const float* pose,
+                         const float* grad_pose_plus, const float* t_x3d, const float* t_x2d, const float* t_w2d,
+                         const float* t_delta, const float* t_cam, const float* t_lb, const float* t_ub,
+                         float* h_x3d, float* h_x2d, float* h_w2d, float* h_delta, float* h_cam, float* h_lb,
+                         float* h_ub, float* h_grad, int B, int N, int dof, float z_min, float eps, float huber_eps,
+                         void* stream);
+
 /* Epilogue on the AMIS outputs -- the step AFTER the path in every caller of monte_carlo_forward (one pass over the
  * object-major log-weights instead of a dozen torch ops on (M, B) views):
  *   lse (B)        = logsumexp_m logw[b, m]      -- `loss_pred` of MonteCarloPoseLoss.forward
