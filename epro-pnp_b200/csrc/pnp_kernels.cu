@@ -13,6 +13,9 @@
 //   evaluate_backward_kernel         the backward of evaluate_full_kernel's residual / Jacobian / cost (CTA per object, any N).
 //   cost_hvp_point_kernel, cost_hvp_pose_kernel    second order through the cost: Hessian-vector products, point-major
 //                                    (CTA per object) and pose-major (thread per pose), points streamed from global memory.
+//   evaluate_jvp_kernel, evaluate_jvp_cost_kernel   forward mode of evaluate_full_kernel: the Jacobian-vector product of
+//                                    the residual, Jacobian and cost (CTA per pose and object), and of the cost alone at many
+//                                    poses (thread per pose, points staged through shared memory).
 //   cost_pose_backward_kernel, cost_pose_backward_split_kernel    the cost's gradient with respect to stacked poses: thread per
 //                                    pose over the resident points; the split form on cost_split_kernel's clusters.
 //   epnp_init_kernel (pnp_epnp.cuh)  EPnP initialiser with the confidence-quantile point selection, fp64, CTA per object.
@@ -2144,6 +2147,156 @@ __global__ void __launch_bounds__(NT) evaluate_backward_kernel(const EvalBwArgs 
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Forward mode of evaluate_full_kernel's residual, Jacobian and cost at S stacked poses (S, B, D): the Jacobian-vector
+// product with one tangent v (optional parts: x3d, x2d, w2d, delta, every pose, K, lb, ub), the transpose of what
+// evaluate_backward_kernel computes.  Every input is a Dual<1> seeded with its tangent and pushed through
+// point_residual_jac's formulas as residual_jac_vjp writes them, with its gates: no tangent through a depth clamped at
+// z_min, a clamped coordinate takes its bound's tangent (ub when it equals ub, the outer min, else lb), the clip mask is
+// constant, the Huber scale keeps its branches and huber_eps, the Jacobian's rows are differentiated as written, and
+// the rotation is the forward's (ww + xx - yy - zz, ...) of the raw pose components.  A body of its own: the validated
+// backwards' instantiations of residual_jac_vjp stay as they are.
+struct JvpArgs {
+    HvpArgs h;                  // problem, poses (S, B, D) as rows s B + b, the tangent (t_pose (S, B, D)); h.P = S
+    float *dres, *djac, *dcost; // [opt] (S, B, 2N), (S, B, 2N, DOF), (S, B)
+    int clip;
+};
+
+// One (pose, point): the cost with its tangent; r~ and the Jacobian's two rows (u then v) too when RJ.
+template <int DOF, bool RJ>
+__device__ __forceinline__ D1 point_residual_jac_jvp(const D1 (&R)[9], const D1 (&t)[3], const D1 (&K)[9],
+                                                     const D1 (&bnd)[4], const Cam& cam, const D1& delta,
+                                                     float huber_eps, bool clip, const D1 (&pt)[7], D1* r, D1* j) {
+    const D1 &X = pt[0], &Y = pt[1], &Z = pt[2], &u = pt[3], &v = pt[4], &wu = pt[5], &wv = pt[6];
+    const D1 xr = X * R[0] + Y * R[1] + Z * R[2];
+    const D1 yr = X * R[3] + Y * R[4] + Z * R[5];
+    const D1 zr = X * R[6] + Y * R[7] + Z * R[8];
+    const D1 xc = xr + t[0], yc = yr + t[1], zc = zr + t[2];
+    const D1 xh = K[0] * xc + K[1] * yc + K[2] * zc;
+    const D1 yh = K[3] * xc + K[4] * yc + K[5] * zc;
+    const D1 zh = K[6] * xc + K[7] * yc + K[8] * zc;
+    const D1 z = dual_gate(zh, fmaxf(zh.v, cam.z_min), zh.v >= cam.z_min);
+    const D1 iz = dual_recip(z);
+    D1 px = xh * iz, py = yh * iz;
+    if (cam.bounded) {
+        const float cx = fminf(fmaxf(px.v, cam.lbx), cam.ubx), cy = fminf(fmaxf(py.v, cam.lby), cam.uby);
+        if (cx != px.v) px = cx == cam.ubx ? bnd[2] : bnd[0];
+        if (cy != py.v) py = cy == cam.uby ? bnd[3] : bnd[1];
+    }
+    const D1 rx = (px - u) * wu, ry = (py - v) * wv;
+    const D1 s2 = rx * rx + ry * ry;
+    const float s = sqrtf(s2.v), dl = delta.v;
+    const D1 cost = s <= dl ? s2 * 0.5f : delta * dual_sqrt(s2) - delta * delta * 0.5f;
+    if constexpr (RJ) {
+        D1 sc = dual_const<1>(1.0f);
+        if (!(s <= dl && dl >= huber_eps)) {
+            const float sm = fmaxf(s, huber_eps);
+            if (dl / sm < 1.0f) {
+                const D1 sd = (s >= huber_eps && s > 0.f) ? dual_sqrt(s2) : dual_const<1>(sm);
+                sc = dual_sqrt(dual_recip(sd) * delta);
+            }
+        }
+        r[0] = rx * sc; r[1] = ry * sc;
+        if (j) {
+            const bool cz = (z.v == cam.z_min);
+            const bool clip_x = clip && (cz || (cam.bounded && (px.v == cam.lbx || px.v == cam.ubx)));
+            const bool clip_y = clip && (cz || (cam.bounded && (py.v == cam.lby || py.v == cam.uby)));
+            const D1 sx = clip_x ? dual_const<1>(0.f) : sc * wu;
+            const D1 sy = clip_y ? dual_const<1>(0.f) : sc * wv;
+            D1* jx = j; D1* jy = j + DOF;
+            jx[0] = K[0] * iz; jx[1] = K[1] * iz; jx[2] = (K[2] - px) * iz;
+            jy[0] = K[3] * iz; jy[1] = K[4] * iz; jy[2] = (K[5] - py) * iz;
+            if (DOF == 6) {
+                const D1 ax = xr * 2.0f, ay = yr * 2.0f, az = zr * 2.0f;
+                jx[3] = jx[1] * az - jx[2] * ay; jx[4] = jx[2] * ax - jx[0] * az; jx[5] = jx[0] * ay - jx[1] * ax;
+                jy[3] = jy[1] * az - jy[2] * ay; jy[4] = jy[2] * ax - jy[0] * az; jy[5] = jy[0] * ay - jy[1] * ax;
+            } else {
+                jx[3] = jx[0] * zr - jx[2] * xr;
+                jy[3] = jy[0] * zr - jy[2] * xr;
+            }
+#pragma unroll
+            for (int i = 0; i < DOF; ++i) { jx[i] = jx[i] * sx; jy[i] = jy[i] * sy; }
+        }
+    }
+    return cost;
+}
+
+// Point-major: one CTA per (pose, object) row s B + b, as evaluate_full_kernel runs one CTA per object, thread <-> point
+// with the points streamed from global memory (any N).  d cost is one fixed-order block sum.
+template <int DOF>
+__global__ void __launch_bounds__(NT) evaluate_jvp_kernel(const JvpArgs g) {
+    __shared__ float red[2 * NW * 32];
+    constexpr int PD = Dim<DOF>::POSE;
+    const KArgs& a = g.h.k;
+    const size_t row = blockIdx.x;
+    const int obj = (int)(row % a.B), tid = threadIdx.x;
+    Cam cam;
+    D1 K[9], bnd[4], delta, R[9], t[3], p[PD];
+    hvp_object(g.h, obj, cam, K, bnd, delta);
+    hvp_pose<DOF>(g.h, row, R, t, p);
+    const float heps = a.p.huber_eps;
+    float dc = 0.f;
+    for (int n = tid; n < a.N; n += NT) {
+        D1 pt[7], r[2], j[2 * DOF];
+        hvp_point(g.h, (size_t)obj * a.N + n, pt);
+        dc += point_residual_jac_jvp<DOF, true>(R, t, K, bnd, cam, delta, heps, g.clip != 0, pt, r,
+                                                g.djac ? j : nullptr).d[0];
+        const size_t o = row * a.N + n;
+        if (g.dres) { g.dres[2 * o] = r[0].d[0]; g.dres[2 * o + 1] = r[1].d[0]; }
+        if (g.djac) {
+#pragma unroll
+            for (int k = 0; k < 2 * DOF; ++k) g.djac[o * 2 * DOF + k] = j[k].d[0];
+        }
+    }
+    if (g.dcost) {
+        float v[1] = {dc};
+        block_sum<1>(v, red, 0);
+        if (tid == 0) g.dcost[row] = v[0];
+    }
+}
+
+// Pose-major, d cost alone (many poses per object: the Monte-Carlo log-weights): thread <-> pose, grid B x tiles of NT
+// poses, the object's points staged NT at a time (value and tangent) in shared memory and read as broadcasts.  Each
+// pose's sum runs over the points in order.
+constexpr int JVP_POSE_MAJOR_MIN_S = 64;        // below it the pose-major CTAs would be mostly idle
+
+template <int DOF>
+__global__ void __launch_bounds__(NT) evaluate_jvp_cost_kernel(const JvpArgs g, const int tiles) {
+    __shared__ float pts[NT * 14];
+    constexpr int PD = Dim<DOF>::POSE;
+    const KArgs& a = g.h.k;
+    const int obj = blockIdx.x / tiles, s = (blockIdx.x % tiles) * NT + threadIdx.x;
+    const bool ok = s < g.h.P;
+    const size_t row = (size_t)(ok ? s : 0) * a.B + obj;
+    Cam cam;
+    D1 K[9], bnd[4], delta, R[9], t[3], p[PD];
+    hvp_object(g.h, obj, cam, K, bnd, delta);
+    hvp_pose<DOF>(g.h, row, R, t, p);
+    float dc = 0.f;
+    for (int base = 0; base < a.N; base += NT) {
+        const int np = min(NT, a.N - base);
+        __syncthreads();                        // the previous tile is consumed
+        if (threadIdx.x < np) {
+            D1 pt[7];
+            hvp_point(g.h, (size_t)obj * a.N + base + threadIdx.x, pt);
+#pragma unroll
+            for (int c = 0; c < 7; ++c) {
+                pts[threadIdx.x * 14 + 2 * c] = pt[c].v;
+                pts[threadIdx.x * 14 + 2 * c + 1] = pt[c].d[0];
+            }
+        }
+        __syncthreads();
+        if (!ok) continue;
+        for (int i = 0; i < np; ++i) {
+            D1 pt[7];
+#pragma unroll
+            for (int c = 0; c < 7; ++c) pt[c] = d1(pts[i * 14 + 2 * c], pts[i * 14 + 2 * c + 1]);
+            dc += point_residual_jac_jvp<DOF, false>(R, t, K, bnd, cam, delta, 0.f, false, pt, nullptr, nullptr).d[0];
+        }
+    }
+    if (ok) g.dcost[row] = dc;
+}
+
 // AdaptiveHuberPnPCost.set_param: delta = mean(w2d) * sqrt(var_x + var_y) * relative_delta
 __global__ void __launch_bounds__(NT) adaptive_delta_kernel(const float* x2d, const float* w2d, float rel,
                                                           float* delta, int N) {
@@ -3708,6 +3861,37 @@ int epnp_evaluate_backward_f32(const float* x3d, const float* x2d, const float* 
     if (B == 0 || S == 0) return EPNP_OK;
     return by_dof(dof, [&](auto D) {
         return launch_plain(evaluate_backward_kernel<D>, B, NT, 0, SmemAttr::none, (cudaStream_t)stream, g);
+    });
+}
+
+int epnp_evaluate_jvp_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                          const float* lb, const float* ub, const float* delta, const float* poses,
+                          const float* t_x3d, const float* t_x2d, const float* t_w2d, const float* t_delta,
+                          const float* t_pose, const float* t_cam, const float* t_lb, const float* t_ub,
+                          float* d_residual, float* d_jac, float* d_cost, int clip_jac, int S, int B, int N, int dof,
+                          float z_min, float huber_eps, void* stream) {
+    JvpArgs g{};
+    KArgs& a = g.h.k;
+    a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
+    a.poses = poses;
+    epnp_default_params(&a.p, dof);
+    a.p.z_min = z_min; a.p.huber_eps = huber_eps;
+    const int rc = check_common(a);
+    if (rc != EPNP_OK) return rc;
+    if (!poses || S < 0 || (long long)S * B > 2147483647LL || (!d_residual && !d_jac && !d_cost)) return EPNP_ERR_BAD_ARG;
+    if (!lb && (t_lb || t_ub)) return EPNP_ERR_BAD_ARG;
+    if (B == 0 || S == 0) return EPNP_OK;
+    g.h.P = S;
+    g.h.tx3d = t_x3d; g.h.tx2d = t_x2d; g.h.tw2d = t_w2d; g.h.tdelta = t_delta; g.h.tpose = t_pose; g.h.tcam = t_cam;
+    g.h.tlb = t_lb; g.h.tub = t_ub;
+    g.dres = d_residual; g.djac = d_jac; g.dcost = d_cost; g.clip = clip_jac;
+    const bool pose_major = !d_residual && !d_jac && S >= JVP_POSE_MAJOR_MIN_S;
+    const int tiles = (S + NT - 1) / NT;
+    return by_dof(dof, [&](auto D) {
+        if (pose_major)
+            return launch_plain(evaluate_jvp_cost_kernel<D>, B * tiles, NT, 0, SmemAttr::none, (cudaStream_t)stream, g,
+                                tiles);
+        return launch_plain(evaluate_jvp_kernel<D>, S * B, NT, 0, SmemAttr::none, (cudaStream_t)stream, g);
     });
 }
 

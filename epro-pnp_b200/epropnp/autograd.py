@@ -36,6 +36,7 @@ import functools
 import os
 
 import torch
+import torch.autograd.forward_ad as fwAD
 
 from epropnp_b200 import native, ops
 
@@ -130,24 +131,60 @@ class _PosePlus(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x3d, x2d, w2d, delta, cam_mats, lb, ub, pose, params, huber_eps):
-        ints, floats = ops.param_lists(params)
-        prob = ops.problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta)
-        plus = ops.lm_solve(*prob, pose, ints, floats, False, False, True)[3]
-        ctx.save_for_backward(*(t for t in prob if t is not None), pose)
-        ctx.bounded = prob[4] is not None
-        ctx.consts = (ints[0], floats[0], floats[6], float(huber_eps))              # dof, z_min, eps, huber_eps
-        return plus.to(x3d.dtype)
+        plus = _PosePlus._plus(x3d, x2d, w2d, delta, cam_mats, lb, ub, pose, params)
+        _PosePlus._setup(ctx, (x3d, x2d, w2d, delta, cam_mats, lb, ub, pose, params, huber_eps))
+        return plus
 
     @staticmethod
-    def backward(ctx, grad_plus):
+    def _plus(x3d, x2d, w2d, delta, cam_mats, lb, ub, pose, params):
+        ints, floats = ops.param_lists(params)
+        prob = ops.problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta)
+        return ops.lm_solve(*prob, pose, ints, floats, False, False, True)[3].to(x3d.dtype)
+
+    @staticmethod
+    def _setup(ctx, inputs):
+        x3d, x2d, w2d, delta, cam_mats, lb, ub, pose, params, huber_eps = inputs
+        ints, floats = ops.param_lists(params)
+        prob = ops.problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta)
+        ctx.save_for_backward(*(t for t in prob if t is not None), pose)
+        if fwAD._current_level >= 0:                                                 # only a forward pass reads it
+            ctx.save_for_forward(*(t for t in prob if t is not None), pose)
+        ctx.bounded = prob[4] is not None
+        ctx.consts = (ints[0], floats[0], floats[6], float(huber_eps))              # dof, z_min, eps, huber_eps
+
+    @staticmethod
+    def _saved(ctx):
         saved = list(ctx.saved_tensors)
         pose = saved.pop()
         x3d, x2d, w2d, cam_mats = saved[:4]
         lb, ub = (saved[4], saved[5]) if ctx.bounded else (None, None)
-        prob = (x3d, x2d, w2d, cam_mats, lb, ub, saved[-1])
+        return (x3d, x2d, w2d, cam_mats, lb, ub, saved[-1]), pose
+
+    @staticmethod
+    def backward(ctx, grad_plus):
+        prob, pose = _PosePlus._saved(ctx)
         n = ctx.needs_input_grad
         g = ops.gn_plus_grads(prob, pose, grad_plus, *ctx.consts, (n[0], n[1], n[2], n[4], n[5], n[6], n[3]))
         return g[0], g[1], g[2], g[6], g[3], g[4], g[5], None, None, None
+
+    @staticmethod
+    def jvp(ctx, t_x3d, t_x2d, t_w2d, t_delta, t_cam, t_lb, t_ub, *_):
+        """d pose_opt_plus . u, the pose held constant (ops.gn_plus_jvp); a Python-float delta or bound has none."""
+        prob, pose = _PosePlus._saved(ctx)
+        t = ops.gn_plus_jvp(prob, pose, (t_x3d, t_x2d, t_w2d, t_cam, t_lb, t_ub, t_delta), *ctx.consts)
+        return None if t is None else t.to(prob[0].dtype)
+
+
+class _PosePlusFunc(_PosePlus):
+    """_PosePlus in setup_context style, which torch.func's transforms (jvp, linearize, grad) require."""
+
+    @staticmethod
+    def forward(x3d, x2d, w2d, delta, cam_mats, lb, ub, pose, params, huber_eps):
+        return _PosePlus._plus(x3d, x2d, w2d, delta, cam_mats, lb, ub, pose, params)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        _PosePlus._setup(ctx, inputs)
 
 
 def native_gn_step_enabled():
@@ -167,8 +204,9 @@ def pose_plus_autograd(solver, x3d, x2d, w2d, pose, camera, cost_fun):
         plus = ops.lm_solve(*_problem_args(x3d, x2d, w2d, camera, cost_fun), pose.detach(), *params, False, False,
                             True)[3]
         return plus.to(x3d.dtype)
-    return _PosePlus.apply(x3d, x2d, w2d, delta if torch.is_tensor(delta) else float(delta), camera.cam_mats,
-                           camera.lb, camera.ub, pose.detach(), params, float(getattr(cost_fun, "eps", 1e-10)))
+    fn = _PosePlusFunc if torch._C._are_functorch_transforms_active() else _PosePlus
+    return fn.apply(x3d, x2d, w2d, delta if torch.is_tensor(delta) else float(delta), camera.cam_mats,
+                    camera.lb, camera.ub, pose.detach(), params, float(getattr(cost_fun, "eps", 1e-10)))
 
 
 def gn_step_autograd(solver, x3d, x2d, w2d, pose, camera, cost_fun):

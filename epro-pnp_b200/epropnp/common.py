@@ -39,12 +39,14 @@ def _pose_rot(pose):
 
 
 def _needs_grad(*tensors):
-    return torch.is_grad_enabled() and any(torch.is_tensor(t) and t.requires_grad for t in tensors)
+    """A tensor needs a derivative: reverse mode, a forward-mode tangent or a torch.func transform (ops.needs_derivative,
+    the layer's one routing predicate)."""
+    return ops.needs_derivative(*tensors)
 
 
-def _camera_requires_grad(camera):
-    """cam_mats or a tensor bound of `camera` requires grad."""
-    return any(torch.is_tensor(t) and t.requires_grad for t in (camera.cam_mats, camera.lb, camera.ub))
+def _camera_needs_grad(camera):
+    """cam_mats or a tensor bound of `camera` needs a derivative."""
+    return ops.needs_derivative(camera.cam_mats, camera.lb, camera.ub)
 
 
 def _store(out, value):
@@ -78,7 +80,7 @@ def evaluate_pnp(x3d, x2d, w2d, pose, camera, cost_fun,
                                                     want_c)
             return ((_store(out_residual, residual) if want_r else None), (_store(out_cost, cost) if want_c else None),
                     (_store(out_jacobian, jac) if want_j else None))
-        if want_j or want_r or ((pose.requires_grad or camera_grad) and not native_grad):
+        if want_j or want_r or ((_needs_grad(pose) or camera_grad) and not native_grad):
             # the same outputs, or gradients w.r.t. the pose or the camera, of CPU / float64 tensors: the torch
             # composite of the same two methods the reference calls
             x2d_proj, jac_cam = camera.project(x3d, pose, out_jac=(out_jacobian is not False), clip_jac=clip_jac)

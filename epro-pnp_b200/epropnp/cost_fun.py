@@ -100,7 +100,7 @@ class AdaptiveHuberPnPCost(HuberPnPCost):
         self.relative_delta = relative_delta
 
     def set_param(self, x2d, w2d):
-        needs_graph = torch.is_grad_enabled() and (x2d.requires_grad or w2d.requires_grad)
+        needs_graph = ops.needs_derivative(x2d, w2d)
         if x2d.is_cuda and x2d.dim() == 3 and not needs_graph:
             self.delta = ops.adaptive_delta(x2d, w2d, float(self.relative_delta)).to(x2d.dtype)   # one native kernel
             return

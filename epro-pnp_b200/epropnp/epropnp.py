@@ -26,7 +26,7 @@ from abc import ABCMeta, abstractmethod
 import torch
 
 from .builder import PNP, build_pnp
-from .common import _camera_requires_grad, evaluate_pnp, philox_seed, pnp_normalize, pnp_denormalize
+from .common import _needs_grad, evaluate_pnp, philox_seed, pnp_normalize, pnp_denormalize
 from .distributions import AngularCentralGaussian, MultivariateStudentT, VonMisesUniformMix
 
 # The steps of the AMIS loop the reference exposes as methods of the layer (epropnp.py:65-82).  Here the loop runs inside
@@ -140,10 +140,7 @@ class EProPnPBase(torch.nn.Module, metaclass=ABCMeta):
         if kwargs:
             raise TypeError(f"unexpected arguments {sorted(kwargs)}")
         delta = cost_fun.delta
-        differentiable = torch.is_grad_enabled() and (any(t.requires_grad for t in (x3d, x2d, w2d)) or
-                                                      (torch.is_tensor(delta) and delta.requires_grad) or
-                                                      (pose_init is not None and pose_init.requires_grad) or
-                                                      _camera_requires_grad(camera))
+        differentiable = _needs_grad(x3d, x2d, w2d, delta, pose_init, camera.cam_mats, camera.lb, camera.ub)
         if self.normalize:
             transform, x3d, pose_init = pnp_normalize(x3d, pose_init, detach_transformation=True)
         assert x3d.dim() == x2d.dim() == w2d.dim() == 3

@@ -18,7 +18,7 @@ import torch.nn.functional as F
 from epropnp_b200 import ops
 from .autograd import _problem_args
 from .builder import PNP, build_pnp
-from .common import _camera_requires_grad, evaluate_pnp, philox_seed, pnp_normalize, pnp_denormalize
+from .common import _needs_grad, evaluate_pnp, philox_seed, pnp_normalize, pnp_denormalize
 
 
 def solve_wrapper(b, A):
@@ -75,9 +75,8 @@ class LMSolver(nn.Module):
         if normalize:
             transform, x3d, pose_init = pnp_normalize(x3d, pose_init, detach_transformation=True)
         delta = getattr(cost_fun, "delta", None)
-        differentiable = with_pose_opt_plus and torch.is_grad_enabled() and (
-            any(t.requires_grad for t in (x3d, x2d, w2d)) or (torch.is_tensor(delta) and delta.requires_grad) or
-            _camera_requires_grad(camera))
+        differentiable = with_pose_opt_plus and _needs_grad(x3d, x2d, w2d, delta, camera.cam_mats, camera.lb,
+                                                            camera.ub)
         pose_opt, pose_cov, cost, pose_opt_plus = self._solve_impl(
             x3d, x2d, w2d, camera, cost_fun, pose_init=pose_init,
             with_pose_opt_plus=with_pose_opt_plus and not differentiable, **kwargs)

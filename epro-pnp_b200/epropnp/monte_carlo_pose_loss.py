@@ -45,7 +45,7 @@ def mc_logsumexp(pose_sample_logweights):
 def mc_sample_weights(pose_sample_logweights):
     """softmax over the samples, returned as an (mc_samples, num_obj) view like the log-weights themselves."""
     if pose_sample_logweights.dim() == 2 and _use_native(pose_sample_logweights) \
-            and not pose_sample_logweights.requires_grad:
+            and not (pose_sample_logweights.requires_grad or ops.forward_tangent(pose_sample_logweights)):
         w = ops.mc_epilogue(_object_major(pose_sample_logweights), None, None, None, False, False, True, False)[2]
         return w.to(pose_sample_logweights.dtype).transpose(0, 1)
     return pose_sample_logweights.softmax(dim=0)

@@ -570,6 +570,48 @@ def cost_camera_backward(prob: Problem, dof, z_min, poses_a, grad_a, poses_b=Non
     return gcam, glb, gub
 
 
+JVP_TANGENTS = ("x3d", "x2d", "w2d", "delta", "pose", "cam", "lb", "ub")
+JVP_OUTPUTS = ("residual", "jac", "cost")
+
+
+def evaluate_jvp(prob: Problem, poses, dof, z_min, huber_eps, clip_jac, tangents, want):
+    """Forward mode of evaluate_full at stacked poses (S, B, D) (epnp_evaluate_jvp_f32).  `tangents`: the parts of v by
+    name (JVP_TANGENTS; missing or None: zero), shaped (B, N, 3), (B, N, 2), (B, N, 2), (B), (S, B, D), (B, 3, 3),
+    (B, 2), (B, 2).  `want`: three flags in JVP_OUTPUTS order.  Returns the tangents of the residual (S, B, 2N), the
+    Jacobian (S, B, 2N, dof) and the cost (S, B); None where `want` is False."""
+    D = 7 if dof == 6 else 4
+    S, B, N = poses.shape[0], prob.B, prob.N
+    _check_pose(poses, (S, B), D, "poses")
+    if len(want) != len(JVP_OUTPUTS):
+        raise ValueError(f"want: {len(JVP_OUTPUTS)} flags ({', '.join(JVP_OUTPUTS)})")
+    if not any(want):
+        raise ValueError("want: ask for at least one output")
+    unknown = set(tangents) - set(JVP_TANGENTS)
+    if unknown:
+        raise ValueError(f"unknown tangents {sorted(unknown)}; expected some of {JVP_TANGENTS}")
+    shapes = dict(x3d=(B, N, 3), x2d=(B, N, 2), w2d=(B, N, 2), delta=(B,), pose=(S, B, D), cam=(B, 3, 3), lb=(B, 2),
+                  ub=(B, 2))
+    if prob.lb is None and any(tangents.get(k) is not None for k in ("lb", "ub")):
+        raise ValueError("a bound's tangent needs the problem's bounds")
+    tan = []
+    for k in JVP_TANGENTS:
+        t = tangents.get(k)
+        if t is not None:
+            if tuple(t.shape) != shapes[k]:
+                raise ValueError(f"tangent {k} must be {shapes[k]}; got {tuple(t.shape)}")
+            t = _f32c(t)
+        tan.append(t)
+    poses = _f32c(poses)
+    new = (lambda *s: torch.zeros(s, dtype=torch.float32, device=prob.device)) if S == 0 else prob.empty
+    out = [new(*s) if w else None for w, s in zip(want, ((S, B, 2 * N), (S, B, 2 * N, dof), (S, B)))]
+    with torch.cuda.device(prob.device):
+        check(lib().epnp_evaluate_jvp_f32(*prob.common_ptrs(), ptr(poses), *(ptr(t) for t in tan),
+                                          *(ptr(o) for o in out), int(clip_jac), S, B, N, int(dof),
+                                          ctypes.c_float(z_min), ctypes.c_float(huber_eps),
+                                          stream_ptr(prob.device)), "epnp_evaluate_jvp_f32")
+    return tuple(out)
+
+
 HVP_TANGENTS = ("x3d", "x2d", "w2d", "delta", "pose", "cam", "lb", "ub")
 HVP_OUTPUTS = ("x3d", "x2d", "w2d", "delta", "pose", "grad", "cam", "lb", "ub")
 
@@ -855,4 +897,4 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
 
 __all__ = ["Problem", "adaptive_delta", "cost_backward", "cost_camera_backward", "gn_plus_camera_backward",
            "evaluate_cost", "evaluate_cost_split", "evaluate_full", "evaluate_backward", "lm_solve",
-           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "solve_host", "solve_split_host", "solve_workspace_bytes", "rslm_spec", "epnp_spec", "initial_pose", "rslm", "rslm_split", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "cost_hvp", "gn_plus_hvp", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]
+           "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "solve_host", "solve_split_host", "solve_workspace_bytes", "rslm_spec", "epnp_spec", "initial_pose", "rslm", "rslm_split", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "evaluate_jvp", "cost_hvp", "gn_plus_hvp", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

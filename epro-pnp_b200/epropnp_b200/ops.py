@@ -18,13 +18,22 @@ Hessian-vector product cost_hvp), on the pose_opt_plus backwards (gn_plus_backwa
 Hessian-vector product gn_plus_hvp) and on mc_lse_backward.  cost_hvp and gn_plus_hvp have none, so a third derivative
 raises.  evaluate_full's residual / Jacobian are first-order only: a second backward through evaluate_backward raises.
 
+Forward mode (torch.autograd.forward_ad, torch.func.jvp and linearize) runs eagerly through the jvp formulas of the eager Functions of
+evaluate_cost, evaluate_full (the kernel evaluate_jvp), lm_amis_fused (logw and cost_init), lm_solve (pose_opt_plus,
+through gn_plus_hvp) and mc_epilogue (lse); each is the transpose of the reverse-mode formula beside it, with its detach
+rules.  needs_derivative is the one predicate every routing point of the layer uses.  Under torch.func.jvp / linearize
+the formulas run as autograd.Functions and their kernel calls go through the dispatcher (which unwraps functorch's
+tensors).  Under torch.compile / torch.export a forward tangent raises; vmap-based transforms, forward over reverse (the
+backward and Hessian operators) and reverse through evaluate_jvp are not supported.
+
 The module's names (adaptive_delta, ..., mc_lse_backward) are the entry points the layer calls (_entry): the operator
 while anything traces, its implementation directly in eager code.  The operators themselves are FORWARD / BACKWARD /
-SECOND_ORDER and torch.ops.epropnp.*; each entry point's `.op` is its operator.
+SECOND_ORDER / FORWARD_MODE and torch.ops.epropnp.*; each entry point's `.op` is its operator.
 """
 from typing import List, Optional
 
 import torch
+import torch.autograd.forward_ad as _fwAD
 from torch import Tensor
 
 from . import capi, native
@@ -455,6 +464,27 @@ def _(x3d, x2d, w2d, cam_mats, lb, ub, delta, pose, grad_pose_plus, t_x3d, t_x2d
                                    (B, _pose_dim(dof))))
 
 
+@_op("evaluate_jvp")
+def evaluate_jvp(x3d: Tensor, x2d: Tensor, w2d: Tensor, cam_mats: Tensor, lb: Optional[Tensor], ub: Optional[Tensor],
+                 delta: Tensor, poses: Tensor, t_x3d: Optional[Tensor], t_x2d: Optional[Tensor],
+                 t_w2d: Optional[Tensor], t_delta: Optional[Tensor], t_pose: Optional[Tensor], t_cam: Optional[Tensor],
+                 t_lb: Optional[Tensor], t_ub: Optional[Tensor], dof: int, z_min: float, huber_eps: float,
+                 clip_jac: bool, want: List[bool]) -> tuple[Tensor, Tensor, Tensor]:
+    """native.evaluate_jvp: poses (S, B, D) and the tangent's parts (None: zero) -> the tangents of the residual
+    (S, B, 2N), the Jacobian (S, B, 2N, dof) and the cost (S, B)."""
+    prob = _problem(x3d, x2d, w2d, cam_mats, lb, ub, delta)
+    tangents = dict(zip(native.JVP_TANGENTS, (t_x3d, t_x2d, t_w2d, t_delta, t_pose, t_cam, t_lb, t_ub)))
+    out = native.evaluate_jvp(prob, poses, dof, z_min, huber_eps, clip_jac, tangents, tuple(want))
+    return tuple(_or_empty(t, x3d) for t in out)
+
+
+@evaluate_jvp.register_fake
+def _(x3d, x2d, w2d, cam_mats, lb, ub, delta, poses, t_x3d, t_x2d, t_w2d, t_delta, t_pose, t_cam, t_lb, t_ub, dof,
+      z_min, huber_eps, clip_jac, want):
+    S, B, N = poses.shape[0], x3d.shape[0], x3d.shape[1]
+    return _grad_fakes(x3d, want, ((S, B, 2 * N), (S, B, 2 * N, dof), (S, B)))
+
+
 @_op("mc_lse_backward")
 def mc_lse_backward(logw_bm: Tensor, lse: Tensor, grad_lse: Tensor) -> Tensor:
     """grad_logw (B, M) = grad_lse[b] * exp(logw[b, m] - lse[b]) (native.mc_lse_backward)."""
@@ -478,20 +508,43 @@ def _sum_to(like, g):
 
 
 _EAGER = {}
+_EAGER_FUNC = {}
 
 
-def _register_autograd(op, backward, setup_context):
-    """op.register_autograd, and the same two functions as an autograd.Function that runs the implementation directly:
-    the eager driver of the formula (see _entry)."""
+def _register_autograd(op, backward, setup_context, jvp=None):
+    """op.register_autograd, and the same functions as autograd.Functions that run the implementation directly: the
+    eager drivers of the formula (see _entry).  `jvp(ctx, inputs, output, tangents)` [opt]: the forward-mode formula,
+    the tangents of the outputs (None: none) from those of the inputs; it runs eagerly only (the operator's
+    register_autograd has no forward rule).  Two classes: one with forward(ctx, ...) for reverse mode and
+    torch.autograd.forward_ad, and, for torch.func's transforms, one in setup_context style (which torch.func requires,
+    but whose apply binds the arguments through inspect.signature on every call: host time the training step does not
+    need to pay)."""
     op.register_autograd(backward, setup_context=setup_context)
     impl = _IMPLS[op]
 
+    def setup(ctx, inputs, output):
+        setup_context(ctx, inputs, output)
+        if jvp is not None and _fwAD._current_level >= 0:         # a forward-AD level (torch.func.jvp opens one too)
+            ctx.fw_consts = tuple(None if torch.is_tensor(a) else a for a in inputs)
+            ctx.fw_tensor = tuple(torch.is_tensor(a) for a in inputs)
+            ctx.save_for_forward(*(a for a in inputs if torch.is_tensor(a)), *output)
+
     def forward(ctx, *args):
         out = impl(*args)
-        setup_context(ctx, args, out)
+        setup(ctx, args, out)
         return out
-    _EAGER[op] = type(f"epropnp_{op._name.split('::')[-1]}", (torch.autograd.Function,),
-                      dict(forward=staticmethod(forward), backward=staticmethod(backward)))
+
+    name = f"epropnp_{op._name.split('::')[-1]}"
+    body = dict(backward=staticmethod(backward))
+    if jvp is not None:
+        def fw(ctx, *tangents):
+            saved = iter(ctx.saved_tensors)
+            inputs = tuple(next(saved) if t else c for t, c in zip(ctx.fw_tensor, ctx.fw_consts))
+            return jvp(ctx, inputs, tuple(saved), tangents)
+        body["jvp"] = staticmethod(fw)
+    _EAGER[op] = type(name, (torch.autograd.Function,), dict(body, forward=staticmethod(forward)))
+    _EAGER_FUNC[op] = type(name, (torch.autograd.Function,),
+                           dict(body, forward=staticmethod(impl), setup_context=staticmethod(setup)))
 
 
 def _save_problem(ctx, inputs, extra=()):
@@ -565,7 +618,49 @@ def _evaluate_cost_backward(ctx, g_cost):
     return grads + (gpose, None, None)
 
 
-_register_autograd(evaluate_cost, _evaluate_cost_backward, _evaluate_cost_setup)
+# ------------------------------------------------------------------------------------------------ forward-mode formulas
+def _expand_to(t, shape):
+    """The reverse of _sum_to: a tangent of a broadcast input (a scalar delta, a (3, 3) camera, a (2,) bound, a
+    (B, N, 1) weight) expanded to the native shape (None stays None)."""
+    if t is None:
+        return None
+    if t.numel() == 1:
+        return t.reshape(()).expand(shape)
+    return t.reshape(shape) if t.numel() == _numel(shape) else t.expand(shape)
+
+
+def _numel(shape):
+    n = 1
+    for s in shape:
+        n *= s
+    return n
+
+
+def _problem_tangents(prob, tangents):
+    """The tangents of the seven problem inputs (argument order) by native.JVP_TANGENTS name, in the native shapes: none
+    for a bound without the other one (it does not clamp)."""
+    x3d = prob[0]
+    B, N = x3d.shape[0], x3d.shape[1]
+    bounded = _bounded(prob[4], prob[5])
+    t_x3d, t_x2d, t_w2d, t_cam, t_lb, t_ub, t_delta = tangents[:7]
+    return dict(x3d=_expand_to(t_x3d, (B, N, 3)), x2d=_expand_to(t_x2d, (B, N, 2)), w2d=_expand_to(t_w2d, (B, N, 2)),
+                delta=_expand_to(t_delta, (B,)), cam=_expand_to(t_cam, (B, 3, 3)),
+                lb=_expand_to(t_lb, (B, 2)) if bounded else None, ub=_expand_to(t_ub, (B, 2)) if bounded else None)
+
+
+def cost_jvp(prob, poses, t_prob, t_pose, dof, z_min):
+    """d cost(poses) . v (S, B) at poses (S, B, D): v = the problem tangents (a dict, _problem_tangents) and t_pose
+    (S, B, D) or None."""
+    t = dict(t_prob, pose=t_pose)
+    return evaluate_jvp(*prob, poses, *(t.get(k) for k in native.JVP_TANGENTS), dof, z_min, 1e-10, False,
+                        [False, False, True])[2]
+
+
+def _evaluate_cost_jvp(ctx, inputs, output, tangents):
+    return cost_jvp(inputs[:7], inputs[7], _problem_tangents(inputs[:7], tangents), tangents[7], ctx.dof, ctx.z_min)
+
+
+_register_autograd(evaluate_cost, _evaluate_cost_backward, _evaluate_cost_setup, _evaluate_cost_jvp)
 
 
 def _evaluate_full_setup(ctx, inputs, output):
@@ -593,7 +688,16 @@ def _evaluate_full_backward(ctx, g_res, g_cost, g_jac):
     return out + (gpose,) + (None,) * 7
 
 
-_register_autograd(evaluate_full, _evaluate_full_backward, _evaluate_full_setup)
+def _evaluate_full_jvp(ctx, inputs, output, tangents):
+    dof, z_min, huber_eps, clip_jac = ctx.consts
+    want = list(inputs[12:15])                                                   # (r, j, c)
+    t = dict(_problem_tangents(inputs[:7], tangents), pose=tangents[7])
+    d_r, d_j, d_c = evaluate_jvp(*inputs[:8], *(t.get(k) for k in native.JVP_TANGENTS), dof, z_min, huber_eps,
+                                 clip_jac, want)
+    return d_r if want[0] else None, d_c if want[2] else None, d_j if want[1] else None
+
+
+_register_autograd(evaluate_full, _evaluate_full_backward, _evaluate_full_setup, _evaluate_full_jvp)
 
 
 def _fused_setup(ctx, inputs, output):
@@ -627,7 +731,27 @@ def _fused_backward(ctx, g_pose, g_cost, g_plus, g_cost_init, g_samples, g_logw)
     return grads + (None, gpose) + (None,) * 10
 
 
-_register_autograd(lm_amis_fused, _fused_backward, _fused_setup)
+def _fused_jvp(ctx, inputs, output, tangents):
+    """logw = -cost(samples) - log q: -d cost(samples) . v with the samples constant; cost_init (at cost_init_pose):
+    d cost(cost_init_pose) . (v, its tangent), in the same launch.  pose_opt, cost, pose_opt_plus and the samples carry
+    none, as in reverse mode."""
+    prob, samples = inputs[:7], output[4]
+    B = samples.shape[0]
+    poses = samples.transpose(0, 1)                                              # (M, B, D)
+    t_pose = None
+    if ctx.has_ci:
+        poses = torch.cat((inputs[8].to(poses.dtype).reshape(1, B, -1), poses))
+        tci = tangents[8]
+        t_pose = torch.zeros(poses.shape, dtype=torch.float32, device=poses.device)
+        if tci is not None:
+            t_pose[0] = tci.reshape(B, -1)
+    dc = cost_jvp(prob, poses.contiguous(), _problem_tangents(prob, tangents), t_pose, ctx.dof, ctx.z_min)
+    t_ci = dc[0].clone() if ctx.has_ci else None
+    t_logw = -dc[1 if ctx.has_ci else 0:].transpose(0, 1).contiguous()         # the layout of logw (B, M)
+    return None, None, None, t_ci, None, t_logw
+
+
+_register_autograd(lm_amis_fused, _fused_backward, _fused_setup, _fused_jvp)
 
 
 def gn_plus_grads(prob, pose, grad_plus, dof, z_min, eps, huber_eps, needs):
@@ -650,6 +774,18 @@ def gn_plus_grads(prob, pose, grad_plus, dof, z_min, eps, huber_eps, needs):
     return _problem_grads(prob, corr, cam)
 
 
+def gn_plus_jvp(prob, pose, tangents, dof, z_min, eps, huber_eps):
+    """d pose_opt_plus . u (B, D) of pose_opt_plus = pose (+) gn_step(pose), the pose held constant: gn_plus_hvp's grad
+    output with no problem output wanted.  `tangents`: those of the seven problem inputs in argument order."""
+    t = _problem_tangents(prob, tangents)
+    if all(v is None for v in t.values()):
+        return None
+    pose = pose.detach()
+    zero = torch.zeros(pose.shape, dtype=torch.float32, device=pose.device)
+    return gn_plus_hvp(*prob, pose, zero, *(t[k] for k in native.GN_HVP_TANGENTS), dof, z_min, eps, huber_eps,
+                       [False] * 7 + [True])[7]
+
+
 def _lm_solve_setup(ctx, inputs, output):
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[:3])
@@ -665,7 +801,13 @@ def _lm_solve_backward(ctx, g_opt, g_cov, g_cost, g_plus):
     return gn_plus_grads(prob, pose, g_plus, *ctx.consts, ctx.needs_input_grad[:7]) + (None,) * 6
 
 
-_register_autograd(lm_solve, _lm_solve_backward, _lm_solve_setup)
+def _lm_solve_jvp(ctx, inputs, output, tangents):
+    if not inputs[12]:                                                           # want_plus
+        return None, None, None, None
+    return None, None, None, gn_plus_jvp(inputs[:7], inputs[7], tangents[:7], *ctx.consts)
+
+
+_register_autograd(lm_solve, _lm_solve_backward, _lm_solve_setup, _lm_solve_jvp)
 
 
 def _mc_epilogue_setup(ctx, inputs, output):
@@ -681,7 +823,21 @@ def _mc_epilogue_backward(ctx, g_lse, g_loss, g_weights, g_score):
     return (g,) + (None,) * 7
 
 
-_register_autograd(mc_epilogue, _mc_epilogue_backward, _mc_epilogue_setup)
+def _mc_epilogue_jvp(ctx, inputs, output, tangents):
+    """lse: sum_m softmax(logw)_m t_logw_m (torch on (B, M)).  The loss and the weights are non-differentiable outputs
+    in reverse mode; with a tangent they raise rather than come back with none (the layer asks for them only without
+    one: mc_sample_weights takes torch's softmax then).  The score carries none (its inputs are detached)."""
+    if inputs[5] or inputs[6]:
+        raise RuntimeError("epropnp::mc_epilogue: the loss and the sample weights have no forward-mode formula; take "
+                           "them from logw with torch ops (logsumexp, softmax) under forward AD")
+    t = tangents[0]
+    if t is None or not inputs[4]:
+        return None, None, None, None
+    w = torch.exp(inputs[0].to(torch.float32) - output[0].unsqueeze(1))
+    return (w * t.to(torch.float32)).sum(1), None, None, None
+
+
+_register_autograd(mc_epilogue, _mc_epilogue_backward, _mc_epilogue_setup, _mc_epilogue_jvp)
 
 
 # ---------------------------------------------------------------------------------------------- second-order formulas
@@ -792,6 +948,37 @@ FORWARD = (adaptive_delta, evaluate_cost, evaluate_full, lm_solve, lm_amis_fused
 BACKWARD = (cost_backward, cost_pose_backward, cost_camera_backward, gn_plus_backward, gn_plus_camera_backward,
             evaluate_backward, mc_lse_backward)
 SECOND_ORDER = (cost_hvp, gn_plus_hvp)
+FORWARD_MODE = (evaluate_jvp,)
+# operators whose outputs the layer never differentiates (the solver's start): under forward AD their inputs' tangents
+# are dropped, as reverse mode's no_grad drops the graph
+_NO_DERIVATIVE = (rslm_draw, rslm, epnp_init)
+
+
+@torch.compiler.disable
+def _eager_call(fn, *args):
+    """fn(*args) with torch.compile's frame evaluation off: when a compiled region falls back to running an entry point
+    eagerly (its refusal of a forward tangent), the ctypes calls below must not be traced frame by frame."""
+    return fn(*args)
+
+
+def forward_tangent(*args):
+    """An argument carries a forward-mode tangent (torch.autograd.forward_ad, torch.func.jvp) or is wrapped by a
+    torch.func transform.  One module-attribute read when neither is active."""
+    if _fwAD._current_level < 0 and not torch._C._are_functorch_transforms_active():
+        return False
+    for a in args:
+        if torch.is_tensor(a) and (torch._C._functorch.is_functorch_wrapped_tensor(a)
+                                   or (_fwAD._current_level >= 0 and _fwAD.unpack_dual(a).tangent is not None)):
+            return True
+    return False
+
+
+def needs_derivative(*args):
+    """The layer's one routing predicate: an argument needs the differentiable path -- reverse mode (grad enabled and
+    requires_grad), a forward-mode tangent or a torch.func transform (forward_tangent).  Non-tensors are ignored."""
+    if torch.is_grad_enabled() and any(torch.is_tensor(a) and a.requires_grad for a in args):
+        return True
+    return forward_tangent(*args)
 
 
 def _entry(op):
@@ -800,13 +987,57 @@ def _entry(op):
     gradient, under the operator's own autograd formula (_register_autograd); an operator without a formula is called
     as such, so that differentiating through it raises.  The direct call skips the dispatcher and custom_op's argument
     handling, whose eager host time per call is several small kernel launches' worth."""
-    impl, eager = _IMPLS[op], _EAGER.get(op)
+    impl, eager, eager_func = _IMPLS[op], _EAGER.get(op), _EAGER_FUNC.get(op)
+    name = op._name
+
+    def dual_tangent(args):
+        return _fwAD._current_level >= 0 and any(torch.is_tensor(a) and _fwAD.unpack_dual(a).tangent is not None
+                                                 for a in args)
+
+    def under_functorch(args):
+        # torch.func.jvp / linearize: the tensors are functorch wrappers.  A call with a tangent at this level runs its
+        # formula as an autograd.Function (functorch unwraps the forward's arguments); a call without one -- a formula's
+        # own kernel call on the primals and tangents -- goes through the dispatcher, which unwraps its arguments before
+        # the implementation.  So ctypes never sees a wrapper.
+        if not dual_tangent(args):
+            return op(*args)
+        if eager is not None and "jvp" in vars(eager):
+            return eager_func.apply(*args)
+        if op in _NO_DERIVATIVE:
+            return op(*(a.detach() if torch.is_tensor(a) else a for a in args))
+        raise RuntimeError(f"{name} has no forward-mode formula: a tangent cannot pass through it (forward over "
+                           "reverse is not supported)")
 
     def entry(*args):
-        if torch.compiler.is_compiling() or torch._C._len_torch_dispatch_stack():
+        if torch.compiler.is_compiling():
+            # the traced operator has no forward rule and would drop a tangent; the module attribute is traceable
+            if _fwAD._current_level >= 0:
+                raise RuntimeError(f"{name}: forward-mode tangents are not supported under torch.compile / "
+                                   "torch.export; compute the JVP eagerly")
+            return op(*args)
+        if torch._C._len_torch_dispatch_stack():
+            if forward_tangent(*args):
+                # torch.func.linearize traces a forward-AD pass under make_fx's dispatch mode: the formulas run, and
+                # their kernel calls are traced as operators
+                if torch._C._are_functorch_transforms_active():
+                    return under_functorch(args)
+                if eager is not None and "jvp" in vars(eager):
+                    return eager.apply(*args)
+                raise RuntimeError(f"{name} has no forward-mode formula: a tangent cannot pass through it")
             return op(*args)
         if torch.is_grad_enabled() and any(torch.is_tensor(a) and a.requires_grad for a in args):
-            return op(*args) if eager is None else eager.apply(*args)
+            if eager is None:
+                return op(*args)
+            return (eager_func if torch._C._are_functorch_transforms_active() else eager).apply(*args)
+        if forward_tangent(*args):
+            if torch._C._are_functorch_transforms_active():
+                return under_functorch(args)
+            if eager is not None and "jvp" in vars(eager):
+                return _eager_call(eager.apply, *args)
+            if op in _NO_DERIVATIVE:
+                return _eager_call(impl, *(a.detach() if torch.is_tensor(a) else a for a in args))
+            raise RuntimeError(f"{name} has no forward-mode formula: a tangent cannot pass through it (forward over "
+                               "reverse is not supported)")
         return impl(*args)
     entry.op = op
     return entry
@@ -818,3 +1049,4 @@ def _entry(op):
 (cost_backward, cost_pose_backward, cost_camera_backward, gn_plus_backward, gn_plus_camera_backward, evaluate_backward,
  mc_lse_backward) = (_entry(op) for op in BACKWARD)
 cost_hvp, gn_plus_hvp = (_entry(op) for op in SECOND_ORDER)
+evaluate_jvp = _entry(evaluate_jvp)

@@ -133,6 +133,23 @@ int epnp_evaluate_backward_f32(const float* x3d, const float* x2d, const float* 
                                float* grad_cam, float* grad_lb, float* grad_ub, int clip_jac, int S, int B, int N,
                                int dof, float z_min, float huber_eps, void* stream);
 
+/* Forward mode of epnp_evaluate_f32's outputs at S stacked poses (S, B, D): the Jacobian-vector product with one
+ * tangent, the transpose of epnp_evaluate_backward_f32 (<g, J v> = <J^T g, v>) with its gates.  Tangent [opt, NULL =
+ * zero]: t_x3d (B,N,3), t_x2d / t_w2d (B,N,2), t_delta (B), t_pose (S,B,D) (raw components, through the forward's
+ * rotation), t_cam (B,3,3), t_lb / t_ub (B,2).  Outputs, each optional but at least one:
+ *   d_residual (S, B, 2N), d_jac (S, B, 2N, dof), d_cost (S, B)
+ * Two launches: point-major (one CTA per pose and object, the points streamed from global memory: any N; d_cost one
+ * fixed-order block sum) and, for d_cost alone at S >= 64 poses, pose-major (thread per pose, the points staged through
+ * shared memory).  No atomics: results are bit-identical from run to run.  Refusals as epnp_evaluate_backward_f32
+ * (S < 0, S * B above INT_MAX, no output) and t_lb / t_ub without bounds: EPNP_ERR_BAD_ARG.  B = 0 or S = 0 writes
+ * nothing.                                                                                                       */
+int epnp_evaluate_jvp_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                          const float* lb, const float* ub, const float* delta, const float* poses,
+                          const float* t_x3d, const float* t_x2d, const float* t_w2d, const float* t_delta,
+                          const float* t_pose, const float* t_cam, const float* t_lb, const float* t_ub,
+                          float* d_residual, float* d_jac, float* d_cost, int clip_jac, int S, int B, int N, int dof,
+                          float z_min, float huber_eps, void* stream);
+
 /* Backward of the derivative-regularisation branch: pose_opt_plus = pose (+) gn_step(pose) with the pose detached
  * (LMSolver.forward :66-68, gn_step :243-253, pose_add :255-265, evaluated with autograd on in the reference:
  * camera.py:119-129, cost_fun.py:52-84).  Given dL/d pose_opt_plus (B, D), writes dL/d x3d (B, N, 3), dL/d x2d
