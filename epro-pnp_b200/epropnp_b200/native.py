@@ -604,6 +604,8 @@ def evaluate_jvp(prob: Problem, poses, dof, z_min, huber_eps, clip_jac, tangents
     poses = _f32c(poses)
     new = (lambda *s: torch.zeros(s, dtype=torch.float32, device=prob.device)) if S == 0 else prob.empty
     out = [new(*s) if w else None for w, s in zip(want, ((S, B, 2 * N), (S, B, 2 * N, dof), (S, B)))]
+    if S == 0:                  # no pose, nothing to compute: an empty poses tensor has no pointer to pass
+        return tuple(out)
     with torch.cuda.device(prob.device):
         check(lib().epnp_evaluate_jvp_f32(*prob.common_ptrs(), ptr(poses), *(ptr(t) for t in tan),
                                           *(ptr(o) for o in out), int(clip_jac), S, B, N, int(dof),

@@ -520,7 +520,13 @@ def _register_autograd(op, backward, setup_context, jvp=None):
     but whose apply binds the arguments through inspect.signature on every call: host time the training step does not
     need to pay)."""
     op.register_autograd(backward, setup_context=setup_context)
-    impl = _IMPLS[op]
+    impl_direct = _IMPLS[op]
+
+    def impl(*args):
+        # under a torch-dispatch mode (make_fx, which torch.func.linearize traces with) the operator itself, which the
+        # mode records: the implementation's ctypes call is invisible to it, and its outputs would be traced as empty
+        # tensors that a replay of the graph leaves unwritten
+        return op(*args) if torch._C._len_torch_dispatch_stack() else impl_direct(*args)
 
     def setup(ctx, inputs, output):
         setup_context(ctx, inputs, output)

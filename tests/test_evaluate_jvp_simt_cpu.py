@@ -72,6 +72,34 @@ def test_forward_mode_through_evaluate_pnp(monkeypatch, mode):
     jv.assert_close(dict(zip(jv.OUTPUTS, got)), c, mode)
 
 
+@pytest.mark.parametrize("mode", ["jvp", "linearize"])
+def test_gn_step_under_torch_func(monkeypatch, mode):
+    """LMSolver.gn_step's tangent under torch.func.jvp and torch.func.linearize equals torch.autograd.forward_ad's.
+    linearize traces the step with make_fx and replays the graph, so every kernel call, the primal evaluation's
+    included, must be in that graph.  Fresh native output buffers are filled with NaN here: a call the trace missed
+    leaves them so in the replay."""
+    simt_native.install(monkeypatch)
+    from epropnp.camera import PerspectiveCamera
+    from epropnp.cost_fun import HuberPnPCost
+    from epropnp.levenberg_marquardt import LMSolver
+    from epropnp_b200 import native
+    monkeypatch.setattr(torch.Tensor, "is_cuda", property(lambda self: True))
+    monkeypatch.setattr(native.Problem, "empty",
+                        lambda self, *s: torch.full(s, float("nan"), dtype=torch.float32, device=self.device))
+    c = jv.build_case(6, 40, 1, 3, CPU, bounds=True)
+    solver = LMSolver(dof=6, num_iter=3)
+    names = ("x3d", "x2d", "w2d", "delta", "cam", "lb", "ub")
+    src = dict(x3d=c["x3d"], x2d=c["x2d"], w2d=c["w2d"], delta=c["delta"], cam=c["cam_mats"], lb=c["lb"], ub=c["ub"])
+
+    def f(x3d, x2d, w2d, delta, cam, lb, ub):
+        camera = PerspectiveCamera(cam_mats=cam, z_min=c["z_min"], lb=lb, ub=ub)
+        return (solver.gn_step(x3d, x2d, w2d, c["poses"][0], camera, HuberPnPCost(delta=delta)),)
+    run = lambda m: jv.forward_mode(f, [src[k] for k in names], [c["t"][k] for k in names], m)[0]
+    ref, got = run("fwad"), run(mode)
+    assert torch.isfinite(ref).all() and torch.isfinite(got).all(), mode
+    assert torch.allclose(got, ref, rtol=1e-5, atol=1e-6 * float(ref.abs().max())), mode
+
+
 def test_needs_derivative():
     import torch.autograd.forward_ad as fwAD
     from epropnp_b200 import ops
