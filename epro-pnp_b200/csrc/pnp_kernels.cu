@@ -5,6 +5,8 @@
 //                                    6x6 damped Cholesky + SE(3) retraction + trust region on lane 0, no block barrier.
 //   amis_kernel (pnp_amis.cuh)       the AMIS Monte-Carlo loop, ONE CTA per object: TMA ring -> packed pair records, one
 //                                    thread per sample, packed fp32x2 cost sweep, refits as block reductions; five CTAs per SM.
+//   lm_stacked_kernel (pnp_lm.cuh)   the same solve from S stacked starts per object: the hypotheses of one object share
+//                                    one staged copy of its points, H hypothesis warps per CTA, each warp lm_warp_kernel's body.
 //   epnp_lm_amis_fused_f32           = lm_warp_kernel, then amis_kernel, on the caller's stream (no host round trip); the
 //                                    split is what a measurement asked for: as one kernel the LM half ran latency-bound at
 //                                    4 points per thread between block barriers (DESIGN.md section 4).
@@ -2894,6 +2896,35 @@ int launch_lm(KArgs& a, cudaStream_t stream) {
     });
 }
 
+// Hypothesis warps per CTA of the staged stacked LM kernel for S starts: the CTAs of an object take equal shares of the
+// starts, at most LM_STACK_MAX_H each.  A function of S only (not B), like lm_warps_per_object of N.
+int lm_stack_h(int S) {
+    const int chunks = (S + LM_STACK_MAX_H - 1) / LM_STACK_MAX_H;
+    return (S + chunks - 1) / chunks;
+}
+
+template <int DOF, bool STAGED, int WARPS>
+int launch_lm_stacked_as(KArgs& a, int S, int H, cudaStream_t stream) {
+    const int chunks = (S + H - 1) / H;
+    const int smem_bytes = H * lm_head_bytes<DOF, WARPS>() + (STAGED ? 28 * lm_padded_points(a.N) : 0);
+    return launch_plain(lm_stacked_kernel<DOF, STAGED, WARPS>, a.B * chunks, 32 * WARPS * H, smem_bytes,
+                        STAGED ? SmemAttr::size_and_carveout : SmemAttr::none, stream, a, S, H);
+}
+
+// LM / GN solve of S stacked starts per object (a.pose_init (S, B, D), outputs in rows s B + b): the staged objects'
+// hypotheses share one staged copy of the points, H of them per CTA; the others run one start per CTA with
+// lm_warp_kernel's warp count and point order.  Either way each start's sums are those of launch_lm.
+int launch_lm_stacked(KArgs& a, int S, cudaStream_t stream) {
+    if (a.B == 0 || S == 0) return EPNP_OK;
+    const int rc = prepare_launch(a);
+    if (rc != EPNP_OK) return rc;
+    return by_dof(a.p.dof, [&](auto D) {
+        if (a.N <= LM_STAGE_MAX_N) return launch_lm_stacked_as<D, true, 1>(a, S, lm_stack_h(S), stream);
+        if (lm_warps_per_object(a.N) == 1) return launch_lm_stacked_as<D, false, 1>(a, S, 1, stream);
+        return launch_lm_stacked_as<D, false, 8>(a, S, 1, stream);
+    });
+}
+
 // The LM launch of the fused calls; its pose and covariance are the AMIS kernel's inputs.
 int launch_lm_for_amis(KArgs& a, cudaStream_t stream) {
     const int rc = launch_lm(a, stream);
@@ -3269,6 +3300,22 @@ int epnp_lm_solve_f32(const float* x3d, const float* x2d, const float* w2d, cons
     if (fast_mode_without_steps(*p) && (pose_cov || cost || cost_init)) return EPNP_ERR_BAD_ARG;
     a.cov_stride = p->dof * p->dof;
     return launch_lm(a, (cudaStream_t)stream);
+}
+
+int epnp_lm_solve_stacked_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                              const float* lb, const float* ub, const float* delta, const float* pose_init,
+                              float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus, float* cost_init,
+                              int S, int B, int N, const EpnpParams* p, void* stream) {
+    if (!p) return EPNP_ERR_BAD_ARG;
+    KArgs a = problem_args(x3d, x2d, w2d, cam_mats, lb, ub, delta, B, N);
+    a.pose_init = pose_init; a.pose_opt = pose_opt; a.pose_cov = pose_cov; a.cost = cost;
+    a.pose_plus = pose_opt_plus; a.cost_init = cost_init; a.p = *p;
+    const int rc = check_common(a);
+    if (rc != EPNP_OK) return rc;
+    if (!pose_init || !pose_opt || p->lm_iter < 0 || S < 0 || (long long)S * B > 2147483647LL) return EPNP_ERR_BAD_ARG;
+    if (fast_mode_without_steps(*p) && (pose_cov || cost || cost_init)) return EPNP_ERR_BAD_ARG;
+    a.cov_stride = p->dof * p->dof;
+    return launch_lm_stacked(a, S, (cudaStream_t)stream);
 }
 
 // The checked arguments of epnp_gn_plus_backward_f32 and its split form, or the refusal.

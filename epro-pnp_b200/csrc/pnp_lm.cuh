@@ -27,6 +27,7 @@ constexpr int LM_STAGE_MAX_N = 640;     // 28 N bytes of shared memory per warp:
                                         // that the K + 1 evaluations read shared memory instead of going back to L1 / L2
 
 constexpr int LM_MAX_WARPS = 8;
+constexpr int LM_STACK_MAX_H = 8;       // hypothesis warps per CTA of the staged stacked kernel
 template <int DOF, int WARPS> struct LmHead {
     uint64_t bar;
     float ev[32];                       // reduced evaluation: NV floats
@@ -48,11 +49,14 @@ template <int DOF, int WARPS> __host__ __device__ inline int lm_smem_bytes(int N
 // Normal equations at `pose` over the object's N points by the object's WARPS warps: result in ev[0..NV) (visible to
 // every thread of the group on return).  Jacobian rows u / v in the two lanes of fp32x2 registers (27 V2 multiply-adds
 // per point, two FFMA each on sm_90a).
+// `gt`: the thread's index within the group.  A group of several warps is its whole CTA (its barriers are
+// __syncthreads), so there the index is read as threadIdx.x, which keeps lm_warp_kernel's multi-warp code as it was.
 template <int DOF, bool CLIP, int WARPS>
 __device__ __forceinline__ void warp_normal_eq(const float* p3, const float* p2, const float* pw, int N, const float* pose,
-                                               const Cam& cam, float delta, float huber_eps, float* ev, float* part) {
+                                               const Cam& cam, float delta, float huber_eps, float* ev, float* part,
+                                               int gt) {
     constexpr int NP = Dim<DOF>::NA + DOF;
-    const int lane = threadIdx.x & 31;
+    const int lane = threadIdx.x & 31, tid = WARPS == 1 ? gt : (int)threadIdx.x;
     float R[9], t[3];
     {
         float ps[Dim<DOF>::POSE];
@@ -68,7 +72,7 @@ __device__ __forceinline__ void warp_normal_eq(const float* p3, const float* p2,
     float cost = 0.f;
     const float2* uv2 = reinterpret_cast<const float2*>(p2);
     const float2* w2 = reinterpret_cast<const float2*>(pw);
-    for (int n = threadIdx.x; n < N; n += 32 * WARPS) {
+    for (int n = tid; n < N; n += 32 * WARPS) {
         const float X = p3[3 * n], Y = p3[3 * n + 1], Z = p3[3 * n + 2];
         const float2 uv = uv2[n], w = w2[n];
         point_normal_eq_rows<DOF, CLIP>(R, t, cam, kuv, delta, huber_eps, X, Y, Z, -uv.x, -uv.y, w.x, w.y, acc2, cost);
@@ -96,13 +100,80 @@ __device__ __forceinline__ void warp_normal_eq(const float* p3, const float* p2,
     }
 }
 
+// The LM / GN solve of one start by one group of 32 WARPS threads, once the object's points p3 / p2 / pw are readable by
+// the group.  `obj` picks the camera and Huber scale, `row` the start and the output rows, `lane` is the thread's index
+// within the group.  Every sum runs in the same order whatever CTA the group belongs to.
+template <int DOF, int WARPS>
+__device__ __forceinline__ void lm_solve_group(const KArgs& a, LmHead<DOF, WARPS>& sh, const float* p3, const float* p2,
+                                               const float* pw, int obj, int row, int lane) {
+    constexpr int PD = Dim<DOF>::POSE;
+    const Params& p = a.p;
+    const int N = a.N;
+    const Cam cam = load_cam(a, obj);
+    const float delta = __ldg(a.delta + obj);
+    if (lane == 0) {
+#pragma unroll
+        for (int i = 0; i < PD; ++i) sh.lm.pose[i] = __ldg(a.pose_init + (size_t)row * PD + i);
+        sh.lm.radius = p.initial_radius;
+        sh.lm.shrink = 2.0f;
+    }
+    lm_group_sync<WARPS>();
+    if (!p.fast_mode) {
+        warp_normal_eq<DOF, true, WARPS>(p3, p2, pw, N, sh.lm.pose, cam, delta, p.huber_eps, sh.ev, sh.part, lane);
+        if (lane == 0) {
+            lm_adopt<DOF>(sh.lm, sh.ev);
+            if (a.cost_init) a.cost_init[row] = sh.lm.cost;
+            if (p.lm_iter > 0) lm_propose<DOF>(sh.lm, p);
+        }
+        lm_group_sync<WARPS>();
+        for (int it = 0; it < p.lm_iter; ++it) {
+            warp_normal_eq<DOF, true, WARPS>(p3, p2, pw, N, sh.lm.pose_new, cam, delta, p.huber_eps, sh.ev, sh.part, lane);
+            if (lane == 0) {
+                lm_update<DOF>(sh.lm, sh.ev, p);
+                if (it + 1 < p.lm_iter) lm_propose<DOF>(sh.lm, p);
+            }
+            lm_group_sync<WARPS>();
+        }
+    } else {
+        for (int it = 0; it < p.lm_iter; ++it) {
+            warp_normal_eq<DOF, false, WARPS>(p3, p2, pw, N, sh.lm.pose, cam, delta, p.huber_eps, sh.ev, sh.part, lane);
+            if (lane == 0) {
+                lm_adopt<DOF>(sh.lm, sh.ev);                 // kept for covariance / cost (pre-step)
+                if (it == 0 && a.cost_init) a.cost_init[row] = sh.lm.cost;
+                gn_advance<DOF>(sh.lm.pose, sh.ev, p.eps, sh.lm.pose);
+            }
+            lm_group_sync<WARPS>();
+        }
+    }
+    if (lane < PD) a.pose_opt[(size_t)row * PD + lane] = sh.lm.pose[lane];
+    if (lane == 8 && a.cost) a.cost[row] = sh.lm.cost;
+    if (a.pose_cov) {
+        if (lane < DOF) {                   // one covariance column per lane (fp64 Cholesky + one solve)
+            float col[DOF];
+            pose_covariance_column<DOF>(sh.lm.a, p.eps, lane, col);
+#pragma unroll
+            for (int i = 0; i < DOF; ++i) sh.cov[i * DOF + lane] = col[i];
+        }
+        lm_group_sync<WARPS>();
+        for (int i = lane; i < DOF * DOF; i += 32 * WARPS) a.pose_cov[(size_t)row * a.cov_stride + i] = sh.cov[i];
+    }
+    if (a.pose_plus) {      // y* (+) one undamped GN step, clip_jac always on (gn_step default)
+        lm_group_sync<WARPS>();
+        warp_normal_eq<DOF, true, WARPS>(p3, p2, pw, N, sh.lm.pose, cam, delta, p.huber_eps, sh.ev, sh.part, lane);
+        if (lane == 0) {
+            float plus[PD];
+            gn_advance<DOF>(sh.lm.pose, sh.ev, p.eps, plus);
+#pragma unroll
+            for (int i = 0; i < PD; ++i) a.pose_plus[(size_t)row * PD + i] = plus[i];
+        }
+    }
+}
+
 // One object per CTA of WARPS warps (blockDim.x = 32 WARPS, blockIdx.x = object).
 template <int DOF, bool STAGED, int WARPS>
 __global__ void __launch_bounds__(32 * WARPS) lm_warp_kernel(const KArgs a) {
     EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
     LmHead<DOF, WARPS>& sh = *reinterpret_cast<LmHead<DOF, WARPS>*>(smem_raw);
-    constexpr int PD = Dim<DOF>::POSE;
-    const Params& p = a.p;
     const int lane = threadIdx.x, obj = blockIdx.x, N = a.N;     // `lane`: index within the object's group of 32 WARPS threads
     const float *p3, *p2, *pw;
     if constexpr (STAGED) {
@@ -134,64 +205,48 @@ __global__ void __launch_bounds__(32 * WARPS) lm_warp_kernel(const KArgs a) {
         p2 = a.x2d + (size_t)obj * N * 2;
         pw = a.w2d + (size_t)obj * N * 2;
     }
-    const Cam cam = load_cam(a, obj);
-    const float delta = __ldg(a.delta + obj);
-    if (lane == 0) {
-#pragma unroll
-        for (int i = 0; i < PD; ++i) sh.lm.pose[i] = __ldg(a.pose_init + (size_t)obj * PD + i);
-        sh.lm.radius = p.initial_radius;
-        sh.lm.shrink = 2.0f;
-    }
-    lm_group_sync<WARPS>();
-    if (!p.fast_mode) {
-        warp_normal_eq<DOF, true, WARPS>(p3, p2, pw, N, sh.lm.pose, cam, delta, p.huber_eps, sh.ev, sh.part);
-        if (lane == 0) {
-            lm_adopt<DOF>(sh.lm, sh.ev);
-            if (a.cost_init) a.cost_init[obj] = sh.lm.cost;
-            if (p.lm_iter > 0) lm_propose<DOF>(sh.lm, p);
-        }
-        lm_group_sync<WARPS>();
-        for (int it = 0; it < p.lm_iter; ++it) {
-            warp_normal_eq<DOF, true, WARPS>(p3, p2, pw, N, sh.lm.pose_new, cam, delta, p.huber_eps, sh.ev, sh.part);
-            if (lane == 0) {
-                lm_update<DOF>(sh.lm, sh.ev, p);
-                if (it + 1 < p.lm_iter) lm_propose<DOF>(sh.lm, p);
+    lm_solve_group<DOF, WARPS>(a, sh, p3, p2, pw, obj, obj, lane);
+}
+
+// Stacked starts: pose_init (S, B, D), every start solved as lm_warp_kernel solves it alone, into row s B + b of the
+// outputs.  CTA c of object b (blockIdx.x = b * ceil(S / H) + c) runs starts c H .. c H + H - 1, one group of WARPS
+// warps each, with H = 1 when WARPS > 1 (blockDim.x = 32 WARPS H).  STAGED: the CTA copies the object's points into
+// shared memory once and its H hypothesis warps all read that copy -- one 28 N-byte copy and H heads per CTA instead of
+// H copies.  Groups past S only help stage.
+template <int DOF, bool STAGED, int WARPS>
+__global__ void __launch_bounds__(STAGED ? 32 * LM_STACK_MAX_H : 32 * WARPS) lm_stacked_kernel(const KArgs a, const int S,
+                                                                                               const int H) {
+    EPNP_DYN_SMEM(unsigned char, smem_raw, 128);
+    const int chunks = (S + H - 1) / H, obj = blockIdx.x / chunks, N = a.N;
+    const int group = threadIdx.x / (32 * WARPS), lane = threadIdx.x - 32 * WARPS * group;
+    const int s = (blockIdx.x - obj * chunks) * H + group;
+    LmHead<DOF, WARPS>& sh = *reinterpret_cast<LmHead<DOF, WARPS>*>(smem_raw + group * lm_head_bytes<DOF, WARPS>());
+    const float *p3 = a.x3d + (size_t)obj * N * 3, *p2 = a.x2d + (size_t)obj * N * 2, *pw = a.w2d + (size_t)obj * N * 2;
+    if constexpr (STAGED) {
+        float* st = reinterpret_cast<float*>(smem_raw + H * lm_head_bytes<DOF, WARPS>());
+        const int np = lm_padded_points(N);
+        float *s3 = st, *s2 = st + 3 * np, *sw = st + 5 * np;
+        uint64_t* bar = &reinterpret_cast<LmHead<DOF, WARPS>*>(smem_raw)->bar;
+        if (a.use_tma) {
+            if (threadIdx.x == 0) {
+                mbar_init(bar, 1);
+                fence_barrier_init();
+                mbar_expect_tx(bar, (uint32_t)N * 28u);
+                tma_load_1d(s3, p3, (uint32_t)N * 12u, bar);
+                tma_load_1d(s2, p2, (uint32_t)N * 8u, bar);
+                tma_load_1d(sw, pw, (uint32_t)N * 8u, bar);
             }
-            lm_group_sync<WARPS>();
+            __syncthreads();
+            mbar_wait(bar, 0u);
+        } else {
+            for (int i = threadIdx.x; i < 3 * N; i += blockDim.x) s3[i] = __ldg(p3 + i);
+            for (int i = threadIdx.x; i < 2 * N; i += blockDim.x) { s2[i] = __ldg(p2 + i); sw[i] = __ldg(pw + i); }
+            __syncthreads();
         }
-    } else {
-        for (int it = 0; it < p.lm_iter; ++it) {
-            warp_normal_eq<DOF, false, WARPS>(p3, p2, pw, N, sh.lm.pose, cam, delta, p.huber_eps, sh.ev, sh.part);
-            if (lane == 0) {
-                lm_adopt<DOF>(sh.lm, sh.ev);                 // kept for covariance / cost (pre-step)
-                if (it == 0 && a.cost_init) a.cost_init[obj] = sh.lm.cost;
-                gn_advance<DOF>(sh.lm.pose, sh.ev, p.eps, sh.lm.pose);
-            }
-            lm_group_sync<WARPS>();
-        }
+        p3 = s3; p2 = s2; pw = sw;
     }
-    if (lane < PD) a.pose_opt[(size_t)obj * PD + lane] = sh.lm.pose[lane];
-    if (lane == 8 && a.cost) a.cost[obj] = sh.lm.cost;
-    if (a.pose_cov) {
-        if (lane < DOF) {                   // one covariance column per lane (fp64 Cholesky + one solve)
-            float col[DOF];
-            pose_covariance_column<DOF>(sh.lm.a, p.eps, lane, col);
-#pragma unroll
-            for (int i = 0; i < DOF; ++i) sh.cov[i * DOF + lane] = col[i];
-        }
-        lm_group_sync<WARPS>();
-        for (int i = lane; i < DOF * DOF; i += 32 * WARPS) a.pose_cov[(size_t)obj * a.cov_stride + i] = sh.cov[i];
-    }
-    if (a.pose_plus) {      // y* (+) one undamped GN step, clip_jac always on (gn_step default)
-        lm_group_sync<WARPS>();
-        warp_normal_eq<DOF, true, WARPS>(p3, p2, pw, N, sh.lm.pose, cam, delta, p.huber_eps, sh.ev, sh.part);
-        if (lane == 0) {
-            float plus[PD];
-            gn_advance<DOF>(sh.lm.pose, sh.ev, p.eps, plus);
-#pragma unroll
-            for (int i = 0; i < PD; ++i) a.pose_plus[(size_t)obj * PD + i] = plus[i];
-        }
-    }
+    if (s >= S) return;
+    lm_solve_group<DOF, WARPS>(a, sh, p3, p2, pw, obj, s * a.B + obj, lane);
 }
 
 // ------------------------------------------------------------------------------------------------

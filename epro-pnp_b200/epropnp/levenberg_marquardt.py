@@ -5,6 +5,8 @@ What runs where:
   * the K-iteration Levenberg-Marquardt (or Gauss-Newton `fast_mode`) loop, the pose covariance and
     the optional extra GN step are ONE kernel launch (epnp_lm_solve_f32): no per-iteration launches,
     no host round trips, no materialised (B, 2N, 6) Jacobian;
+  * stacked starts, pose_init (*, B, D): one launch of epnp_lm_solve_stacked_f32, each start solved as the (B, D) call
+    solves it, the hypotheses of an object sharing one staged copy of its points;
   * RSLMSolver: two launches -- the random subsets / start orientations (epnp_rslm_draw_f32), then refining and
     scoring all P hypotheses of every object (epnp_rslm_f32); with cluster_split=True, objects too large for one SM
     take epnp_rslm_split_f32 instead (refine, score on a thread-block cluster, select: three launches).
@@ -77,6 +79,9 @@ class LMSolver(nn.Module):
         delta = getattr(cost_fun, "delta", None)
         differentiable = with_pose_opt_plus and _needs_grad(x3d, x2d, w2d, delta, camera.cam_mats, camera.lb,
                                                             camera.ub)
+        if differentiable and pose_init is not None and pose_init.dim() > 2:
+            raise ValueError("with_pose_opt_plus from stacked starts (pose_init (*, B, D)) is not differentiable: "
+                             "detach the problem, or solve each start as a (B, D) call")
         pose_opt, pose_cov, cost, pose_opt_plus = self._solve_impl(
             x3d, x2d, w2d, camera, cost_fun, pose_init=pose_init,
             with_pose_opt_plus=with_pose_opt_plus and not differentiable, **kwargs)
@@ -93,7 +98,11 @@ class LMSolver(nn.Module):
 
     def solve(self, x3d, x2d, w2d, camera, cost_fun, pose_init=None, cost_init=None,
               with_pose_cov=False, with_cost=False, force_init_solve=False, fast_mode=False):
-        """-> pose_opt (B, 4|7), pose_cov (B, dof, dof) | None, cost (B) | None."""
+        """-> pose_opt (B, 4|7), pose_cov (B, dof, dof) | None, cost (B) | None.
+
+        pose_init may stack several starts per object, (*, B, D): each is refined exactly as a (B, D) call would refine
+        it, all in one launch, and the outputs get the same leading dimensions, (*, B, D), (*, B, dof, dof) and
+        (*, B).  force_init_solve is refused with stacked starts."""
         return self._solve_impl(x3d, x2d, w2d, camera, cost_fun, pose_init=pose_init, cost_init=cost_init,
                                 with_pose_cov=with_pose_cov, with_cost=with_cost,
                                 force_init_solve=force_init_solve, fast_mode=fast_mode)[:3]
@@ -116,6 +125,9 @@ class LMSolver(nn.Module):
     @torch.no_grad()
     def _solve_impl(self, x3d, x2d, w2d, camera, cost_fun, pose_init=None, cost_init=None, with_pose_cov=False,
                     with_cost=False, force_init_solve=False, fast_mode=False, with_pose_opt_plus=False):
+        if pose_init is not None and pose_init.dim() > 2:
+            return self._solve_stacked(x3d, x2d, w2d, camera, cost_fun, pose_init, with_pose_cov, with_cost,
+                                       force_init_solve, fast_mode, with_pose_opt_plus)
         num_obj = x2d.size(0)
         kw = dict(dtype=x2d.dtype, device=x2d.device)
         if num_obj == 0:
@@ -129,6 +141,24 @@ class LMSolver(nn.Module):
         cast = lambda t, want: t.to(x2d.dtype) if want else None
         return (cast(out[0], True), cast(out[1], with_pose_cov), cast(out[2], with_cost),
                 cast(out[3], with_pose_opt_plus))
+
+    def _solve_stacked(self, x3d, x2d, w2d, camera, cost_fun, pose_init, with_pose_cov, with_cost, force_init_solve,
+                       fast_mode, with_pose_opt_plus):
+        """_solve_impl from stacked starts pose_init (*, B, D): one epnp_lm_solve_stacked_f32 launch, where the objects'
+        hypotheses share each staged copy of the points."""
+        if force_init_solve:
+            raise ValueError("force_init_solve=True takes a (B, D) pose_init: with stacked starts it is ambiguous which "
+                             "start the init solver's pose would replace")
+        B, D = x2d.size(0), self._pose_dim()
+        if tuple(pose_init.shape[-2:]) != (B, D):
+            raise ValueError(f"stacked pose_init must be (*, {B}, {D}); got {tuple(pose_init.shape)}")
+        lead = tuple(pose_init.shape[:-2]) + (B,)
+        out = ops.lm_solve_stacked(*_problem_args(x3d, x2d, w2d, camera, cost_fun),
+                                   pose_init.detach().flatten(0, -3), *self.param_lists(camera, cost_fun, fast_mode),
+                                   with_pose_cov, with_cost, with_pose_opt_plus)
+        shaped = lambda t, want, *tail: t.reshape(lead + tail).to(x2d.dtype) if want else None
+        return (shaped(out[0], True, D), shaped(out[1], with_pose_cov, self.dof, self.dof), shaped(out[2], with_cost),
+                shaped(out[3], with_pose_opt_plus, D))
 
     def gn_step(self, x3d, x2d, w2d, pose, camera, cost_fun):
         """Undamped Gauss-Newton increment -(J^T J + eps I)^-1 J^T r at `pose` (levenberg_marquardt.py:243-253)."""

@@ -59,6 +59,7 @@ _SIGNATURES = {
     "epnp_evaluate_backward_f32": (ctypes.c_int, [_P] * 19 + [_I, _I, _I, _I, _I, _F, _F, _P]),
     "epnp_evaluate_jvp_f32": (ctypes.c_int, [_P] * 19 + [_I, _I, _I, _I, _I, _F, _F, _P]),
     "epnp_lm_solve_f32": (ctypes.c_int, [_P] * 13 + [_I, _I, ctypes.POINTER(EpnpParams), _P]),
+    "epnp_lm_solve_stacked_f32": (ctypes.c_int, [_P] * 13 + [_I, _I, _I, ctypes.POINTER(EpnpParams), _P]),
     "epnp_gn_plus_backward_f32": (ctypes.c_int, [_P] * 13 + [_I, _I, _I, _F, _F, _F, _P]),
     "epnp_gn_plus_backward_split_f32": (ctypes.c_int, [_P] * 13 + [_I, _I, _I, _F, _F, _F, _I, _P]),
     "epnp_rslm_draw_f32": (ctypes.c_int, [_P] * 5 + [ctypes.c_uint64, ctypes.c_uint32, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),

@@ -210,6 +210,35 @@ def lm_solve(prob: Problem, pose_init, params, want_cov=False, want_cost=False, 
     return out
 
 
+def lm_solve_stacked(prob: Problem, pose_init, params, want_cov=False, want_cost=False, want_plus=False,
+                     want_cost_init=False):
+    """lm_solve from S stacked starts per object (epnp_lm_solve_stacked_f32): pose_init (S, B, D) -> dict(pose_opt
+    (S, B, D), pose_cov (S, B, dof, dof), cost (S, B), pose_opt_plus (S, B, D), cost_init (S, B)), None where not
+    wanted.  Start s of object b gives what lm_solve gives with pose_init = pose_init[s], bit for bit."""
+    D = 7 if params.dof == 6 else 4
+    B = prob.B
+    if pose_init is None:
+        raise ValueError("lm_solve_stacked needs pose_init (S, B, D): there is no initialiser for stacked starts")
+    if pose_init.dim() != 3:
+        raise ValueError(f"pose_init must be (S, {B}, {D}); got {tuple(pose_init.shape)}")
+    S = pose_init.shape[0]
+    _check_pose(pose_init, (S, B), D, "pose_init")
+    pose_init = _f32c(pose_init)
+    out = dict(pose_opt=prob.empty(S, B, D),
+               pose_cov=prob.empty(S, B, params.dof, params.dof) if want_cov else None,
+               cost=prob.empty(S, B) if want_cost else None,
+               pose_opt_plus=prob.empty(S, B, D) if want_plus else None,
+               cost_init=prob.empty(S, B) if want_cost_init else None)
+    if S == 0 or B == 0:        # empty tensors have no storage; the call would write nothing
+        return out
+    with torch.cuda.device(prob.device):
+        check(lib().epnp_lm_solve_stacked_f32(*prob.common_ptrs(), ptr(pose_init), ptr(out["pose_opt"]),
+                                              ptr(out["pose_cov"]), ptr(out["cost"]), ptr(out["pose_opt_plus"]),
+                                              ptr(out["cost_init"]), S, B, prob.N, ctypes.byref(params),
+                                              stream_ptr(prob.device)), "epnp_lm_solve_stacked_f32")
+    return out
+
+
 def rslm_draw(x3d, x2d, w2d, cam_mats, P, n, dof, eps=1e-5, seed=0, obj_offset=0, t_init=None, want_t=False):
     """Everything before the solves of the random-sample initialiser in one launch (epnp_rslm_draw_f32): the
     centre-based translation guess (unless t_init (B, 3) is given -- then x3d / x2d / cam_mats may be None), inds
@@ -898,5 +927,5 @@ def mc_lse_backward(logw_bm, lse, grad_lse):
 
 
 __all__ = ["Problem", "adaptive_delta", "cost_backward", "cost_camera_backward", "gn_plus_camera_backward",
-           "evaluate_cost", "evaluate_cost_split", "evaluate_full", "evaluate_backward", "lm_solve",
+           "evaluate_cost", "evaluate_cost_split", "evaluate_full", "evaluate_backward", "lm_solve", "lm_solve_stacked",
            "amis", "lm_amis_fused", "lm_amis_fused_split", "max_points", "max_points_split", "split_ctas", "lm_amis_fused_host", "lm_amis_fused_push", "lm_amis_fused_split_host", "lm_amis_fused_split_push", "fused_workspace_bytes", "solve_host", "solve_split_host", "solve_workspace_bytes", "rslm_spec", "epnp_spec", "initial_pose", "rslm", "rslm_split", "epnp_init", "epnp_init_split", "gn_plus_backward", "gn_plus_backward_split", "evaluate_jvp", "cost_hvp", "gn_plus_hvp", "mc_epilogue", "mc_lse_backward", "default_params", "NativeError", "capi"]

@@ -17,6 +17,7 @@ mc_epilogue, and for second order on the cost backwards (cost_backward, cost_pos
 Hessian-vector product cost_hvp), on the pose_opt_plus backwards (gn_plus_backward, gn_plus_camera_backward: the
 Hessian-vector product gn_plus_hvp) and on mc_lse_backward.  cost_hvp and gn_plus_hvp have none, so a third derivative
 raises.  evaluate_full's residual / Jacobian are first-order only: a second backward through evaluate_backward raises.
+lm_solve_stacked (the solve from stacked starts) has no differentiable output.
 
 Forward mode (torch.autograd.forward_ad, torch.func.jvp and linearize) runs eagerly through the jvp formulas of the eager Functions of
 evaluate_cost, evaluate_full (the kernel evaluate_jvp), lm_amis_fused (logw and cost_init), lm_solve (pose_opt_plus,
@@ -28,7 +29,7 @@ backward and Hessian operators) and reverse through evaluate_jvp are not support
 
 The module's names (adaptive_delta, ..., mc_lse_backward) are the entry points the layer calls (_entry): the operator
 while anything traces, its implementation directly in eager code.  The operators themselves are FORWARD / BACKWARD /
-SECOND_ORDER / FORWARD_MODE and torch.ops.epropnp.*; each entry point's `.op` is its operator.
+SECOND_ORDER / FORWARD_MODE / STACKED and torch.ops.epropnp.*; each entry point's `.op` is its operator.
 """
 from typing import List, Optional
 
@@ -217,6 +218,28 @@ def _(x3d, x2d, w2d, cam_mats, lb, ub, delta, pose_init, ints, floats, want_cov,
     D = _pose_dim(dof)
     return (new(B, D), new(B, dof, dof) if want_cov else new(0), new(B) if want_cost else new(0),
             new(B, D) if want_plus else new(0))
+
+
+@_op("lm_solve_stacked")
+def lm_solve_stacked(x3d: Tensor, x2d: Tensor, w2d: Tensor, cam_mats: Tensor, lb: Optional[Tensor],
+                     ub: Optional[Tensor], delta: Tensor, pose_init: Tensor, ints: List[int], floats: List[float],
+                     want_cov: bool, want_cost: bool, want_plus: bool) -> tuple[Tensor, Tensor, Tensor, Tensor]:
+    """lm_solve from stacked starts pose_init (S, B, D) -> pose_opt (S, B, D), pose_cov (S, B, dof, dof), cost (S, B),
+    pose_opt_plus (S, B, D); start s of object b as lm_solve solves it with pose_init[s].  No output is
+    differentiable."""
+    prob = _problem(x3d, x2d, w2d, cam_mats, lb, ub, delta)
+    out = native.lm_solve_stacked(prob, pose_init, make_params(ints, floats), want_cov=want_cov, want_cost=want_cost,
+                                  want_plus=want_plus)
+    return tuple(_or_empty(out[k], x3d) for k in ("pose_opt", "pose_cov", "cost", "pose_opt_plus"))
+
+
+@lm_solve_stacked.register_fake
+def _(x3d, x2d, w2d, cam_mats, lb, ub, delta, pose_init, ints, floats, want_cov, want_cost, want_plus):
+    S, B, dof = pose_init.shape[0], x3d.shape[0], ints[0]
+    new = lambda *s: x3d.new_empty(s, dtype=torch.float32)
+    D = _pose_dim(dof)
+    return (new(S, B, D), new(S, B, dof, dof) if want_cov else new(0), new(S, B) if want_cost else new(0),
+            new(S, B, D) if want_plus else new(0))
 
 
 @_op("lm_amis_fused")
@@ -816,6 +839,17 @@ def _lm_solve_jvp(ctx, inputs, output, tangents):
 _register_autograd(lm_solve, _lm_solve_backward, _lm_solve_setup, _lm_solve_jvp)
 
 
+def _lm_solve_stacked_setup(ctx, inputs, output):
+    ctx.mark_non_differentiable(*output)
+
+
+def _lm_solve_stacked_backward(ctx, *grads):
+    return (None,) * 13
+
+
+_register_autograd(lm_solve_stacked, _lm_solve_stacked_backward, _lm_solve_stacked_setup)
+
+
 def _mc_epilogue_setup(ctx, inputs, output):
     ctx.mark_non_differentiable(*output[1:])
     ctx.save_for_backward(inputs[0], output[0])
@@ -955,9 +989,10 @@ BACKWARD = (cost_backward, cost_pose_backward, cost_camera_backward, gn_plus_bac
             evaluate_backward, mc_lse_backward)
 SECOND_ORDER = (cost_hvp, gn_plus_hvp)
 FORWARD_MODE = (evaluate_jvp,)
-# operators whose outputs the layer never differentiates (the solver's start): under forward AD their inputs' tangents
-# are dropped, as reverse mode's no_grad drops the graph
-_NO_DERIVATIVE = (rslm_draw, rslm, epnp_init)
+STACKED = (lm_solve_stacked,)                       # the solve from stacked starts, pose_init (S, B, D)
+# operators whose outputs the layer never differentiates (the solver's start, the stacked solve): under forward AD their
+# inputs' tangents are dropped, as reverse mode's no_grad drops the graph
+_NO_DERIVATIVE = (rslm_draw, rslm, epnp_init, lm_solve_stacked)
 
 
 @torch.compiler.disable
@@ -1056,3 +1091,4 @@ def _entry(op):
  mc_lse_backward) = (_entry(op) for op in BACKWARD)
 cost_hvp, gn_plus_hvp = (_entry(op) for op in SECOND_ORDER)
 evaluate_jvp = _entry(evaluate_jvp)
+lm_solve_stacked = _entry(lm_solve_stacked)

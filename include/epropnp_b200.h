@@ -274,6 +274,19 @@ int epnp_lm_solve_f32(const float* x3d, const float* x2d, const float* w2d, cons
                       float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus,
                       float* cost_init, int B, int N, const EpnpParams* p, void* stream);
 
+/* epnp_lm_solve_f32 from S stacked starts per object (the yaw ambiguity, top-k hypotheses, symmetric objects, a grid of
+ * starts): pose_init (S, B, D); start s of object b is solved exactly as epnp_lm_solve_f32 solves it with pose_init =
+ * its row s, bit for bit, into row (s, b) of every output:
+ *   pose_opt (S, B, D); pose_cov [opt] (S, B, dof, dof); cost [opt] (S, B); pose_opt_plus [opt] (S, B, D);
+ *   cost_init [opt] (S, B)
+ * Objects of up to 640 points stage their correspondences into shared memory once per CTA and up to 8 hypothesis warps
+ * of the CTA share that copy; longer objects run one start per CTA from global memory.  Refusals, before any launch:
+ * epnp_lm_solve_f32's, and S < 0 or S * B above INT_MAX (EPNP_ERR_BAD_ARG).  B = 0 or S = 0 writes nothing.        */
+int epnp_lm_solve_stacked_f32(const float* x3d, const float* x2d, const float* w2d, const float* cam_mats,
+                              const float* lb, const float* ub, const float* delta, const float* pose_init,
+                              float* pose_opt, float* pose_cov, float* cost, float* pose_opt_plus,
+                              float* cost_init, int S, int B, int N, const EpnpParams* p, void* stream);
+
 /* The AMIS loop of EProPnPBase.monte_carlo_forward (epropnp.py:132-182) for EProPnP6DoF
  * (initial_fit :288-302, gen_new/old_distr :304-315, estimate_params :317-342; proposals from
  * distributions.py:15-52 and pyro MultivariateStudentT), starting from a given local solution.
